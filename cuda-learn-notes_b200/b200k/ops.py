@@ -186,6 +186,38 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
                                        1 if causal else 0, sl, variant, _stream(q)))
 
 
+def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
+                   scale: Optional[float] = None, causal: bool = False) -> None:
+    """FA-2 forward on packed variable-length sequences (the forward of flash-attn's ``flash_attn_varlen_func``).
+    q, o [total_q, H, D]; k, v [total_k, H_kv, D] with H % H_kv == 0 (query head h reads K/V head h // (H // H_kv));
+    fp16 or bf16.  ``cu_seqlens_q`` / ``cu_seqlens_k``: int32 [B + 1] cumulative token offsets on the device.
+    ``max_seqlen_q`` (a Python int, >= every query length) sizes the grid, so nothing is read back to the host.
+    ``causal`` is aligned bottom-right (row r sees keys <= r + Lk - Lq); rows that see no key are 0."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    for t in (q, k, v, o):
+        _check_dtype(t, dt)
+    if q.dim() != 3 or k.dim() != 3:
+        raise RuntimeError("Tensor size mismatch!")
+    total_q, H, D = q.shape
+    total_k, H_kv = k.size(0), k.size(1)
+    if tuple(k.shape) != (total_k, H_kv, D) or tuple(v.shape) != tuple(k.shape) or tuple(o.shape) != tuple(q.shape):
+        raise RuntimeError("Tensor size mismatch!")
+    if H_kv < 1 or H % H_kv:
+        raise RuntimeError("Tensor size mismatch!")
+    if D not in FA2_HEADDIMS:
+        raise RuntimeError("headdim not support!")
+    _check_dtype(cu_seqlens_q, torch.int32)
+    _check_dtype(cu_seqlens_k, torch.int32)
+    B = cu_seqlens_q.numel() - 1
+    if B < 1 or cu_seqlens_k.numel() != B + 1:
+        raise RuntimeError("Tensor size mismatch!")
+    _check_cuda_contig(q, k, v, o, cu_seqlens_q, cu_seqlens_k)
+    with _DeviceGuard(q):
+        L.check(_lib.b200k_fa2_fwd_varlen(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), cu_seqlens_q.data_ptr(),
+                                          cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
+                                          float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+
+
 def ffpa_fwd(q, k, v, o, scale: Optional[float] = None, variant: int = 0) -> None:
     B, H, N, D = _check_qkvo(q, k, v, o)
     with _DeviceGuard(q):

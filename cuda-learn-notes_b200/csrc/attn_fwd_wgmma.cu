@@ -12,6 +12,8 @@
 // Head dims above 256 split O into ceil(D / 256) column slices, one per CTA (grid.y); each slice recomputes S.
 // Ragged N and head dims that are not multiples of 64 are zero-filled by TMA (3-D maps: per head) and clipped on the
 // store; padded keys are masked.  Causal CTAs stop at their diagonal tile.
+// Packed variable-length sequences with grouped K/V heads (AttnCfg::VARLEN) run the same main loop; only the tensor
+// maps, the TMA coordinates, the per-CTA key length, the causal diagonal and the epilogue's addressing differ.
 #include "abi_common.cuh"
 #include "ptx.cuh"
 
@@ -25,10 +27,19 @@ struct AttnMask {
   int causal = 0;
 };
 
-template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_>  // DT: 0 f16, 1 bf16
+// Packed sequences (Cfg::VARLEN): sequence b is tokens [cu_q[b], cu_q[b+1]) of Q / O ([total_q, H, D]) and
+// [cu_k[b], cu_k[b+1]) of K / V ([total_k, H / group, D]); query head h reads K / V head h / group.
+struct AttnVarlen {
+  const int* cu_q = nullptr;
+  const int* cu_k = nullptr;
+  int group = 1;
+  int total_q = 0;
+};
+
+template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_, bool VARLEN_ = false>  // DT: 0 f16, 1 bf16
 struct AttnCfg {
   static constexpr int DT = DT_, DV = DV_, NWG = NWG_, BN = BN_;
-  static constexpr bool V_DN = V_DN_;
+  static constexpr bool V_DN = V_DN_, VARLEN = VARLEN_;
   static constexpr int BM = 64 * NWG;
   static constexpr int THREADS = 128 * (NWG + 1);
   static constexpr int KSTAGES = 4, VSTAGES = 2;
@@ -88,10 +99,17 @@ __device__ __forceinline__ uint32_t pack_round(float& lo, float& hi) {
   }
 }
 
+// KV tiles a CTA visits.  q0 is the diagonal of its first row: the key index that row sees last under the causal mask
+// (the row itself, or row + Lk - Lq for packed sequences, which can be negative: no key visible).
 template <class Cfg>
 __device__ __forceinline__ int attn_num_tiles(int q0, int kv_len, const AttnMask& mask) {
   int nt = (kv_len + Cfg::BN - 1) / Cfg::BN;
-  if (mask.causal) nt = min(nt, (q0 + Cfg::BM - 1) / Cfg::BN + 1);
+  if constexpr (Cfg::VARLEN) {
+    const int last = q0 + Cfg::BM - 1;
+    if (mask.causal) nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
+  } else {
+    if (mask.causal) nt = min(nt, (q0 + Cfg::BM - 1) / Cfg::BN + 1);
+  }
   return nt;
 }
 
@@ -99,8 +117,9 @@ template <class Cfg>
 __global__ void __launch_bounds__(Cfg::THREADS, 1)
     attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, void* O, int N, int D, int nqc, float scale_log2,
-                          const AttnMask mask) {
+                          const AttnMask mask, const AttnVarlen vl) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DV = Cfg::DV, KST = Cfg::KSTAGES, VST = Cfg::VSTAGES;
+  static_assert(!(Cfg::VARLEN && Cfg::V_DN), "packed sequences take V as [tokens, heads, D]");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u;
   const uint32_t sK = sQ + nqc * BM * 128, sV = sK + KST * Cfg::K_BYTES;
@@ -109,8 +128,20 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   const int bh = blockIdx.z, q0 = blockIdx.x * BM, dv0 = blockIdx.y * DV;
   int kv_len = N;
-  if (mask.seqlens) kv_len = min(max(__ldg(mask.seqlens + bh / mask.H), 1), N);
-  const int ntiles = attn_num_tiles<Cfg>(q0, kv_len, mask);
+  // packed sequences: first query and key token of the sequence, and the causal shift Lk - Lq (row r sees keys <= r + shift)
+  int q_tok = 0, k_tok = 0, shift = 0;
+  if constexpr (Cfg::VARLEN) {
+    const int b = bh / mask.H;
+    q_tok = __ldg(vl.cu_q + b);
+    const int q_len = __ldg(vl.cu_q + b + 1) - q_tok;
+    if (q0 >= q_len) return;  // no rows of this sequence here; no barrier is initialised yet
+    k_tok = __ldg(vl.cu_k + b);
+    kv_len = __ldg(vl.cu_k + b + 1) - k_tok;
+    shift = kv_len - q_len;
+  } else {
+    if (mask.seqlens) kv_len = min(max(__ldg(mask.seqlens + bh / mask.H), 1), N);
+  }
+  const int ntiles = attn_num_tiles<Cfg>(q0 + shift, kv_len, mask);
   const int wg = threadIdx.x / 128;
 
   if (threadIdx.x == 0) {
@@ -129,15 +160,23 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   if (wg == 0) {
     if (threadIdx.x == 0) {
+      // packed maps are (D, heads, tokens): coordinates (column, head, token) instead of (column, row, batch * head)
+      const int head = bh % mask.H, kv_head = head / vl.group;
       mbar_arrive_expect_tx(qbar, nqc * BM * 128);
-      for (int c = 0; c < nqc; ++c) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, q0, bh, kPolicyEvictFirst);
+      for (int c = 0; c < nqc; ++c) {
+        if constexpr (Cfg::VARLEN) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, head, q_tok + q0, kPolicyEvictFirst);
+        else tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, q0, bh, kPolicyEvictFirst);
+      }
       int kc = 0;
       for (int j = 0; j < ntiles; ++j) {
         for (int c = 0; c < nqc; ++c, ++kc) {
           const int s = kc % KST;
           if (kc >= KST) mbar_wait(kempty + 8 * s, ((kc / KST) - 1) & 1);
           mbar_arrive_expect_tx(kfull + 8 * s, Cfg::K_BYTES);
-          tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, j * BN, bh, kPolicyEvictNormal);
+          if constexpr (Cfg::VARLEN)
+            tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
+          else
+            tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, j * BN, bh, kPolicyEvictNormal);
         }
         const int s = j % VST;
         if (j >= VST) mbar_wait(vempty + 8 * s, ((j / VST) - 1) & 1);
@@ -149,8 +188,12 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
             tma_load_3d(dst + c * DV * 128, &tmV, vfull + 8 * s, j * BN + c * 64, dv0, bh, kPolicyEvictNormal);
         } else {
 #pragma unroll
-          for (int c = 0; c < DV / 64; ++c)
-            tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, j * BN, bh, kPolicyEvictNormal);
+          for (int c = 0; c < DV / 64; ++c) {
+            if constexpr (Cfg::VARLEN)
+              tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
+            else
+              tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, j * BN, bh, kPolicyEvictNormal);
+          }
         }
       }
     }
@@ -192,9 +235,10 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     fence_regs<BN / 2>(s_acc);
     if (leader) mbar_arrive(kempty + 8 * ((kc - 1) % KST));
 
-    // ---- masks: keys past the valid length, keys after the query row (causal)
+    // ---- masks: keys past the valid length, keys after the query row + shift (causal).  The shift is selected at
+    // compile time rather than added as 0, which keeps the dense instantiations' machine code as it was.
     const int k0 = j * BN;
-    if (k0 + BN > kv_len || (mask.causal && k0 + BN - 1 > q0 + cw * 64)) {
+    if (k0 + BN > kv_len || (mask.causal && k0 + BN - 1 > (Cfg::VARLEN ? q0 + shift : q0) + cw * 64)) {
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i)
 #pragma unroll
@@ -202,7 +246,8 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int key = k0 + 8 * i + 2 * (lane & 3) + e;
-            if (key >= kv_len || (mask.causal && key > row0 + 8 * h)) s_acc[4 * i + 2 * h + e] = -INFINITY;
+            if (key >= kv_len || (mask.causal && key > (Cfg::VARLEN ? row0 + shift : row0) + 8 * h))
+              s_acc[4 * i + 2 * h + e] = -INFINITY;
           }
     }
 
@@ -261,7 +306,14 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     if (leader) mbar_arrive(vempty + 8 * sv);
   }
 
-  // ---- epilogue: O / l, clipped to N rows and D columns
+  // ---- epilogue: O / l, clipped to N rows (packed: the sequence's rows and tokens [0, total_q)) and D columns.  Rows
+  // that saw no key have l = 0 and store 0.
+  int q_len = N;
+  if constexpr (Cfg::VARLEN) {  // reloaded rather than kept in registers through the main loop
+    const int b = bh / mask.H;
+    q_tok = vl.cu_q[b];
+    q_len = vl.cu_q[b + 1] - q_tok;
+  }
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float t = l[h];
@@ -269,8 +321,15 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     t += __shfl_xor_sync(0xffffffffu, t, 2);
     const float inv = t > 0.f ? 1.f / t : 0.f;
     const int r = row0 + 8 * h;
-    if (r >= N) continue;
-    const size_t row_off = (size_t(bh) * N + r) * size_t(D);
+    if (r >= q_len) continue;
+    size_t row_off;
+    if constexpr (Cfg::VARLEN) {
+      const long long tok = (long long)q_tok + r;
+      if (tok < 0 || tok >= vl.total_q) continue;
+      row_off = (size_t(tok) * mask.H + bh % mask.H) * size_t(D);
+    } else {
+      row_off = (size_t(bh) * N + r) * size_t(D);
+    }
 #pragma unroll
     for (int i = 0; i < DV / 8; ++i) {
       const int c = dv0 + 8 * i + 2 * (lane & 3);
@@ -300,7 +359,40 @@ static int launch_attn(const void* Q, const void* K, const void* V, void* O, int
   auto kern = attn_fwd_wgmma_kernel<Cfg>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
   dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask);
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask,
+                                        AttnVarlen());
+  B200K_CHECK_CUDA(cudaGetLastError());
+  return B200K_OK;
+}
+
+// Packed sequences: one 3-D map per tensor over (D, heads, tokens), box (64, 1, BM or BN), so shared memory holds the
+// same 128-byte swizzled rows as the dense maps and only the coordinates differ.  Grid: ceil(max_seqlen_q / BM) query
+// tiles x B * H; CTAs past their sequence's length return at once.
+template <class Cfg>
+static int launch_attn_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_q, const int* cu_k,
+                              int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv,
+                              int64_t D, float scale, int causal, cudaStream_t s, const DeviceInfo& di) {
+  const int nqc = int((D + 63) / 64);
+  const int smem = Cfg::smem_bytes(nqc);
+  if (smem > di.max_smem_optin)
+    return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  if ((rc = make_tmap_3d_u16(&tmQ, Q, total_q, H, D, uint64_t(H) * D, D, Cfg::BM, 1, 64, 128))) return rc;
+  if ((rc = make_tmap_3d_u16(&tmK, K, total_k, H_kv, D, uint64_t(H_kv) * D, D, Cfg::BN, 1, 64, 128))) return rc;
+  if ((rc = make_tmap_3d_u16(&tmV, V, total_k, H_kv, D, uint64_t(H_kv) * D, D, Cfg::BN, 1, 64, 128))) return rc;
+  auto kern = attn_fwd_wgmma_kernel<Cfg>;
+  if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
+  AttnMask mask;
+  mask.H = int(H);
+  mask.causal = causal ? 1 : 0;
+  AttnVarlen vl;
+  vl.cu_q = cu_q;
+  vl.cu_k = cu_k;
+  vl.group = int(H / H_kv);
+  vl.total_q = int(total_q);
+  dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask, vl);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -363,6 +455,44 @@ extern "C" int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* 
                   : launch_attn<AttnCfg<0, 128, 2, 128, true>>(Q, K, V, O, B, H, N, D, scale, mask, s, di);
   return narrow ? launch_attn<AttnCfg<0, 64, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di)
                 : launch_attn<AttnCfg<0, 128, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di);
+}
+
+extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
+                                    const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q,
+                                    int64_t total_k, int64_t H, int64_t H_kv, int64_t D, float scale, int dtype,
+                                    int causal, void* stream) {
+  using namespace b200k;
+  if (!Q || !K || !V || !O || !cu_seqlens_q || !cu_seqlens_k)
+    return set_error(B200K_EARG, "b200k_fa2_fwd_varlen: null pointer");
+  if (dtype != B200K_F16 && dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "b200k_fa2_fwd_varlen: dtype %d not supported (f16, bf16)", dtype);
+  if (D != 32 && D != 64 && D != 96 && D != 128)
+    return set_error(B200K_EHEADDIM, "headdim not support! (b200k_fa2_fwd_varlen: D=%lld, supported 32/64/96/128)",
+                     (long long)D);
+  if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)",
+                     (long long)B, (long long)H, (long long)H_kv);
+  if (total_q < 1 || total_q > INT32_MAX || total_k < 1 || total_k > INT32_MAX || max_seqlen_q < 1 || max_seqlen_q > total_q)
+    return set_error(B200K_ESHAPE,
+                     "b200k_fa2_fwd_varlen: need 1 <= total_q, total_k <= 2^31 - 1 and 1 <= max_seqlen_q <= total_q "
+                     "(got total_q=%lld total_k=%lld max_seqlen_q=%lld)",
+                     (long long)total_q, (long long)total_k, (long long)max_seqlen_q);
+  if (B > 65535 || H > 65535 || B * H > 65535)
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: B * H = %lld CTAs per query tile, the grid allows 65535",
+                     (long long)B * (long long)H);
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  DeviceInfo di;
+  int rc = get_device_info(&di);
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  auto run = [&](auto cfg) {
+    return launch_attn_varlen<decltype(cfg)>(Q, K, V, O, cu_seqlens_q, cu_seqlens_k, B, max_seqlen_q, total_q, total_k,
+                                             H, H_kv, D, scale, causal, s, di);
+  };
+  const bool narrow = D <= 64;  // O columns: 64 for D = 32 / 64, 128 for D = 96 / 128
+  if (dtype == B200K_BF16)
+    return narrow ? run(AttnCfg<1, 64, 2, 128, false, true>()) : run(AttnCfg<1, 128, 2, 128, false, true>());
+  return narrow ? run(AttnCfg<0, 64, 2, 128, false, true>()) : run(AttnCfg<0, 128, 2, 128, false, true>());
 }
 
 extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,

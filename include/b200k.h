@@ -103,6 +103,29 @@ int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int
  * b200k_fa2_fwd_f16(...) == b200k_fa2_fwd(..., B200K_F16, 0, NULL, ...). */
 int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
                   float scale, int v_is_dn, int dtype, int causal, const int* seqlens_k, int variant, void* stream);
+/* b200k_fa2_fwd_varlen — the same FA-2 kernel on packed variable-length sequences with grouped-query K/V heads (the
+ * counterpart of flash-attn's flash_attn_varlen_func forward):
+ *   layouts    Q, O [total_q, H, D]; K, V [total_k, H_kv, D]; contiguous, one dtype (B200K_F16 or B200K_BF16);
+ *              D in {32, 64, 96, 128}; scale <= 0 means 1/sqrt(D)
+ *   sequences  cu_seqlens_q, cu_seqlens_k: int32 device arrays [B + 1], non-decreasing, starting at 0.  Sequence b is
+ *              query tokens [cu_seqlens_q[b], cu_seqlens_q[b+1]) and key tokens [cu_seqlens_k[b], cu_seqlens_k[b+1]);
+ *              their lengths Lq and Lk may differ, and either may be 0
+ *   heads      H % H_kv == 0; query head h reads K/V head h / (H / H_kv) (GQA; H_kv == 1 is MQA, H_kv == H is MHA), the
+ *              grouping of torch.repeat_interleave and scaled_dot_product_attention(enable_gqa=True)
+ *   causal     != 0: aligned bottom-right, query row r of a sequence sees key j iff j <= r + Lk - Lq (flash-attn >= 2.1);
+ *              with Lq == Lk this is the causal mask of b200k_fa2_fwd
+ *   zero rows  a row that sees no key (Lk == 0, or causal with r + Lk - Lq < 0) is written as 0
+ *   no sync    max_seqlen_q (>= every Lq; a longer sequence is a caller error) sizes the grid, so the call never reads
+ *              the lengths back to the host and can be captured in a CUDA graph.  Stores are clipped to tokens
+ *              [0, total_q) whatever cu_seqlens holds; reads past total_k are zero-filled
+ *   neighbours the last KV tile of a sequence also reads keys of the next one; they are masked to -inf, so with finite
+ *              K/V each sequence's O has the same bits as when computed alone.  A non-finite V in a neighbouring
+ *              sequence leaks through as 0 * Inf = NaN (the same contract as the padded keys of b200k_fa2_fwd)
+ * Errors: B200K_EARG for a null pointer, B200K_EDTYPE, B200K_EHEADDIM, and B200K_ESHAPE unless B >= 1, H, H_kv >= 1,
+ * H % H_kv == 0, 1 <= max_seqlen_q <= total_q, 1 <= total_q, total_k <= INT32_MAX and B * H <= 65535. */
+int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
+                         const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k,
+                         int64_t H, int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* stream);
 
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
