@@ -3,7 +3,8 @@
 //
 // One CTA computes a 128 x 256 tile of C: warpgroup 0 is the producer (one thread issues the TMA loads), warpgroups 1
 // and 2 each own 64 rows of the tile and issue m64n256 wgmma instructions straight from shared memory.  A consumer
-// keeps one k-block of MMAs in flight and hands the stage before it back to the producer.  128 x 256 x 64 (16-bit) or
+// keeps one k-block of MMAs in flight and hands the stage before it back to the producer; that overlap exists in the
+// machine code only while the kernel contains no function call, hence mbar_wait_nocall.  128 x 256 x 64 (16-bit) or
 // x 32 (fp32) per stage = 48 KB, 4 stages = 192 KB of the 227 KB a block may use on H100.
 //
 // Operand storage: K-major tiles (A [M,K], B^T [N,K]) and, for 16-bit types, MN-major tiles (A^T [K,M], B [K,N]) are
@@ -82,7 +83,7 @@ __global__ void __launch_bounds__(gemm::THREADS, 1)
       tma_prefetch_desc(&tmB);
       for (int kb = 0; kb < nkb; ++kb) {
         const int s = kb % STAGES;
-        if (kb >= STAGES) mbar_wait(empty0 + 8 * s, ((kb / STAGES) - 1) & 1);
+        if (kb >= STAGES) mbar_wait_nocall(empty0 + 8 * s, ((kb / STAGES) - 1) & 1);
         const uint32_t bar = full0 + 8 * s, sA = base + s * Cfg::STAGE_BYTES, sB = sA + Cfg::A_BYTES;
         mbar_arrive_expect_tx(bar, Cfg::STAGE_BYTES);
         if constexpr (Cfg::A_MN) {
@@ -110,7 +111,7 @@ __global__ void __launch_bounds__(gemm::THREADS, 1)
   for (int i = 0; i < 128; ++i) d[i] = 0.f;
   for (int kb = 0; kb < nkb; ++kb) {
     const int s = kb % STAGES;
-    mbar_wait(full0 + 8 * s, (kb / STAGES) & 1);
+    mbar_wait_nocall(full0 + 8 * s, (kb / STAGES) & 1);
     const uint32_t sA = base + s * Cfg::STAGE_BYTES, sB = sA + Cfg::A_BYTES;
     fence_regs<128>(d);
     wgmma_fence();

@@ -16,8 +16,8 @@ namespace b200k {
 
 #ifndef B200K_SPIN_LIMIT_CYCLES
 // A protocol bug in an mbarrier pipeline shows up as a hang.  Every spin-wait below gives up after this many
-// SM cycles (~5 s), prints which barrier it was waiting on and traps, so a bug becomes a CUDA error instead
-// of a dead GPU box.  The check is only reached after a failed try_wait (slow path).
+// SM cycles (~5 s), prints which barrier it was waiting on (mbar_wait_nocall: does not print) and traps, so a bug
+// becomes a CUDA error instead of a dead GPU box.  The check is only reached after a failed try_wait (slow path).
 #define B200K_SPIN_LIMIT_CYCLES (10LL * 1000 * 1000 * 1000)
 #endif
 
@@ -132,6 +132,16 @@ __device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
   long long t0 = clock64();
   while (!mbar_try_wait(bar, parity)) {
     if (clock64() - t0 > B200K_SPIN_LIMIT_CYCLES) mbar_timeout_trap(bar, parity);
+  }
+}
+// The same wait with no function call in it: on timeout it traps inline, without the message.  ptxas serialises every
+// wgmma of a kernel that contains a call (info C7510: each MMA then waits for the previous one to finish), and the
+// printf behind mbar_wait is such a call.  A kernel that overlaps wgmma must use this wait for every barrier it waits on.
+__device__ __forceinline__ void mbar_wait_nocall(uint32_t bar, uint32_t parity) {
+  if (mbar_try_wait(bar, parity)) return;
+  long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (clock64() - t0 > B200K_SPIN_LIMIT_CYCLES) asm volatile("trap;");
   }
 }
 
