@@ -5,7 +5,8 @@
 // and 2 each own 64 rows of the tile and issue m64n256 wgmma instructions straight from shared memory.  A consumer
 // keeps one k-block of MMAs in flight and hands the stage before it back to the producer; that overlap exists in the
 // machine code only while the kernel contains no function call, hence mbar_wait_nocall.  128 x 256 x 64 (16-bit) or
-// x 32 (fp32) per stage = 48 KB, 4 stages = 192 KB of the 227 KB a block may use on H100.
+// x 32 (fp32) per stage = 48 KB, 4 stages = 192 KB, plus 32 KB of epilogue staging, of the 227 KB a block may use.
+// C leaves through that staging buffer and TMA stores.
 //
 // Operand storage: K-major tiles (A [M,K], B^T [N,K]) and, for 16-bit types, MN-major tiles (A^T [K,M], B [K,N]) are
 // consumed in place through the transpose bits of wgmma.  TF32 wgmma reads K-major operands only, so an fp32 B stored
@@ -17,6 +18,7 @@ namespace b200k {
 
 namespace gemm {
 constexpr int BM = 128, BN = 256, STAGES = 4, THREADS = 384, GROUP_M = 16;
+constexpr int STG_BYTES = 16384;  // epilogue staging per consumer warpgroup: two 64-row x 128-byte TMA boxes
 }
 
 template <int DT_, bool A_MN_, bool B_MN_>  // DT: 0 f16, 1 bf16, 2 tf32 (fp32 storage)
@@ -29,8 +31,9 @@ struct GemmCfg {
   static constexpr int A_BYTES = gemm::BM * BK * ES;
   static constexpr int B_BYTES = gemm::BN * BK * ES;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  static constexpr int SMEM_BYTES = gemm::STAGES * STAGE_BYTES + 1024 + 2 * gemm::STAGES * 8;
+  static constexpr int SMEM_BYTES = gemm::STAGES * STAGE_BYTES + 2 * gemm::STG_BYTES + 1024 + 2 * gemm::STAGES * 8;
   static_assert(!(DT == 2 && (A_MN || B_MN)), "tf32 wgmma reads K-major operands only");
+  static_assert(SMEM_BYTES <= 232448, "more shared memory than an H100 block may use");
 };
 
 template <class Cfg>
@@ -52,14 +55,69 @@ __device__ __forceinline__ void gemm_mma_kblock(float* d, uint32_t sA, uint32_t 
   }
 }
 
+// Epilogue of one warpgroup: its 64 x 256 accumulators -> C through a 16 KB staging buffer, in column slices (two for
+// 16-bit, four for fp32).  Each slice is two 64-row x 128-byte boxes in the 128B-swizzled layout of tmC; TMA clips the
+// store to [M, N].  A slice is written only after the store of the one before it has read the buffer.
+template <class Cfg>
+__device__ __forceinline__ void gemm_store_tile(const float* d, const CUtensorMap* tmC, uint32_t stg, int cw, int row0,
+                                                int col0) {
+  constexpr int SLICES = Cfg::DT == 2 ? 4 : 2, JS = 32 / SLICES, JB = JS / 2;  // 8-column groups per slice / per box
+  const int t = threadIdx.x & 127, lane = t & 31, warp = t / 32;
+  const bool leader = t == 0;
+#pragma unroll
+  for (int sl = 0; sl < SLICES; ++sl) {
+    if (leader) tma_store_wait_read<0>();
+    named_bar_sync(1 + cw, 128);
+    if constexpr (Cfg::DT == 2) {
+      // thread owns rows r, r + 8 and column pair 8j + 2q: 8 bytes in 16-byte chunk 2 (j % 4) + q / 2
+      const int q = lane & 3;
+#pragma unroll
+      for (int jj = 0; jj < JS; ++jj) {
+        const int j = sl * JS + jj;
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int r = warp * 16 + 8 * h + lane / 4;
+          const int chunk = 2 * (jj % JB) + q / 2;
+          const uint32_t a = stg + (jj / JB) * 8192 + r * 128 + ((chunk ^ (r & 7)) << 4) + (q & 1) * 8;
+          asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(a), "f"(d[4 * j + 2 * h]), "f"(d[4 * j + 2 * h + 1])
+                       : "memory");
+        }
+      }
+    } else {
+      // one stmatrix.x4 per two 8-column groups: matrices (rows +0, j), (rows +8, j), (rows +0, j+1), (rows +8, j+1)
+      const int m = lane / 8, r = warp * 16 + 8 * (m & 1) + (lane & 7);
+#pragma unroll
+      for (int jj = 0; jj < JS; jj += 2) {
+        const int j = sl * JS + jj, chunk = jj % JB + (m >> 1);
+        const uint32_t a = stg + (jj / JB) * 8192 + r * 128 + ((chunk ^ (r & 7)) << 4);
+        uint32_t p[4];
+#pragma unroll
+        for (int i = 0; i < 4; ++i)
+          p[i] = Cfg::DT == 1 ? pack_bf162(d[4 * j + 2 * i], d[4 * j + 2 * i + 1])
+                              : pack_half2(d[4 * j + 2 * i], d[4 * j + 2 * i + 1]);
+        stmatrix_x4(a, p[0], p[1], p[2], p[3]);
+      }
+    }
+    fence_proxy_async_smem();
+    named_bar_sync(1 + cw, 128);
+    if (leader) {
+      const int c = col0 + sl * (gemm::BN / SLICES);
+      tma_store_2d(tmC, stg, c, row0);
+      tma_store_2d(tmC, stg + 8192, c + 128 / Cfg::ES, row0);
+      tma_store_commit();
+    }
+  }
+}
+
 template <class Cfg>
 __global__ void __launch_bounds__(gemm::THREADS, 1)
-    hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, void* C, int M,
-                       int N, int K, int tiles_m, int tiles_n) {
+    hgemm_wgmma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
+                       const __grid_constant__ CUtensorMap tmC, int K, int tiles_m, int tiles_n) {
   using namespace gemm;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023) & ~1023u;
-  const uint32_t full0 = base + STAGES * Cfg::STAGE_BYTES, empty0 = full0 + STAGES * 8;
+  const uint32_t stg0 = base + STAGES * Cfg::STAGE_BYTES;
+  const uint32_t full0 = stg0 + 2 * STG_BYTES, empty0 = full0 + STAGES * 8;
   const int wg = threadIdx.x / 128;
 
   // grouped rasterisation: GROUP_M row tiles share each B column tile while it is in L2
@@ -105,7 +163,9 @@ __global__ void __launch_bounds__(gemm::THREADS, 1)
     return;
   }
 
-  const int cw = wg - 1;
+  const int cw = wg - 1, t = threadIdx.x & 127;
+  const bool leader = t == 0;
+  if (leader) tma_prefetch_desc(&tmC);
   float d[128];
 #pragma unroll
   for (int i = 0; i < 128; ++i) d[i] = 0.f;
@@ -119,52 +179,30 @@ __global__ void __launch_bounds__(gemm::THREADS, 1)
     wgmma_commit();
     wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
     fence_regs<128>(d);
-    if (kb > 0 && (threadIdx.x & 127) == 0) mbar_arrive(empty0 + 8 * ((kb - 1) % STAGES));
+    if (kb > 0 && leader) mbar_arrive(empty0 + 8 * ((kb - 1) % STAGES));
   }
   wgmma_wait<0>();
   fence_regs<128>(d);
-
-  // epilogue: accumulator fragment -> global, clipped to [M, N].  Thread owns rows r0, r0 + 8 and column pairs 8j + 2q.
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
-  const int r0 = tm * BM + cw * 64 + warp * 16 + lane / 4;
-  const int c0 = tn * BN + 2 * (lane & 3);
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int r = r0 + 8 * h;
-    if (r >= M) continue;
-#pragma unroll
-    for (int j = 0; j < 32; ++j) {
-      const int c = c0 + 8 * j;
-      if (c >= N) continue;  // N is even, so c + 1 < N as well
-      const float x = d[4 * j + 2 * h], y = d[4 * j + 2 * h + 1];
-      const size_t off = size_t(r) * N + c;
-      if constexpr (Cfg::DT == 2) {
-        *reinterpret_cast<float2*>(static_cast<float*>(C) + off) = make_float2(x, y);
-      } else if constexpr (Cfg::DT == 1) {
-        *reinterpret_cast<uint32_t*>(static_cast<__nv_bfloat16*>(C) + off) = pack_bf162(x, y);
-      } else {
-        *reinterpret_cast<uint32_t*>(static_cast<__half*>(C) + off) = pack_half2(x, y);
-      }
-    }
-  }
+  gemm_store_tile<Cfg>(d, &tmC, stg0 + cw * STG_BYTES, cw, tm * BM + cw * 64, tn * BN);
+  if (leader) tma_store_wait_all<0>();
 }
 
 template <class Cfg>
 static int launch_gemm(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, cudaStream_t s,
                        const DeviceInfo& di) {
   using namespace gemm;
-  CUtensorMap tmA, tmB;
+  CUtensorMap tmA, tmB, tmC;
   int rc = Cfg::A_MN ? make_tmap_2d(&tmA, A, K, M, M, Cfg::BK, 64, Cfg::ES)
                      : make_tmap_2d(&tmA, A, M, K, K, BM, Cfg::BK, Cfg::ES);
   if (rc) return rc;
   rc = Cfg::B_MN ? make_tmap_2d(&tmB, B, K, N, N, Cfg::BK, 64, Cfg::ES) : make_tmap_2d(&tmB, B, N, K, K, BN, Cfg::BK, Cfg::ES);
   if (rc) return rc;
-  const int64_t tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN;
-  if (tiles_m * tiles_n > INT32_MAX) return set_error(B200K_ESHAPE, "GEMM too large: %lld tiles", (long long)(tiles_m * tiles_n));
+  if ((rc = make_tmap_2d(&tmC, C, M, N, N, 64, 128 / Cfg::ES, Cfg::ES))) return rc;
+  const int64_t tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN, tiles = tiles_m * tiles_n;
+  if (tiles > INT32_MAX) return set_error(B200K_ESHAPE, "GEMM too large: %lld tiles", (long long)tiles);
   auto kern = hgemm_wgmma_kernel<Cfg>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, Cfg::SMEM_BYTES))) return rc;
-  kern<<<unsigned(tiles_m * tiles_n), THREADS, Cfg::SMEM_BYTES, s>>>(tmA, tmB, C, int(M), int(N), int(K), int(tiles_m),
-                                                                      int(tiles_n));
+  kern<<<unsigned(tiles), THREADS, Cfg::SMEM_BYTES, s>>>(tmA, tmB, tmC, int(K), int(tiles_m), int(tiles_n));
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -174,6 +212,7 @@ static int gemm_dispatch(const char* who, const void* A, const void* B, void* C,
                          int b_is_nk, int variant, void* stream, int a_is_km = 0) {
   constexpr int PACK = (DT == 2) ? 4 : 8;  // elements per 16 bytes
   if (!A || !B || !C) return set_error(B200K_EARG, "%s: null pointer", who);
+  if (reinterpret_cast<uintptr_t>(C) & 15) return set_error(B200K_EALIGN, "%s: C (%p) must be 16-byte aligned", who, C);
   if (M < 1 || N < 1 || K < 1 || M > INT32_MAX || N > INT32_MAX || K > INT32_MAX)
     return set_error(B200K_ESHAPE, "%s: M,N,K must be in [1, 2^31) (got %lld,%lld,%lld)", who, (long long)M, (long long)N,
                      (long long)K);

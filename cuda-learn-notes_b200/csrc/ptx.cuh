@@ -192,6 +192,13 @@ template <int N>
 __device__ __forceinline__ void tma_store_wait_all() {  // global writes are complete
   asm volatile("cp.async.bulk.wait_group %0;" ::"n"(N) : "memory");
 }
+// Four 8x8 16-bit matrices to shared memory: lanes 8i .. 8i+7 give the row addresses of matrix i, and register i of
+// lane l holds row l / 4, columns 2 (l % 4) and 2 (l % 4) + 1 of matrix i (the wgmma accumulator fragment, packed).
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r0), "r"(r1), "r"(r2),
+               "r"(r3)
+               : "memory");
+}
 
 // ---------------------------------------------------------------------------------------------- wgmma
 // Shared-memory matrix descriptor (64 bit):

@@ -47,7 +47,8 @@ int b200k_device_info(int* sm_count, int* cc_major, int* cc_minor);
  *       kernels/hgemm/mma/swizzle/hgemm_mma_stage_tn_swizzle_x4.cu:L860, kernels/hgemm/cutlass/hgemm_mma_stage_tn_cute.cu:L522,
  *       kernels/hgemm/cublas/hgemm_cublas.cu:L63-84 (hgemm_cublas_tensor_op_tn)
  * All matrices contiguous row-major; M,N,K >= 1; K % 8 == 0 and N % 8 == 0 (16-byte row pitch for TMA).
- * Ragged M/N/K (not multiples of the tile) are handled by TMA zero-fill / store clipping.
+ * A, B and C must be 16-byte aligned (C is written by TMA stores); an unaligned C returns B200K_EALIGN before any
+ * CUDA call.  Ragged M/N/K (not multiples of the tile) are handled by TMA zero-fill / store clipping.
  * variant (low 8 bits): 0 .. 4, the B200K_HGEMM_* names below.  They are kept for source compatibility: every value
  *   runs the same 128 x 256 tile kernel, so all of them give the same bits.  Higher bits are ignored.
  */
