@@ -74,70 +74,26 @@ static int get_encode_fn(EncodeTiledFn* fn) {
   return B200K_OK;
 }
 
-int make_tmap_2d_u16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
-                     uint32_t box_rows, uint32_t box_cols, bool swizzle128) {
+int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims, const uint64_t* strides,
+              const uint32_t* box) {
   EncodeTiledFn fn;
   int rc = get_encode_fn(&fn);
   if (rc) return rc;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((pitch_elems * 2) & 15))
-    return set_error(B200K_EALIGN, "TMA needs a 16-byte aligned base (%p) and row pitch (%llu bytes)", base,
-                     (unsigned long long)(pitch_elems * 2));
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {pitch_elems * 2};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  bool aligned = (reinterpret_cast<uintptr_t>(base) & 15) == 0;
+  for (int i = 0; i < rank - 1; ++i) aligned = aligned && (strides[i] & 15) == 0;
+  if (!aligned)
+    return set_error(B200K_EALIGN, "TMA needs a 16-byte aligned base (%p) and strides (row stride %llu bytes)", base,
+                     (unsigned long long)strides[0]);
+  const cuuint32_t estr[3] = {1, 1, 1};
+  CUresult r = fn(out, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank,
+                  const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)
-    return set_error(B200K_ECUDA, "cuTensorMapEncodeTiled(2d rows=%llu cols=%llu box=%ux%u) failed with CUresult %d",
-                     (unsigned long long)rows, (unsigned long long)cols, box_rows, box_cols, (int)r);
-  return B200K_OK;
-}
-
-int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems, uint32_t box_rows,
-                 uint32_t box_cols, int elem_bytes, bool atom32) {
-  if (elem_bytes == 2) return make_tmap_2d_u16(out, base, rows, cols, pitch_elems, box_rows, box_cols, true);
-  EncodeTiledFn fn;
-  int rc = get_encode_fn(&fn);
-  if (rc) return rc;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((pitch_elems * 4) & 15))
-    return set_error(B200K_EALIGN, "TMA needs a 16-byte aligned base (%p) and row pitch (%llu bytes)", base,
-                     (unsigned long long)(pitch_elems * 4));
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {pitch_elems * 4};
-  cuuint32_t box[2] = {box_cols, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, atom32 ? CU_TENSOR_MAP_SWIZZLE_128B_ATOM_32B : CU_TENSOR_MAP_SWIZZLE_128B,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return set_error(B200K_ECUDA, "cuTensorMapEncodeTiled(2d f32 rows=%llu cols=%llu box=%ux%u) failed with CUresult %d",
-                     (unsigned long long)rows, (unsigned long long)cols, box_rows, box_cols, (int)r);
-  return B200K_OK;
-}
-
-int make_tmap_3d_u16(CUtensorMap* out, const void* base, uint64_t d2, uint64_t d1, uint64_t d0, uint64_t stride2,
-                     uint64_t stride1, uint32_t box2, uint32_t box1, uint32_t box0, int swizzle_bytes) {
-  EncodeTiledFn fn;
-  int rc = get_encode_fn(&fn);
-  if (rc) return rc;
-  if ((reinterpret_cast<uintptr_t>(base) & 15) || ((stride1 * 2) & 15) || ((stride2 * 2) & 15))
-    return set_error(B200K_EALIGN, "TMA needs 16-byte aligned base and strides");
-  cuuint64_t dims[3] = {d0, d1, d2};
-  cuuint64_t strides[2] = {stride1 * 2, stride2 * 2};
-  cuuint32_t box[3] = {box0, box1, box2};
-  cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<void*>(base), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE,
-                  swizzle_bytes == 128  ? CU_TENSOR_MAP_SWIZZLE_128B
-                  : swizzle_bytes == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
-                  : swizzle_bytes == 32 ? CU_TENSOR_MAP_SWIZZLE_32B
-                                        : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS)
-    return set_error(B200K_ECUDA, "cuTensorMapEncodeTiled(3d %llux%llux%llu box=%ux%ux%u) failed with CUresult %d",
-                     (unsigned long long)d2, (unsigned long long)d1, (unsigned long long)d0, box2, box1, box0, (int)r);
+    return set_error(B200K_ECUDA,
+                     "cuTensorMapEncodeTiled(%d-byte elements, dims %llu x %llu x %llu, box %u x %u x %u, innermost first) "
+                     "failed with CUresult %d",
+                     elem_bytes, (unsigned long long)dims[0], (unsigned long long)dims[1],
+                     (unsigned long long)(rank == 3 ? dims[2] : 1), box[0], box[1], rank == 3 ? box[2] : 1u, (int)r);
   return B200K_OK;
 }
 

@@ -35,15 +35,10 @@ int get_device_info(DeviceInfo* out);
 // recorded size only grows, so a transient failure is retried by the next launch instead of poisoning it.
 int ensure_dynamic_smem(const void* func, int device, int bytes);
 
-// 2-D row-major fp16/any-16-bit tensor map: global [rows, cols] (cols contiguous, row pitch `pitch_elems`),
-// box [box_rows, box_cols], 128B swizzle when box_cols*2 == 128, else no swizzle.
-int make_tmap_2d_u16(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems,
-                     uint32_t box_rows, uint32_t box_cols, bool swizzle128);
-// same, for 2-byte (f16 / bf16) or 4-byte (fp32) elements; always SWIZZLE_128B
-int make_tmap_2d(CUtensorMap* out, const void* base, uint64_t rows, uint64_t cols, uint64_t pitch_elems, uint32_t box_rows,
-                 uint32_t box_cols, int elem_bytes, bool atom32 = false);
-// 3-D variant: [d2, d1, d0] with d0 contiguous, strides in elements; swizzle_bytes in {0, 32, 64, 128}.
-int make_tmap_3d_u16(CUtensorMap* out, const void* base, uint64_t d2, uint64_t d1, uint64_t d0, uint64_t stride2,
-                     uint64_t stride1, uint32_t box2, uint32_t box1, uint32_t box0, int swizzle_bytes);
+// TMA tensor map with 128-byte swizzle over a rank-2 or rank-3 global array of 2-byte elements (f16 and bf16 alike,
+// encoded as FLOAT16) or 4-byte fp32 ones.  dims[rank] and box[rank] list the innermost dimension first; strides[rank - 1]
+// are the byte strides of dims[1 ..].  The base and every stride must be multiples of 16 bytes (B200K_EALIGN otherwise).
+int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, const uint64_t* dims, const uint64_t* strides,
+              const uint32_t* box);
 
 }  // namespace b200k

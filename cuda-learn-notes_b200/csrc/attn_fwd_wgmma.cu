@@ -49,31 +49,6 @@ struct AttnCfg {
   static int smem_bytes(int nqc) { return 1024 + nqc * BM * 128 + KSTAGES * K_BYTES + VSTAGES * V_BYTES + BAR_BYTES; }
 };
 
-template <int DT, int N, int TA, int TB>
-__device__ __forceinline__ void mma_ss(float* d, uint64_t da, uint64_t db, int scale_d) {
-  if constexpr (DT == 0) {
-    if constexpr (N == 64) wgmma_ss_f16_n64<TA, TB>(d, da, db, scale_d);
-    else wgmma_ss_f16_n128<TA, TB>(d, da, db, scale_d);
-  } else {
-    if constexpr (N == 64) wgmma_ss_bf16_n64<TA, TB>(d, da, db, scale_d);
-    else wgmma_ss_bf16_n128<TA, TB>(d, da, db, scale_d);
-  }
-}
-template <int DT, int N, int TB>
-__device__ __forceinline__ void mma_rs(float* d, const uint32_t* a, uint64_t db, int scale_d) {
-  if constexpr (DT == 0) {
-    if constexpr (N == 64) wgmma_rs_f16_n64<TB>(d, a, db, scale_d);
-    else if constexpr (N == 128) wgmma_rs_f16_n128<TB>(d, a, db, scale_d);
-    else if constexpr (N == 192) wgmma_rs_f16_n192<TB>(d, a, db, scale_d);
-    else wgmma_rs_f16_n256<TB>(d, a, db, scale_d);
-  } else {
-    if constexpr (N == 64) wgmma_rs_bf16_n64<TB>(d, a, db, scale_d);
-    else if constexpr (N == 128) wgmma_rs_bf16_n128<TB>(d, a, db, scale_d);
-    else if constexpr (N == 192) wgmma_rs_bf16_n192<TB>(d, a, db, scale_d);
-    else wgmma_rs_bf16_n256<TB>(d, a, db, scale_d);
-  }
-}
-
 __device__ __forceinline__ float ex2(float x) {
   float y;
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -224,7 +199,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
       for (int k = 0; k < 4; ++k) {
         const uint64_t da = wgmma_desc(sQ + c * BM * 128 + cw * 64 * 128 + k * 32, 16, 1024);
         const uint64_t db = wgmma_desc(sK + s * Cfg::K_BYTES + k * 32, 16, 1024);
-        mma_ss<Cfg::DT, BN, 0, 0>(s_acc, da, db, 1);
+        wgmma_ss<Cfg::DT, BN, 0, 0>(s_acc, da, db, 1);
       }
       wgmma_commit();
       wgmma_wait<1>();
@@ -294,7 +269,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     for (int kk = 0; kk < BN / 16; ++kk) {
       const uint64_t db = Cfg::V_DN ? wgmma_desc(vb + (kk / 4) * DV * 128 + (kk % 4) * 32, 16, 1024)
                                     : wgmma_desc(vb + kk * 2048, BN * 128, 1024);
-      mma_rs<Cfg::DT, DV, Cfg::V_DN ? 0 : 1>(o, pa[kk], db, 1);
+      wgmma_rs<Cfg::DT, DV, Cfg::V_DN ? 0 : 1>(o, pa[kk], db, 1);
     }
     wgmma_commit();
     wgmma_wait<0>();
@@ -341,6 +316,13 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   }
 }
 
+// Tensor map over a contiguous 16-bit [d2, d1, d0] array, box [box2, box1, 64]: each box row is one 128-byte swizzle row.
+static int attn_tmap(CUtensorMap* m, const void* p, uint64_t d2, uint64_t d1, uint64_t d0, uint32_t box2, uint32_t box1) {
+  const uint64_t dims[3] = {d0, d1, d2}, strides[2] = {2 * d0, 2 * d0 * d1};
+  const uint32_t box[3] = {64, box1, box2};
+  return make_tmap(m, p, 2, 3, dims, strides, box);
+}
+
 template <class Cfg>
 static int launch_attn(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
                        float scale, const AttnMask& mask, cudaStream_t s, const DeviceInfo& di) {
@@ -351,10 +333,10 @@ static int launch_attn(const void* Q, const void* K, const void* V, void* O, int
     return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  if ((rc = make_tmap_3d_u16(&tmQ, Q, BH, N, D, uint64_t(N) * D, D, 1, Cfg::BM, 64, 128))) return rc;
-  if ((rc = make_tmap_3d_u16(&tmK, K, BH, N, D, uint64_t(N) * D, D, 1, Cfg::BN, 64, 128))) return rc;
-  if (Cfg::V_DN) rc = make_tmap_3d_u16(&tmV, V, BH, D, N, uint64_t(N) * D, N, 1, Cfg::DV, 64, 128);
-  else rc = make_tmap_3d_u16(&tmV, V, BH, N, D, uint64_t(N) * D, D, 1, Cfg::BN, 64, 128);
+  if ((rc = attn_tmap(&tmQ, Q, BH, N, D, 1, Cfg::BM))) return rc;
+  if ((rc = attn_tmap(&tmK, K, BH, N, D, 1, Cfg::BN))) return rc;
+  if (Cfg::V_DN) rc = attn_tmap(&tmV, V, BH, D, N, 1, Cfg::DV);
+  else rc = attn_tmap(&tmV, V, BH, N, D, 1, Cfg::BN);
   if (rc) return rc;
   auto kern = attn_fwd_wgmma_kernel<Cfg>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
@@ -378,9 +360,9 @@ static int launch_attn_varlen(const void* Q, const void* K, const void* V, void*
     return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
   CUtensorMap tmQ, tmK, tmV;
   int rc;
-  if ((rc = make_tmap_3d_u16(&tmQ, Q, total_q, H, D, uint64_t(H) * D, D, Cfg::BM, 1, 64, 128))) return rc;
-  if ((rc = make_tmap_3d_u16(&tmK, K, total_k, H_kv, D, uint64_t(H_kv) * D, D, Cfg::BN, 1, 64, 128))) return rc;
-  if ((rc = make_tmap_3d_u16(&tmV, V, total_k, H_kv, D, uint64_t(H_kv) * D, D, Cfg::BN, 1, 64, 128))) return rc;
+  if ((rc = attn_tmap(&tmQ, Q, total_q, H, D, Cfg::BM, 1))) return rc;
+  if ((rc = attn_tmap(&tmK, K, total_k, H_kv, D, Cfg::BN, 1))) return rc;
+  if ((rc = attn_tmap(&tmV, V, total_k, H_kv, D, Cfg::BN, 1))) return rc;
   auto kern = attn_fwd_wgmma_kernel<Cfg>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
   AttnMask mask;

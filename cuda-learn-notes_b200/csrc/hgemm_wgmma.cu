@@ -45,13 +45,7 @@ __device__ __forceinline__ void gemm_mma_kblock(float* d, uint32_t sA, uint32_t 
     const uint64_t da = Cfg::A_MN ? wgmma_desc(sA + cw * 64 * Cfg::BK * Cfg::ES + k * 2048, 64 * Cfg::BK * Cfg::ES, 1024)
                                   : wgmma_desc(sA + cw * 64 * 128 + k * 32, 16, 1024);
     const uint64_t db = Cfg::B_MN ? wgmma_desc(sB + k * 2048, 64 * Cfg::BK * Cfg::ES, 1024) : wgmma_desc(sB + k * 32, 16, 1024);
-    if constexpr (Cfg::DT == 2) {
-      wgmma_ss_tf32_n256(d, da, db, 1);
-    } else if constexpr (Cfg::DT == 1) {
-      wgmma_ss_bf16_n256<Cfg::A_MN ? 1 : 0, Cfg::B_MN ? 1 : 0>(d, da, db, 1);
-    } else {
-      wgmma_ss_f16_n256<Cfg::A_MN ? 1 : 0, Cfg::B_MN ? 1 : 0>(d, da, db, 1);
-    }
+    wgmma_ss<Cfg::DT, 256, Cfg::A_MN, Cfg::B_MN>(d, da, db, 1);
   }
 }
 
@@ -191,13 +185,18 @@ template <class Cfg>
 static int launch_gemm(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, cudaStream_t s,
                        const DeviceInfo& di) {
   using namespace gemm;
+  // every operand is a contiguous row-major [rows, cols] array
+  auto tmap = [](CUtensorMap* m, const void* p, int64_t rows, int64_t cols, uint32_t box_rows, uint32_t box_cols) {
+    const uint64_t dims[2] = {uint64_t(cols), uint64_t(rows)}, strides[1] = {uint64_t(cols) * Cfg::ES};
+    const uint32_t box[2] = {box_cols, box_rows};
+    return make_tmap(m, p, Cfg::ES, 2, dims, strides, box);
+  };
   CUtensorMap tmA, tmB, tmC;
-  int rc = Cfg::A_MN ? make_tmap_2d(&tmA, A, K, M, M, Cfg::BK, 64, Cfg::ES)
-                     : make_tmap_2d(&tmA, A, M, K, K, BM, Cfg::BK, Cfg::ES);
+  int rc = Cfg::A_MN ? tmap(&tmA, A, K, M, Cfg::BK, 64) : tmap(&tmA, A, M, K, BM, Cfg::BK);
   if (rc) return rc;
-  rc = Cfg::B_MN ? make_tmap_2d(&tmB, B, K, N, N, Cfg::BK, 64, Cfg::ES) : make_tmap_2d(&tmB, B, N, K, K, BN, Cfg::BK, Cfg::ES);
+  rc = Cfg::B_MN ? tmap(&tmB, B, K, N, Cfg::BK, 64) : tmap(&tmB, B, N, K, BN, Cfg::BK);
   if (rc) return rc;
-  if ((rc = make_tmap_2d(&tmC, C, M, N, N, 64, 128 / Cfg::ES, Cfg::ES))) return rc;
+  if ((rc = tmap(&tmC, C, M, N, 64, 128 / Cfg::ES))) return rc;
   const int64_t tiles_m = (M + BM - 1) / BM, tiles_n = (N + BN - 1) / BN, tiles = tiles_m * tiles_n;
   if (tiles > INT32_MAX) return set_error(B200K_ESHAPE, "GEMM too large: %lld tiles", (long long)tiles);
   auto kern = hgemm_wgmma_kernel<Cfg>;
