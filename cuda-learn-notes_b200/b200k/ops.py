@@ -9,6 +9,7 @@ PyTorch is used for device memory and streams only; every computation happens in
 """
 from __future__ import annotations
 
+import ctypes
 import math
 from typing import Optional
 
@@ -216,6 +217,62 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
         L.check(_lib.b200k_fa2_fwd_varlen(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), cu_seqlens_q.data_ptr(),
                                           cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
                                           float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+
+
+def fa2_fwd_kvcache_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int) -> int:
+    """Workspace bytes :func:`fa2_fwd_kvcache` needs for these shapes (0 when it runs unsplit); queries the device."""
+    n = ctypes.c_size_t(0)
+    L.check(_lib.b200k_fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, max_seqlen_k, ctypes.byref(n)))
+    return n.value
+
+
+def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_table: Optional[torch.Tensor] = None,
+                    scale: Optional[float] = None, causal: bool = False) -> None:
+    """Attention of the newest Lq query tokens of each sequence against its KV cache (the forward of flash-attn's
+    ``flash_attn_with_kvcache``, without appending K/V or rotary).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
+    [B, S, H_kv, D] without ``block_table``, or [num_pages, page_size, H_kv, D] with an int32 ``block_table``
+    [B, pages_per_seq] (key j of sequence b is slot j % page_size of page block_table[b, j // page_size]).
+    ``cache_seqlens``: int32 [B] key counts on the device.  ``causal``: token t sees keys <= t + Lk - Lq.  H % H_kv == 0
+    (query head h reads K/V head h // (H // H_kv)).  Nothing is read back to the host, so the call can be captured in a
+    CUDA graph; the split workspace is allocated per call on the current stream."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    for t in (q, k_cache, v_cache, o):
+        _check_dtype(t, dt)
+    if q.dim() != 4 or k_cache.dim() != 4:
+        raise RuntimeError("Tensor size mismatch!")
+    B, Lq, H, D = q.shape
+    num_pages, page_size, H_kv = k_cache.size(0), k_cache.size(1), k_cache.size(2)
+    if (tuple(k_cache.shape) != (num_pages, page_size, H_kv, D) or tuple(v_cache.shape) != tuple(k_cache.shape)
+            or tuple(o.shape) != tuple(q.shape)):
+        raise RuntimeError("Tensor size mismatch!")
+    if H_kv < 1 or H % H_kv:
+        raise RuntimeError("Tensor size mismatch!")
+    if D not in FA2_HEADDIMS:
+        raise RuntimeError("headdim not support!")
+    _check_dtype(cache_seqlens, torch.int32)
+    if cache_seqlens.numel() != B:
+        raise RuntimeError("Tensor size mismatch!")
+    tensors = [q, k_cache, v_cache, o, cache_seqlens]
+    if block_table is None:
+        if num_pages != B:
+            raise RuntimeError("Tensor size mismatch!")
+        pages_per_seq = 1
+    else:
+        _check_dtype(block_table, torch.int32)
+        if block_table.dim() != 2 or block_table.size(0) != B:
+            raise RuntimeError("Tensor size mismatch!")
+        pages_per_seq = block_table.size(1)
+        tensors.append(block_table)
+    _check_cuda_contig(*tensors)
+    with _DeviceGuard(q):
+        nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
+        L.check(_lib.b200k_fa2_fwd_kvcache(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
+                                           cache_seqlens.data_ptr(),
+                                           block_table.data_ptr() if block_table is not None else None,
+                                           B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq,
+                                           float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0,
+                                           ws.data_ptr() if ws is not None else None, nbytes, _stream(q)))
 
 
 def ffpa_fwd(q, k, v, o, scale: Optional[float] = None, variant: int = 0) -> None:

@@ -14,6 +14,9 @@
 // store; padded keys are masked.  Causal CTAs stop at their diagonal tile.
 // Packed variable-length sequences with grouped K/V heads (AttnCfg::VARLEN) run the same main loop; only the tensor
 // maps, the TMA coordinates, the per-CTA key length, the causal diagonal and the epilogue's addressing differ.
+// KV-cache decode (AttnCfg::DECODE) runs it too: a CTA owns the query rows of one K/V head (tokens x grouped heads packed
+// into one 64-row tile), reads K / V through a page table, takes one split of the sequence's KV tiles, and writes either
+// O or fp32 partials that attn_combine_kernel merges.
 #include "abi_common.cuh"
 #include "ptx.cuh"
 
@@ -36,10 +39,26 @@ struct AttnVarlen {
   int total_q = 0;
 };
 
-template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_, bool VARLEN_ = false>  // DT: 0 f16, 1 bf16
+// KV-cache decode (Cfg::DECODE).  Q / O are [B, Lq, H, D]; the caches are [num_pages, page_size, H_kv, D], key j of
+// sequence b at slot j % page_size of page table[b * pages_per_seq + j / page_size] (table null: contiguous cache,
+// sequence b at rows [b * page_size, ...)).  mask.seqlens holds the key counts, mask.H the query heads.  The 64 rows of
+// a CTA are T tokens x hb heads of one group (row r = token r / hb, head r % hb).  With more than one split (gridDim.x)
+// the CTA writes O / l and the row's base-2 log-sum-exp to `part` / `lse` ([split][row][D], [split][row], row =
+// (b * Lq + t) * H + h) instead of O.
+struct AttnDecode {
+  const int* table = nullptr;
+  float* part = nullptr;
+  float* lse = nullptr;
+  long long rows = 0;  // B * Lq * H
+  int Lq = 1, group = 1, hb = 1, T = 1, nhb = 1;
+  int page_size = 1, pages_per_seq = 1, box_rows = 1;
+  int oob = 0;  // a row coordinate past the end of the cache maps: TMA zero-fills the box
+};
+
+template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_, bool VARLEN_ = false, bool DECODE_ = false>  // DT: 0 f16, 1 bf16
 struct AttnCfg {
   static constexpr int DT = DT_, DV = DV_, NWG = NWG_, BN = BN_;
-  static constexpr bool V_DN = V_DN_, VARLEN = VARLEN_;
+  static constexpr bool V_DN = V_DN_, VARLEN = VARLEN_, DECODE = DECODE_;
   static constexpr int BM = 64 * NWG;
   static constexpr int THREADS = 128 * (NWG + 1);
   static constexpr int KSTAGES = 4, VSTAGES = 2;
@@ -92,19 +111,23 @@ template <class Cfg>
 __global__ void __launch_bounds__(Cfg::THREADS, 1)
     attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
                           const __grid_constant__ CUtensorMap tmV, void* O, int N, int D, int nqc, float scale_log2,
-                          const AttnMask mask, const AttnVarlen vl) {
+                          const AttnMask mask, const AttnVarlen vl, const AttnDecode dc) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DV = Cfg::DV, KST = Cfg::KSTAGES, VST = Cfg::VSTAGES;
   static_assert(!(Cfg::VARLEN && Cfg::V_DN), "packed sequences take V as [tokens, heads, D]");
+  static_assert(!Cfg::DECODE || (Cfg::NWG == 1 && !Cfg::VARLEN && !Cfg::V_DN), "decode: one consumer warpgroup, V [keys, heads, D]");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u;
   const uint32_t sK = sQ + nqc * BM * 128, sV = sK + KST * Cfg::K_BYTES;
   const uint32_t qbar = sV + VST * Cfg::V_BYTES;
   const uint32_t kfull = qbar + 8, kempty = kfull + 8 * KST, vfull = kempty + 8 * KST, vempty = vfull + 8 * VST;
 
-  const int bh = blockIdx.z, q0 = blockIdx.x * BM, dv0 = blockIdx.y * DV;
+  // decode: blockIdx.x is the split, blockIdx.y the (token tile, head tile), blockIdx.z the (sequence, K/V head)
+  const int bh = blockIdx.z, q0 = Cfg::DECODE ? 0 : blockIdx.x * BM, dv0 = Cfg::DECODE ? 0 : blockIdx.y * DV;
   int kv_len = N;
   // packed sequences: first query and key token of the sequence, and the causal shift Lk - Lq (row r sees keys <= r + shift)
   int q_tok = 0, k_tok = 0, shift = 0;
+  // decode: sequence, K/V head, first query token of the tile (within the sequence), first query head, first KV tile
+  int seq = 0, kvh = 0, t0 = 0, h0 = 0, j0 = 0;
   if constexpr (Cfg::VARLEN) {
     const int b = bh / mask.H;
     q_tok = __ldg(vl.cu_q + b);
@@ -113,10 +136,30 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     k_tok = __ldg(vl.cu_k + b);
     kv_len = __ldg(vl.cu_k + b + 1) - k_tok;
     shift = kv_len - q_len;
+  } else if constexpr (Cfg::DECODE) {
+    const int h_kv = mask.H / dc.group;
+    seq = bh / h_kv;
+    kvh = bh % h_kv;
+    t0 = (blockIdx.y / dc.nhb) * dc.T;
+    h0 = kvh * dc.group + (blockIdx.y % dc.nhb) * dc.hb;
+    kv_len = min(max(__ldg(mask.seqlens + seq), 0), dc.pages_per_seq * dc.page_size);
+    shift = kv_len - dc.Lq;
   } else {
     if (mask.seqlens) kv_len = min(max(__ldg(mask.seqlens + bh / mask.H), 1), N);
   }
-  const int ntiles = attn_num_tiles<Cfg>(q0 + shift, kv_len, mask);
+  int ntiles;
+  if constexpr (Cfg::DECODE) {
+    int nt = (kv_len + BN - 1) / BN;
+    if (mask.causal) {  // the tile's last token sees keys <= its index + shift
+      const int last = min(t0 + dc.T, dc.Lq) - 1 + shift;
+      nt = min(nt, last < 0 ? 0 : last / BN + 1);
+    }
+    // split s of gridDim.x takes tiles [s * nt / splits, (s + 1) * nt / splits) of this sequence; it may take none
+    j0 = int((long long)blockIdx.x * nt / gridDim.x);
+    ntiles = int((long long)(blockIdx.x + 1) * nt / gridDim.x) - j0;
+  } else {
+    ntiles = attn_num_tiles<Cfg>(q0 + shift, kv_len, mask);
+  }
   const int wg = threadIdx.x / 128;
 
   if (threadIdx.x == 0) {
@@ -137,21 +180,46 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     if (threadIdx.x == 0) {
       // packed maps are (D, heads, tokens): coordinates (column, head, token) instead of (column, row, batch * head)
       const int head = bh % mask.H, kv_head = head / vl.group;
-      mbar_arrive_expect_tx(qbar, nqc * BM * 128);
+      // decode: the Q box is T tokens x hb heads; rows it reads past the sequence, the group or the tensor are computed
+      // and never stored (zero-filled past the tensor, which TMA still counts in full)
+      mbar_arrive_expect_tx(qbar, Cfg::DECODE ? nqc * dc.T * dc.hb * 128 : nqc * BM * 128);
       for (int c = 0; c < nqc; ++c) {
         if constexpr (Cfg::VARLEN) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, head, q_tok + q0, kPolicyEvictFirst);
+        else if constexpr (Cfg::DECODE) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, h0, seq * dc.Lq + t0, kPolicyEvictFirst);
         else tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, q0, bh, kPolicyEvictFirst);
       }
       int kc = 0;
       for (int j = 0; j < ntiles; ++j) {
+        // decode: cache row of each box of KV tile j0 + j (BN / box_rows boxes, one per page when pages are smaller
+        // than a tile).  A box past the sequence's last page reads outside the map, so the table is read only up to the
+        // length.
+        [[maybe_unused]] int crow[BN / 16];
+        if constexpr (Cfg::DECODE) {
+#pragma unroll
+          for (int i = 0; i < BN / 16; ++i) {
+            const int key = (j0 + j) * BN + i * dc.box_rows;
+            if (i * dc.box_rows >= BN) break;
+            if (!dc.table) crow[i] = seq * dc.page_size + key;
+            else if (key >= kv_len) crow[i] = dc.oob;
+            else crow[i] = __ldg(dc.table + size_t(seq) * dc.pages_per_seq + key / dc.page_size) * dc.page_size + key % dc.page_size;
+          }
+        }
         for (int c = 0; c < nqc; ++c, ++kc) {
           const int s = kc % KST;
           if (kc >= KST) mbar_wait(kempty + 8 * s, ((kc / KST) - 1) & 1);
           mbar_arrive_expect_tx(kfull + 8 * s, Cfg::K_BYTES);
-          if constexpr (Cfg::VARLEN)
+          if constexpr (Cfg::VARLEN) {
             tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
-          else
+          } else if constexpr (Cfg::DECODE) {
+#pragma unroll
+            for (int i = 0; i < BN / 16; ++i) {
+              if (i * dc.box_rows >= BN) break;
+              tma_load_3d(sK + s * Cfg::K_BYTES + i * dc.box_rows * 128, &tmK, kfull + 8 * s, c * 64, kvh, crow[i],
+                          kPolicyEvictNormal);
+            }
+          } else {
             tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, j * BN, bh, kPolicyEvictNormal);
+          }
         }
         const int s = j % VST;
         if (j >= VST) mbar_wait(vempty + 8 * s, ((j / VST) - 1) & 1);
@@ -164,10 +232,18 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
         } else {
 #pragma unroll
           for (int c = 0; c < DV / 64; ++c) {
-            if constexpr (Cfg::VARLEN)
+            if constexpr (Cfg::VARLEN) {
               tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
-            else
+            } else if constexpr (Cfg::DECODE) {
+#pragma unroll
+              for (int i = 0; i < BN / 16; ++i) {
+                if (i * dc.box_rows >= BN) break;
+                tma_load_3d(dst + c * BN * 128 + i * dc.box_rows * 128, &tmV, vfull + 8 * s, dv0 + c * 64, kvh, crow[i],
+                            kPolicyEvictNormal);
+              }
+            } else {
               tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, j * BN, bh, kPolicyEvictNormal);
+            }
           }
         }
       }
@@ -182,6 +258,12 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
   for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
+  // decode: causal diagonal of rows row0 and row0 + 8 (token t0 + r / hb)
+  [[maybe_unused]] int rdiag[2] = {0, 0};
+  if constexpr (Cfg::DECODE) {
+    rdiag[0] = t0 + row0 / dc.hb + shift;
+    rdiag[1] = t0 + (row0 + 8) / dc.hb + shift;
+  }
   mbar_wait(qbar, 0);
 
   int kc = 0;
@@ -212,8 +294,9 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
     // ---- masks: keys past the valid length, keys after the query row + shift (causal).  The shift is selected at
     // compile time rather than added as 0, which keeps the dense instantiations' machine code as it was.
-    const int k0 = j * BN;
-    if (k0 + BN > kv_len || (mask.causal && k0 + BN - 1 > (Cfg::VARLEN ? q0 + shift : q0) + cw * 64)) {
+    const int k0 = (Cfg::DECODE ? j0 + j : j) * BN;
+    if (k0 + BN > kv_len ||
+        (mask.causal && k0 + BN - 1 > (Cfg::DECODE ? t0 + shift : (Cfg::VARLEN ? q0 + shift : q0) + cw * 64))) {
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i)
 #pragma unroll
@@ -221,7 +304,8 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int key = k0 + 8 * i + 2 * (lane & 3) + e;
-            if (key >= kv_len || (mask.causal && key > (Cfg::VARLEN ? row0 + shift : row0) + 8 * h))
+            if (key >= kv_len ||
+                (mask.causal && key > (Cfg::DECODE ? rdiag[h] : (Cfg::VARLEN ? row0 + shift : row0) + 8 * h)))
               s_acc[4 * i + 2 * h + e] = -INFINITY;
           }
     }
@@ -263,6 +347,20 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     const int sv = j % VST;
     mbar_wait(vfull + 8 * sv, (j / VST) & 1);
     const uint32_t vb = sV + sv * Cfg::V_BYTES;
+    if constexpr (Cfg::DECODE) {
+      // the tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or
+      // Inf in V is NaN in the tensor core, so those V rows are zeroed here (K needs nothing: its scores became -inf)
+      if (k0 + BN > kv_len) {
+        const int r0 = kv_len - k0, words = (BN - r0) * 8;  // 16-byte words per 64-column chunk
+#pragma unroll
+        for (int c = 0; c < DV / 64; ++c)
+          for (int i = threadIdx.x & 127; i < words; i += 128)
+            asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + c * BN * 128 + r0 * 128 + i * 16), "r"(0)
+                         : "memory");
+        fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
+        named_bar_sync(1, 128);
+      }
+    }
     fence_regs<DV / 2>(o);
     wgmma_fence();
 #pragma unroll
@@ -283,7 +381,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   // ---- epilogue: O / l, clipped to N rows (packed: the sequence's rows and tokens [0, total_q)) and D columns.  Rows
   // that saw no key have l = 0 and store 0.
-  int q_len = N;
+  int q_len = Cfg::DECODE ? BM : N;
   if constexpr (Cfg::VARLEN) {  // reloaded rather than kept in registers through the main loop
     const int b = bh / mask.H;
     q_tok = vl.cu_q[b];
@@ -298,7 +396,24 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     const int r = row0 + 8 * h;
     if (r >= q_len) continue;
     size_t row_off;
-    if constexpr (Cfg::VARLEN) {
+    if constexpr (Cfg::DECODE) {
+      // row r is token t0 + r / hb and head h0 + r % hb; rows past the box, the sequence or the group are not stored
+      const int tt = r / dc.hb, hh = r % dc.hb;
+      if (tt >= dc.T || t0 + tt >= dc.Lq || h0 - kvh * dc.group + hh >= dc.group) continue;
+      const size_t row = (size_t(seq) * dc.Lq + t0 + tt) * size_t(mask.H) + h0 + hh;
+      if (gridDim.x > 1) {  // one split of several: O / l in fp32 and the base-2 log-sum-exp (-inf: no key seen)
+        float* dst = dc.part + (size_t(blockIdx.x) * size_t(dc.rows) + row) * size_t(D);
+#pragma unroll
+        for (int i = 0; i < DV / 8; ++i) {
+          const int c = 8 * i + 2 * (lane & 3);
+          if (c >= D) continue;
+          *reinterpret_cast<float2*>(dst + c) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+        }
+        if ((lane & 3) == 0) dc.lse[size_t(blockIdx.x) * size_t(dc.rows) + row] = t > 0.f ? m[h] + log2f(t) : -INFINITY;
+        continue;
+      }
+      row_off = row * size_t(D);
+    } else if constexpr (Cfg::VARLEN) {
       const long long tok = (long long)q_tok + r;
       if (tok < 0 || tok >= vl.total_q) continue;
       row_off = (size_t(tok) * mask.H + bh % mask.H) * size_t(D);
@@ -342,7 +457,7 @@ static int launch_attn(const void* Q, const void* K, const void* V, void* O, int
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
   dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
   kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask,
-                                        AttnVarlen());
+                                        AttnVarlen(), AttnDecode());
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -374,8 +489,149 @@ static int launch_attn_varlen(const void* Q, const void* K, const void* V, void*
   vl.group = int(H / H_kv);
   vl.total_q = int(total_q);
   dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask, vl);
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask, vl,
+                                        AttnDecode());
   B200K_CHECK_CUDA(cudaGetLastError());
+  return B200K_OK;
+}
+
+// KV-cache decode with several splits: O[row] = sum_s 2^(lse_s - max) part_s[row] / sum_s 2^(lse_s - max), summed in
+// split order, so the result does not depend on which split finished first.  A split with no key for the row has
+// lse = -inf and adds nothing; a row no split saw a key for is 0.  One thread per (row, column pair).
+template <int DT>
+__global__ void attn_combine_kernel(const float* __restrict__ part, const float* __restrict__ lse, void* O, long long rows,
+                                    int D, int splits) {
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x, pairs = D / 2;
+  if (i >= rows * pairs) return;
+  const long long row = i / pairs;
+  const int c = 2 * int(i % pairs);
+  float mx = -INFINITY;
+  for (int s = 0; s < splits; ++s) mx = fmaxf(mx, lse[s * rows + row]);
+  float x = 0.f, y = 0.f, den = 0.f;
+  if (mx != -INFINITY) {
+    for (int s = 0; s < splits; ++s) {
+      const float w = ex2(lse[s * rows + row] - mx);
+      const float2 p = *reinterpret_cast<const float2*>(part + (s * rows + row) * D + c);
+      x = fmaf(w, p.x, x);
+      y = fmaf(w, p.y, y);
+      den += w;
+    }
+  }
+  const float inv = den > 0.f ? 1.f / den : 0.f;
+  x *= inv;
+  y *= inv;
+  *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row * D + c) = pack_round<DT>(x, y);
+}
+
+// Launch geometry of KV-cache decode, shared by b200k_fa2_fwd_kvcache and its workspace query.  The 64 rows of a CTA
+// are T tokens x hb query heads of one K/V head's group of G; a group wider than 64 takes nhb head tiles.
+struct KvcacheGrid {
+  int hb = 1, T = 1, nhb = 1, splits = 1;
+  int64_t qtiles = 1;
+  size_t workspace = 0;
+};
+
+// The split rule.  ctas = B * H_kv * q tiles * head tiles CTAs each stream one K/V head of one sequence.  When they fill
+// 80 % of the SMs, one split.  Otherwise each sequence's KV tiles are split s ways, s at most 128 and at most one split
+// per two KV tiles of the capacity (max_seqlen_k); of those, the fewest splits whose grid fills its last wave of SMs
+// within 85 % of the best fill any allowed s reaches.  It depends on the shapes and the SM count only, never on the
+// lengths in the cache, so a captured graph keeps a valid grid while they grow.
+static int kvcache_splits(int64_t ctas, int64_t max_seqlen_k, int sm_count) {
+  if (ctas * 5 >= int64_t(sm_count) * 4) return 1;
+  const int64_t tiles = (max_seqlen_k + 127) / 128;
+  const int max_s = int(tiles / 2 < 1 ? 1 : (tiles / 2 > 128 ? 128 : tiles / 2));
+  auto fill = [&](int s) {
+    const int64_t n = ctas * s, waves = (n + sm_count - 1) / sm_count;
+    return double(n) / double(waves * sm_count);
+  };
+  double best = 0.0;
+  for (int s = 1; s <= max_s; ++s) best = fill(s) > best ? fill(s) : best;
+  for (int s = 1; s <= max_s; ++s)
+    if (fill(s) >= 0.85 * best) return s;
+  return 1;
+}
+
+static KvcacheGrid kvcache_grid(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D, int64_t max_seqlen_k,
+                                int sm_count) {
+  KvcacheGrid g;
+  const int64_t G = H / H_kv;
+  g.hb = int(G < 64 ? G : 64);
+  g.T = 64 / g.hb;
+  g.nhb = int((G + g.hb - 1) / g.hb);
+  g.qtiles = (Lq + g.T - 1) / g.T;
+  g.splits = kvcache_splits(B * H_kv * g.qtiles * g.nhb, max_seqlen_k, sm_count);
+  if (g.splits > 1) g.workspace = size_t(g.splits) * size_t(B * Lq * H) * size_t(D + 1) * sizeof(float);
+  return g;
+}
+
+static int kvcache_check_headdim(const char* fn, int64_t D) {
+  if (D != 32 && D != 64 && D != 96 && D != 128)
+    return set_error(B200K_EHEADDIM, "headdim not support! (%s: D=%lld, supported 32/64/96/128)", fn, (long long)D);
+  return B200K_OK;
+}
+
+// Shape checks shared by both decode entry points (before any CUDA call).
+static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t max_seqlen_k) {
+  if (B < 1 || Lq < 1 || H < 1 || H_kv < 1 || max_seqlen_k < 1 || H % H_kv != 0 || H > INT32_MAX)
+    return set_error(B200K_ESHAPE, "%s: need B, Lq, H, H_kv, key capacity >= 1 and H %% H_kv == 0 (got B=%lld Lq=%lld "
+                     "H=%lld H_kv=%lld capacity=%lld)", fn, (long long)B, (long long)Lq, (long long)H, (long long)H_kv,
+                     (long long)max_seqlen_k);
+  if (max_seqlen_k > INT32_MAX || B > INT32_MAX / Lq)
+    return set_error(B200K_ESHAPE, "%s: B * Lq and the key capacity must be <= 2^31 - 1", fn);
+  const int64_t G = H / H_kv, hb = G < 64 ? G : 64, tiles = ((Lq + 64 / hb - 1) / (64 / hb)) * ((G + hb - 1) / hb);
+  if (tiles > 65535 || B * H_kv > 65535)
+    return set_error(B200K_ESHAPE, "%s: %lld (token, head) tiles and %lld (sequence, K/V head) pairs, the grid allows 65535 "
+                     "each", fn, (long long)tiles, (long long)(B * H_kv));
+  return B200K_OK;
+}
+
+template <class Cfg>
+static int launch_attn_kvcache(const void* Q, const void* Kc, const void* Vc, void* O, const int* seqlens,
+                               const int* table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                               int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int causal,
+                               const KvcacheGrid& g, void* workspace, cudaStream_t s, const DeviceInfo& di) {
+  const int nqc = int((D + 63) / 64);
+  const int smem = Cfg::smem_bytes(nqc);
+  if (smem > di.max_smem_optin)
+    return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
+  // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
+  const int box_rows = table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
+  CUtensorMap tmQ, tmK, tmV;
+  int rc;
+  if ((rc = attn_tmap(&tmQ, Q, B * Lq, H, D, g.T, g.hb))) return rc;
+  if ((rc = attn_tmap(&tmK, Kc, num_pages * page_size, H_kv, D, box_rows, 1))) return rc;
+  if ((rc = attn_tmap(&tmV, Vc, num_pages * page_size, H_kv, D, box_rows, 1))) return rc;
+  auto kern = attn_fwd_wgmma_kernel<Cfg>;
+  if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
+  AttnMask mask;
+  mask.seqlens = seqlens;
+  mask.H = int(H);
+  mask.causal = causal ? 1 : 0;
+  AttnDecode dc;
+  dc.table = table;
+  dc.rows = B * Lq * H;
+  dc.Lq = int(Lq);
+  dc.group = int(H / H_kv);
+  dc.hb = g.hb;
+  dc.T = g.T;
+  dc.nhb = g.nhb;
+  dc.page_size = int(page_size);
+  dc.pages_per_seq = int(pages_per_seq);
+  dc.box_rows = box_rows;
+  dc.oob = int(num_pages * page_size);
+  if (g.splits > 1) {
+    dc.part = static_cast<float*>(workspace);
+    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
+  }
+  dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask,
+                                        AttnVarlen(), dc);
+  B200K_CHECK_CUDA(cudaGetLastError());
+  if (g.splits > 1) {
+    const long long work = dc.rows * (D / 2);
+    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(dc.part, dc.lse, O, dc.rows, int(D), g.splits);
+    B200K_CHECK_CUDA(cudaGetLastError());
+  }
   return B200K_OK;
 }
 
@@ -475,6 +731,61 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
   if (dtype == B200K_BF16)
     return narrow ? run(AttnCfg<1, 64, 2, 128, false, true>()) : run(AttnCfg<1, 128, 2, 128, false, true>());
   return narrow ? run(AttnCfg<0, 64, 2, 128, false, true>()) : run(AttnCfg<0, 128, 2, 128, false, true>());
+}
+
+extern "C" int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                                     int64_t max_seqlen_k, size_t* bytes) {
+  using namespace b200k;
+  if (!bytes) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache_workspace_bytes: null pointer");
+  int rc = kvcache_check_headdim("b200k_fa2_fwd_kvcache_workspace_bytes", D);
+  if (rc || (rc = kvcache_check("b200k_fa2_fwd_kvcache_workspace_bytes", B, Lq, H, H_kv, max_seqlen_k))) return rc;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  *bytes = kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count).workspace;
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const void* V_cache, void* O,
+                                     const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq, int64_t H,
+                                     int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                     float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  using namespace b200k;
+  if (!Q || !K_cache || !V_cache || !O || !cache_seqlens) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: null pointer");
+  if (dtype != B200K_F16 && dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "b200k_fa2_fwd_kvcache: dtype %d not supported (f16, bf16)", dtype);
+  int rc = kvcache_check_headdim("b200k_fa2_fwd_kvcache", D);
+  if (rc) return rc;
+  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)",
+                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
+  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: num_pages * page_size and pages_per_seq * page_size must be "
+                     "<= 2^31 - 1");
+  if ((rc = kvcache_check("b200k_fa2_fwd_kvcache", B, Lq, H, H_kv, pages_per_seq * page_size))) return rc;
+  if (block_table && page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: page_size %lld (16, 32, 64 or a multiple of 128)",
+                     (long long)page_size);
+  if (!block_table && (num_pages != B || pages_per_seq != 1))
+    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: a contiguous cache (no block table) is num_pages = B pages of "
+                     "page_size = S keys, pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)",
+                     (long long)num_pages, (long long)pages_per_seq);
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
+  if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
+    return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: %zu workspace bytes needed, %zu given", g.workspace,
+                     workspace ? workspace_bytes : size_t(0));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  auto run = [&](auto cfg) {
+    return launch_attn_kvcache<decltype(cfg)>(Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D,
+                                              num_pages, page_size, pages_per_seq, scale, causal, g, workspace, s, di);
+  };
+  const bool narrow = D <= 64;  // O columns: 64 for D = 32 / 64, 128 for D = 96 / 128
+  if (dtype == B200K_BF16)
+    return narrow ? run(AttnCfg<1, 64, 1, 128, false, false, true>()) : run(AttnCfg<1, 128, 1, 128, false, false, true>());
+  return narrow ? run(AttnCfg<0, 64, 1, 128, false, false, true>()) : run(AttnCfg<0, 128, 1, 128, false, false, true>());
 }
 
 extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,

@@ -127,6 +127,40 @@ int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* O, int64_t 
 int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
                          const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k,
                          int64_t H, int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* stream);
+/* b200k_fa2_fwd_kvcache — attention of the newest Lq query tokens of each sequence against its KV cache (decode,
+ * speculative decoding): the forward of flash-attn's flash_attn_with_kvcache, without its append / rotary step.  The
+ * same FA-2 kernel in a decode mode: one CTA per (sequence, K/V head) reads each K/V byte once for all the query heads
+ * of its group, and a long cache is split across CTAs (the split count is chosen by the library from the shapes and the
+ * SM count) and merged by a second kernel in a fixed order, so the result is deterministic.
+ *   Q, O           [B, Lq, H, D] contiguous; dtype B200K_F16 or B200K_BF16; D in {32, 64, 96, 128}; scale <= 0 -> 1/sqrt(D)
+ *   K_cache, V_cache [num_pages, page_size, H_kv, D] contiguous, same dtype; H % H_kv == 0, query head h reads K/V head
+ *                  h / (H / H_kv)
+ *   block_table    NULL: contiguous cache [B, S, H_kv, D], passed as num_pages = B, page_size = S, pages_per_seq = 1
+ *                  (sequence b owns page b).  Otherwise int32 device array [B, pages_per_seq]: key j of sequence b is
+ *                  slot j % page_size of page block_table[b * pages_per_seq + j / page_size]; page_size is 16, 32, 64
+ *                  or a multiple of 128.  Entries past ceil(Lk_b / page_size) are never read
+ *   cache_seqlens  int32 device array [B]: sequence b has Lk_b keys, 0 <= Lk_b <= pages_per_seq * page_size
+ *   causal         query token t of sequence b sees key j iff j <= t + Lk_b - Lq (the new tokens are the last Lq keys)
+ *   zero rows      a row that sees no key is written as 0
+ *   isolation      cache slots at or past Lk_b, and pages a sequence's table does not list, never affect O, whatever
+ *                  they hold (NaN and Inf included): caches are allocated uninitialised and pages are recycled
+ *   workspace      >= the bytes b200k_fa2_fwd_kvcache_workspace_bytes reports for the same shapes (may be NULL when
+ *                  that is 0)
+ *   no sync        nothing is read back to the host, so the call can be captured in a CUDA graph and replayed while
+ *                  cache_seqlens and block_table change
+ * Errors before any CUDA call: B200K_EARG (null pointer), B200K_EDTYPE, B200K_EHEADDIM, B200K_ESHAPE (counts < 1,
+ * H % H_kv, page_size, num_pages * page_size or B * Lq > INT32_MAX, grid limits: at most 65535 (token, head) tiles of
+ * 64 rows per K/V head and B * H_kv <= 65535; without a table num_pages must be B and pages_per_seq 1).  After the device
+ * query (the split count needs the SM count): B200K_EARG when workspace_bytes is below what the workspace function
+ * reports. */
+int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const void* V_cache, void* O, const int* cache_seqlens,
+                          const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                          int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace the call above needs for these shapes (max_seqlen_k = pages_per_seq * page_size); 0 when it runs
+ * unsplit.  Depends on the current device's SM count, so it can fail like any device query. */
+int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                          int64_t max_seqlen_k, size_t* bytes);
 
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
