@@ -431,67 +431,66 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   }
 }
 
-// Tensor map over a contiguous 16-bit [d2, d1, d0] array, box [box2, box1, 64]: each box row is one 128-byte swizzle row.
-static int attn_tmap(CUtensorMap* m, const void* p, uint64_t d2, uint64_t d1, uint64_t d0, uint32_t box2, uint32_t box1) {
-  const uint64_t dims[3] = {d0, d1, d2}, strides[2] = {2 * d0, 2 * d0 * d1};
-  const uint32_t box[3] = {64, box1, box2};
-  return make_tmap(m, p, 2, 3, dims, strides, box);
+// One contiguous 16-bit [d2, d1, d0] tensor read through boxes [box2, box1, 64]: each box row is one 128-byte swizzle row.
+struct AttnTensor {
+  const void* p;
+  int64_t d2, d1, d0;
+  int box2, box1;
+};
+
+static int attn_tmap(CUtensorMap* m, const AttnTensor& t) {
+  const uint64_t dims[3] = {uint64_t(t.d0), uint64_t(t.d1), uint64_t(t.d2)}, strides[2] = {2 * dims[0], 2 * dims[0] * dims[1]};
+  const uint32_t box[3] = {64, uint32_t(t.box1), uint32_t(t.box2)};
+  return make_tmap(m, t.p, 2, 3, dims, strides, box);
 }
 
+// The launch every mode shares: the shared-memory check, Q / K / V as tensor maps, then the kernel on `grid`.
+// scale <= 0 means 1 / sqrt(D).
 template <class Cfg>
-static int launch_attn(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
-                       float scale, const AttnMask& mask, cudaStream_t s, const DeviceInfo& di) {
-  const uint64_t BH = uint64_t(B) * uint64_t(H);
+static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t N, int64_t D, float scale,
+                       const AttnMask& mask, const AttnVarlen& vl, const AttnDecode& dc, cudaStream_t s, const DeviceInfo& di) {
   const int nqc = int((D + 63) / 64);
   const int smem = Cfg::smem_bytes(nqc);
   if (smem > di.max_smem_optin)
     return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
-  CUtensorMap tmQ, tmK, tmV;
+  CUtensorMap tm[3];
   int rc;
-  if ((rc = attn_tmap(&tmQ, Q, BH, N, D, 1, Cfg::BM))) return rc;
-  if ((rc = attn_tmap(&tmK, K, BH, N, D, 1, Cfg::BN))) return rc;
-  if (Cfg::V_DN) rc = attn_tmap(&tmV, V, BH, D, N, 1, Cfg::DV);
-  else rc = attn_tmap(&tmV, V, BH, N, D, 1, Cfg::BN);
-  if (rc) return rc;
+  for (int i = 0; i < 3; ++i)
+    if ((rc = attn_tmap(&tm[i], qkv[i]))) return rc;
   auto kern = attn_fwd_wgmma_kernel<Cfg>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
-  dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask,
-                                        AttnVarlen(), AttnDecode());
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tm[0], tm[1], tm[2], O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask, vl, dc);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
 
-// Packed sequences: one 3-D map per tensor over (D, heads, tokens), box (64, 1, BM or BN), so shared memory holds the
-// same 128-byte swizzled rows as the dense maps and only the coordinates differ.  Grid: ceil(max_seqlen_q / BM) query
-// tiles x B * H; CTAs past their sequence's length return at once.
+// Dense [B, H, N, D]: one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).
 template <class Cfg>
-static int launch_attn_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_q, const int* cu_k,
-                              int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv,
-                              int64_t D, float scale, int causal, cudaStream_t s, const DeviceInfo& di) {
-  const int nqc = int((D + 63) / 64);
-  const int smem = Cfg::smem_bytes(nqc);
-  if (smem > di.max_smem_optin)
-    return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = attn_tmap(&tmQ, Q, total_q, H, D, Cfg::BM, 1))) return rc;
-  if ((rc = attn_tmap(&tmK, K, total_k, H_kv, D, Cfg::BN, 1))) return rc;
-  if ((rc = attn_tmap(&tmV, V, total_k, H_kv, D, Cfg::BN, 1))) return rc;
-  auto kern = attn_fwd_wgmma_kernel<Cfg>;
-  if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
-  AttnMask mask;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  AttnVarlen vl;
-  vl.cu_q = cu_q;
-  vl.cu_k = cu_k;
-  vl.group = int(H / H_kv);
-  vl.total_q = int(total_q);
-  dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask, vl,
-                                        AttnDecode());
-  B200K_CHECK_CUDA(cudaGetLastError());
+static int launch_dense(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
+                        float scale, const AttnMask& mask, cudaStream_t s, const DeviceInfo& di) {
+  const int64_t BH = B * H;
+  AttnTensor v = {V, BH, N, D, 1, Cfg::BN};
+  if (Cfg::V_DN) v = {V, BH, D, N, 1, Cfg::DV};
+  const AttnTensor qkv[3] = {{Q, BH, N, D, 1, Cfg::BM}, {K, BH, N, D, 1, Cfg::BN}, v};
+  const dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
+  return launch_attn<Cfg>(qkv, grid, O, N, D, scale, mask, AttnVarlen(), AttnDecode(), s, di);
+}
+
+// The D <= 128 configurations: BN = 128 keys per tile; O columns DV = 64 for D = 32 / 64, 128 for D = 96 / 128.  V
+// stored [D, N] is built for fp16 only.
+template <int NWG, bool V_DN, bool VARLEN, bool DECODE, class Run>
+static int run_attn_cfg(int dtype, int64_t D, Run run) {
+  const bool narrow = D <= 64;
+  if (dtype != B200K_BF16)
+    return narrow ? run(AttnCfg<0, 64, NWG, 128, V_DN, VARLEN, DECODE>()) : run(AttnCfg<0, 128, NWG, 128, V_DN, VARLEN, DECODE>());
+  if constexpr (V_DN) return set_error(B200K_EARG, "attention: the [B,H,D,N] V layout is built for fp16 only");
+  else return narrow ? run(AttnCfg<1, 64, NWG, 128, false, VARLEN, DECODE>()) : run(AttnCfg<1, 128, NWG, 128, false, VARLEN, DECODE>());
+}
+
+static int check_headdim(const char* fn, int64_t D) {
+  if (D != 32 && D != 64 && D != 96 && D != 128)
+    return set_error(B200K_EHEADDIM, "headdim not support! (%s: D=%lld, supported 32/64/96/128)", fn, (long long)D);
   return B200K_OK;
 }
 
@@ -564,12 +563,6 @@ static KvcacheGrid kvcache_grid(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, 
   return g;
 }
 
-static int kvcache_check_headdim(const char* fn, int64_t D) {
-  if (D != 32 && D != 64 && D != 96 && D != 128)
-    return set_error(B200K_EHEADDIM, "headdim not support! (%s: D=%lld, supported 32/64/96/128)", fn, (long long)D);
-  return B200K_OK;
-}
-
 // Shape checks shared by both decode entry points (before any CUDA call).
 static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t max_seqlen_k) {
   if (B < 1 || Lq < 1 || H < 1 || H_kv < 1 || max_seqlen_k < 1 || H % H_kv != 0 || H > INT32_MAX)
@@ -585,56 +578,6 @@ static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64
   return B200K_OK;
 }
 
-template <class Cfg>
-static int launch_attn_kvcache(const void* Q, const void* Kc, const void* Vc, void* O, const int* seqlens,
-                               const int* table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
-                               int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int causal,
-                               const KvcacheGrid& g, void* workspace, cudaStream_t s, const DeviceInfo& di) {
-  const int nqc = int((D + 63) / 64);
-  const int smem = Cfg::smem_bytes(nqc);
-  if (smem > di.max_smem_optin)
-    return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
-  // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
-  const int box_rows = table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
-  CUtensorMap tmQ, tmK, tmV;
-  int rc;
-  if ((rc = attn_tmap(&tmQ, Q, B * Lq, H, D, g.T, g.hb))) return rc;
-  if ((rc = attn_tmap(&tmK, Kc, num_pages * page_size, H_kv, D, box_rows, 1))) return rc;
-  if ((rc = attn_tmap(&tmV, Vc, num_pages * page_size, H_kv, D, box_rows, 1))) return rc;
-  auto kern = attn_fwd_wgmma_kernel<Cfg>;
-  if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
-  AttnMask mask;
-  mask.seqlens = seqlens;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  AttnDecode dc;
-  dc.table = table;
-  dc.rows = B * Lq * H;
-  dc.Lq = int(Lq);
-  dc.group = int(H / H_kv);
-  dc.hb = g.hb;
-  dc.T = g.T;
-  dc.nhb = g.nhb;
-  dc.page_size = int(page_size);
-  dc.pages_per_seq = int(pages_per_seq);
-  dc.box_rows = box_rows;
-  dc.oob = int(num_pages * page_size);
-  if (g.splits > 1) {
-    dc.part = static_cast<float*>(workspace);
-    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
-  }
-  dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tmQ, tmK, tmV, O, 0, int(D), nqc, scale * 1.4426950408889634f, mask,
-                                        AttnVarlen(), dc);
-  B200K_CHECK_CUDA(cudaGetLastError());
-  if (g.splits > 1) {
-    const long long work = dc.rows * (D / 2);
-    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(dc.part, dc.lse, O, dc.rows, int(D), g.splits);
-    B200K_CHECK_CUDA(cudaGetLastError());
-  }
-  return B200K_OK;
-}
-
 // Large head dims: O in column slices of DV = 192 or 256 (as few slices as possible, each a whole number of 64-column
 // chunks).  DV = 192 runs two consumer warpgroups when Q (128 rows) fits in shared memory next to the K and V rings;
 // DV = 256 needs more registers than a 384-thread block can give each thread (168), so it runs one.
@@ -644,9 +587,9 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
   if constexpr (DV == 192) {
     using Two = AttnCfg<0, DV, 2, 64, false>;
     if (Two::smem_bytes(int((D + 63) / 64)) <= di.max_smem_optin)
-      return launch_attn<Two>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
+      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
   }
-  return launch_attn<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
+  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
 }
 
 }  // namespace b200k
@@ -669,30 +612,20 @@ extern "C" int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* 
   if (B < 1 || H < 1 || N < 1 || N > INT32_MAX || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_f16: need B,H,N >= 1 and B*H <= 65535 (got B=%lld H=%lld N=%lld)",
                      (long long)B, (long long)H, (long long)N);
-  if (D != 32 && D != 64 && D != 96 && D != 128)
-    return set_error(B200K_EHEADDIM, "headdim not support! (b200k_fa2_fwd_f16: D=%lld, supported 32/64/96/128)",
-                     (long long)D);
+  int rc = check_headdim("b200k_fa2_fwd_f16", D);
+  if (rc) return rc;
   if (v_is_dn && (N % 8))
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd: V stored [B,H,D,N] needs N %% 8 == 0 (16-byte rows), got N=%lld",
                      (long long)N);
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
   DeviceInfo di;
-  int rc = get_device_info(&di);
-  if (rc) return rc;
+  if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   AttnMask mask;
   mask.seqlens = seqlens_k;
   mask.H = int(H);
   mask.causal = causal ? 1 : 0;
-  const bool narrow = D <= 64;  // O columns: 64 for D = 32 / 64, 128 for D = 96 / 128
-  if (dtype == B200K_BF16)
-    return narrow ? launch_attn<AttnCfg<1, 64, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di)
-                  : launch_attn<AttnCfg<1, 128, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di);
-  if (v_is_dn)
-    return narrow ? launch_attn<AttnCfg<0, 64, 2, 128, true>>(Q, K, V, O, B, H, N, D, scale, mask, s, di)
-                  : launch_attn<AttnCfg<0, 128, 2, 128, true>>(Q, K, V, O, B, H, N, D, scale, mask, s, di);
-  return narrow ? launch_attn<AttnCfg<0, 64, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di)
-                : launch_attn<AttnCfg<0, 128, 2, 128, false>>(Q, K, V, O, B, H, N, D, scale, mask, s, di);
+  auto run = [&](auto cfg) { return launch_dense<decltype(cfg)>(Q, K, V, O, B, H, N, D, scale, mask, s, di); };
+  return v_is_dn ? run_attn_cfg<2, true, false, false>(dtype, D, run) : run_attn_cfg<2, false, false, false>(dtype, D, run);
 }
 
 extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
@@ -704,9 +637,8 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
     return set_error(B200K_EARG, "b200k_fa2_fwd_varlen: null pointer");
   if (dtype != B200K_F16 && dtype != B200K_BF16)
     return set_error(B200K_EDTYPE, "b200k_fa2_fwd_varlen: dtype %d not supported (f16, bf16)", dtype);
-  if (D != 32 && D != 64 && D != 96 && D != 128)
-    return set_error(B200K_EHEADDIM, "headdim not support! (b200k_fa2_fwd_varlen: D=%lld, supported 32/64/96/128)",
-                     (long long)D);
+  int rc = check_headdim("b200k_fa2_fwd_varlen", D);
+  if (rc) return rc;
   if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)",
                      (long long)B, (long long)H, (long long)H_kv);
@@ -718,26 +650,30 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
   if (B > 65535 || H > 65535 || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: B * H = %lld CTAs per query tile, the grid allows 65535",
                      (long long)B * (long long)H);
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
   DeviceInfo di;
-  int rc = get_device_info(&di);
-  if (rc) return rc;
+  if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  auto run = [&](auto cfg) {
-    return launch_attn_varlen<decltype(cfg)>(Q, K, V, O, cu_seqlens_q, cu_seqlens_k, B, max_seqlen_q, total_q, total_k,
-                                             H, H_kv, D, scale, causal, s, di);
-  };
-  const bool narrow = D <= 64;  // O columns: 64 for D = 32 / 64, 128 for D = 96 / 128
-  if (dtype == B200K_BF16)
-    return narrow ? run(AttnCfg<1, 64, 2, 128, false, true>()) : run(AttnCfg<1, 128, 2, 128, false, true>());
-  return narrow ? run(AttnCfg<0, 64, 2, 128, false, true>()) : run(AttnCfg<0, 128, 2, 128, false, true>());
+  AttnMask mask;
+  mask.H = int(H);
+  mask.causal = causal ? 1 : 0;
+  AttnVarlen vl;
+  vl.cu_q = cu_seqlens_q;
+  vl.cu_k = cu_seqlens_k;
+  vl.group = int(H / H_kv);
+  vl.total_q = int(total_q);
+  return run_attn_cfg<2, false, true, false>(dtype, D, [&](auto cfg) {
+    using Cfg = decltype(cfg);
+    const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1}, {K, total_k, H_kv, D, Cfg::BN, 1}, {V, total_k, H_kv, D, Cfg::BN, 1}};
+    const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
+    return launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, vl, AttnDecode(), s, di);
+  });
 }
 
 extern "C" int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                                      int64_t max_seqlen_k, size_t* bytes) {
   using namespace b200k;
   if (!bytes) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache_workspace_bytes: null pointer");
-  int rc = kvcache_check_headdim("b200k_fa2_fwd_kvcache_workspace_bytes", D);
+  int rc = check_headdim("b200k_fa2_fwd_kvcache_workspace_bytes", D);
   if (rc || (rc = kvcache_check("b200k_fa2_fwd_kvcache_workspace_bytes", B, Lq, H, H_kv, max_seqlen_k))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
@@ -754,7 +690,7 @@ extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const v
   if (!Q || !K_cache || !V_cache || !O || !cache_seqlens) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: null pointer");
   if (dtype != B200K_F16 && dtype != B200K_BF16)
     return set_error(B200K_EDTYPE, "b200k_fa2_fwd_kvcache: dtype %d not supported (f16, bf16)", dtype);
-  int rc = kvcache_check_headdim("b200k_fa2_fwd_kvcache", D);
+  int rc = check_headdim("b200k_fa2_fwd_kvcache", D);
   if (rc) return rc;
   if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)",
@@ -770,7 +706,6 @@ extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const v
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: a contiguous cache (no block table) is num_pages = B pages of "
                      "page_size = S keys, pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)",
                      (long long)num_pages, (long long)pages_per_seq);
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
@@ -778,14 +713,41 @@ extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const v
     return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: %zu workspace bytes needed, %zu given", g.workspace,
                      workspace ? workspace_bytes : size_t(0));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  auto run = [&](auto cfg) {
-    return launch_attn_kvcache<decltype(cfg)>(Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D,
-                                              num_pages, page_size, pages_per_seq, scale, causal, g, workspace, s, di);
-  };
-  const bool narrow = D <= 64;  // O columns: 64 for D = 32 / 64, 128 for D = 96 / 128
-  if (dtype == B200K_BF16)
-    return narrow ? run(AttnCfg<1, 64, 1, 128, false, false, true>()) : run(AttnCfg<1, 128, 1, 128, false, false, true>());
-  return narrow ? run(AttnCfg<0, 64, 1, 128, false, false, true>()) : run(AttnCfg<0, 128, 1, 128, false, false, true>());
+  AttnMask mask;
+  mask.seqlens = cache_seqlens;
+  mask.H = int(H);
+  mask.causal = causal ? 1 : 0;
+  AttnDecode dc;
+  dc.table = block_table;
+  dc.rows = B * Lq * H;
+  dc.Lq = int(Lq);
+  dc.group = int(H / H_kv);
+  dc.hb = g.hb;
+  dc.T = g.T;
+  dc.nhb = g.nhb;
+  dc.page_size = int(page_size);
+  dc.pages_per_seq = int(pages_per_seq);
+  dc.oob = int(num_pages * page_size);
+  if (g.splits > 1) {
+    dc.part = static_cast<float*>(workspace);
+    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
+  }
+  return run_attn_cfg<1, false, false, true>(dtype, D, [&](auto cfg) {
+    using Cfg = decltype(cfg);
+    // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
+    AttnDecode d = dc;
+    d.box_rows = block_table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
+    const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
+                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
+                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
+    const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
+    const int launched = launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, AttnVarlen(), d, s, di);
+    if (launched || g.splits == 1) return launched;
+    const long long work = d.rows * (D / 2);
+    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
+    B200K_CHECK_CUDA(cudaGetLastError());
+    return B200K_OK;
+  });
 }
 
 extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,
@@ -798,7 +760,6 @@ extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, v
     return set_error(B200K_EHEADDIM, "headdim not support! (b200k_ffpa_fwd_f16: D=%lld; supported 32 .. 1024 step 32)", (long long)D);
   if (B < 1 || H < 1 || N < 1 || N > INT32_MAX || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_ffpa_fwd_f16: need B,H,N >= 1 and B*H <= 65535");
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
   DeviceInfo di;
   int rc = get_device_info(&di);
   if (rc) return rc;
