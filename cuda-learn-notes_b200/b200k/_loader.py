@@ -65,6 +65,9 @@ _SIGS = {
     "b200k_fa2_fwd_varlen": (c_int, [c_void_p] * 6 + [c_int64] * 7 + [c_float, c_int, c_int, c_void_p]),
     "b200k_fa2_fwd_kvcache": (c_int, [c_void_p] * 6 + [c_int64] * 8 + [c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "b200k_fa2_fwd_kvcache_workspace_bytes": (c_int, [c_int64] * 6 + [ctypes.POINTER(c_size_t)]),
+    "b200k_fa2_fwd_kvcache_append": (c_int, [c_void_p] * 8 + [c_int64] + [c_void_p] * 2 + [c_int64] * 2 + [c_int]
+                                     + [c_int64] * 8 + [c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
+    "b200k_fa2_fwd_kvcache_append_workspace_bytes": (c_int, [c_int64] * 6 + [c_int, ctypes.POINTER(c_size_t)]),
     "b200k_elementwise_add": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "b200k_reduce_workspace_bytes": (c_size_t, []),
     "b200k_block_all_reduce_sum": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),

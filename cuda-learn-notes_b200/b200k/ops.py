@@ -226,15 +226,34 @@ def fa2_fwd_kvcache_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, 
     return n.value
 
 
+def fa2_fwd_kvcache_append_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int,
+                                           rotary: bool) -> int:
+    """Workspace bytes :func:`fa2_fwd_kvcache` needs with ``k`` / ``v`` for these shapes; queries the device."""
+    n = ctypes.c_size_t(0)
+    L.check(_lib.b200k_fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, max_seqlen_k, 1 if rotary else 0,
+                                                              ctypes.byref(n)))
+    return n.value
+
+
 def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_table: Optional[torch.Tensor] = None,
-                    scale: Optional[float] = None, causal: bool = False) -> None:
-    """Attention of the newest Lq query tokens of each sequence against its KV cache (the forward of flash-attn's
-    ``flash_attn_with_kvcache``, without appending K/V or rotary).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
+                    scale: Optional[float] = None, causal: bool = False, *, k: Optional[torch.Tensor] = None,
+                    v: Optional[torch.Tensor] = None, rotary_cos: Optional[torch.Tensor] = None,
+                    rotary_sin: Optional[torch.Tensor] = None, rotary_interleaved: bool = True) -> None:
+    """Attention of the newest Lq query tokens of each sequence against its KV cache (flash-attn's
+    ``flash_attn_with_kvcache``).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
     [B, S, H_kv, D] without ``block_table``, or [num_pages, page_size, H_kv, D] with an int32 ``block_table``
     [B, pages_per_seq] (key j of sequence b is slot j % page_size of page block_table[b, j // page_size]).
     ``cache_seqlens``: int32 [B] key counts on the device.  ``causal``: token t sees keys <= t + Lk - Lq.  H % H_kv == 0
     (query head h reads K/V head h // (H // H_kv)).  Nothing is read back to the host, so the call can be captured in a
-    CUDA graph; the split workspace is allocated per call on the current stream."""
+    CUDA graph; the workspace is allocated per call on the current stream.
+
+    Append: ``k``, ``v`` [B, L_new, H_kv, D] are written into the caches in place at positions
+    cache_seqlens[b] + i (through the table when paged), and the attention runs over cache_seqlens[b] + L_new keys.
+    ``cache_seqlens`` itself is not updated; the caller adds L_new afterwards.  ``rotary_cos`` / ``rotary_sin``
+    [rotary_seqlen, rotary_dim / 2] in q's dtype (rotary_dim a multiple of 16, at most D; rotary_seqlen at least the
+    capacity) rotate the first rotary_dim columns of k and q: new key i at position cache_seqlens[b] + i, query token t
+    at cache_seqlens[b] + t when causal and at cache_seqlens[b] when not.  ``rotary_interleaved`` pairs columns
+    (2j, 2j + 1); otherwise (j, j + rotary_dim / 2), GPT-NeoX style.  q is not modified."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     for t in (q, k_cache, v_cache, o):
         _check_dtype(t, dt)
@@ -263,6 +282,37 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
             raise RuntimeError("Tensor size mismatch!")
         pages_per_seq = block_table.size(1)
         tensors.append(block_table)
+    rotary = rotary_cos is not None or rotary_sin is not None
+    if k is not None or v is not None or rotary:
+        if k is None or v is None:
+            raise RuntimeError("b200k: append needs both k and v (rotary applies to appended keys)")
+        if (rotary_cos is None) != (rotary_sin is None):
+            raise RuntimeError("b200k: rotary needs both rotary_cos and rotary_sin")
+        for t in (k, v):
+            _check_dtype(t, dt)
+        if k.dim() != 4 or k.size(0) != B or tuple(k.shape[2:]) != (H_kv, D) or tuple(v.shape) != tuple(k.shape):
+            raise RuntimeError("Tensor size mismatch!")
+        tensors += [k, v]
+        cos = sin = None
+        if rotary:
+            _check_dtype(rotary_cos, dt)
+            _check_dtype(rotary_sin, dt)
+            if rotary_cos.dim() != 2 or tuple(rotary_sin.shape) != tuple(rotary_cos.shape):
+                raise RuntimeError("Tensor size mismatch!")
+            cos, sin = rotary_cos, rotary_sin
+            tensors += [cos, sin]
+        _check_cuda_contig(*tensors)
+        with _DeviceGuard(q):
+            nbytes = fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, rotary)
+            ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+            L.check(_lib.b200k_fa2_fwd_kvcache_append(
+                q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), cache_seqlens.data_ptr(),
+                block_table.data_ptr() if block_table is not None else None, k.data_ptr(), v.data_ptr(), k.size(1),
+                cos.data_ptr() if rotary else None, sin.data_ptr() if rotary else None,
+                cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0, 1 if rotary_interleaved else 0,
+                B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0,
+                _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr(), nbytes, _stream(q)))
+        return
     _check_cuda_contig(*tensors)
     with _DeviceGuard(q):
         nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size)

@@ -16,10 +16,12 @@
 // maps, the TMA coordinates, the per-CTA key length, the causal diagonal and the epilogue's addressing differ.
 // KV-cache decode (AttnCfg::DECODE) runs it too: a CTA owns the query rows of one K/V head (tokens x grouped heads packed
 // into one 64-row tile), reads K / V through a page table, takes one split of the sequence's KV tiles, and writes either
-// O or fp32 partials that attn_combine_kernel merges.
+// O or fp32 partials that attn_combine_kernel merges.  kvcache_append_kernel, launched before it, writes new K / V rows
+// (K and Q optionally rotated) into the caches and the lengths the decode kernel reads.
 #include "abi_common.cuh"
 #include "ptx.cuh"
 
+#include <climits>
 #include <cmath>
 
 namespace b200k {
@@ -522,6 +524,112 @@ __global__ void attn_combine_kernel(const float* __restrict__ part, const float*
   *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row * D + c) = pack_round<DT>(x, y);
 }
 
+// KV-cache append (b200k_fa2_fwd_kvcache_append), in front of the decode kernel.  New token i of sequence b goes to cache
+// position p = max(cache_seqlens[b], 0) + i when p < capacity; lens_out[b] = that base + L_new is what the decode kernel
+// reads as its lengths.  With rotary the first rotary_dim columns of each new K row are rotated at p and each Q row at
+// base + t (causal) or base, into q_out.  cos / sin are [rotary_seqlen, rotary_dim / 2].
+struct KvAppend {
+  const uint16_t *q, *k_new, *v_new, *cos, *sin;
+  uint16_t *q_out, *k_cache, *v_cache;
+  const int *seqlens, *table;
+  int* lens_out;
+  long long kv_rows, q_rows;  // B * L_new * H_kv, B * Lq * H (rotary only, else 0)
+  long long rotary_seqlen;
+  int B, L_new, Lq, H, H_kv, D, page_size, pages_per_seq, rotary_dim, causal;
+};
+
+template <int DT>
+__device__ __forceinline__ float2 unpack2(uint32_t w) {
+  if constexpr (DT == 0) return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
+}
+
+// Pair (x0, x1) at position pos becomes (x0 c - x1 s, x0 s + x1 c) in fp32, rounded once.  The products are not left to
+// contraction, so Q and K rows go through the same operations wherever this is inlined.
+__device__ __forceinline__ float rot_lo(float x0, float x1, float c, float s) { return fmaf(x0, c, -__fmul_rn(x1, s)); }
+__device__ __forceinline__ float rot_hi(float x0, float x1, float c, float s) { return fmaf(x0, s, __fmul_rn(x1, c)); }
+
+// Rotates 16-byte vector v (columns 8v .. 8v + 7 < rotary_dim) of `row`.  Interleaved pairs (2j, 2j + 1) lie inside the
+// vector; NeoX pairs (j, j + rotary_dim / 2) pair it with the whole vector rotary_dim / 2 columns away.
+template <int DT, bool INTERLEAVED>
+__device__ __forceinline__ uint4 rotate_vec(uint4 x, const uint16_t* row, int v, long long pos, const KvAppend& a) {
+  const int half = a.rotary_dim / 2;
+  const long long crow = pos < a.rotary_seqlen ? pos : a.rotary_seqlen - 1;
+  const uint16_t* cs = a.cos + crow * half;
+  const uint16_t* sn = a.sin + crow * half;
+  uint32_t* w = reinterpret_cast<uint32_t*>(&x);
+  if constexpr (INTERLEAVED) {
+    const uint2 cw = __ldg(reinterpret_cast<const uint2*>(cs + 4 * v)), sw = __ldg(reinterpret_cast<const uint2*>(sn + 4 * v));
+    const float2 c[2] = {unpack2<DT>(cw.x), unpack2<DT>(cw.y)}, s[2] = {unpack2<DT>(sw.x), unpack2<DT>(sw.y)};
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 p = unpack2<DT>(w[k]);
+      const float ck = k & 1 ? c[k / 2].y : c[k / 2].x, sk = k & 1 ? s[k / 2].y : s[k / 2].x;
+      float lo = rot_lo(p.x, p.y, ck, sk), hi = rot_hi(p.x, p.y, ck, sk);
+      w[k] = pack_round<DT>(lo, hi);
+    }
+  } else {
+    const bool first = 8 * v < half;
+    const int j0 = first ? 8 * v : 8 * v - half;
+    const uint4 y = __ldg(reinterpret_cast<const uint4*>(row + (first ? 8 * v + half : j0)));
+    const uint4 cv = __ldg(reinterpret_cast<const uint4*>(cs + j0)), sv = __ldg(reinterpret_cast<const uint4*>(sn + j0));
+    const uint32_t* yw = reinterpret_cast<const uint32_t*>(&y);
+    const uint32_t* cw = reinterpret_cast<const uint32_t*>(&cv);
+    const uint32_t* sw = reinterpret_cast<const uint32_t*>(&sv);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float2 p = unpack2<DT>(w[k]), q = unpack2<DT>(yw[k]), c = unpack2<DT>(cw[k]), s = unpack2<DT>(sw[k]);
+      // first half: this vector holds x0, the partner x1; second half: the partner holds x0
+      float lo = first ? rot_lo(p.x, q.x, c.x, s.x) : rot_hi(q.x, p.x, c.x, s.x);
+      float hi = first ? rot_lo(p.y, q.y, c.y, s.y) : rot_hi(q.y, p.y, c.y, s.y);
+      w[k] = pack_round<DT>(lo, hi);
+    }
+  }
+  return x;
+}
+
+// One thread per 16-byte vector: K rows, then V rows, then (rotary) Q rows; the first B threads also write lens_out.
+// Cache slots are written only for positions below the capacity, and the block table is read only for those.
+template <int DT, bool ROTARY, bool INTERLEAVED>
+__global__ void __launch_bounds__(256) kvcache_append_kernel(const KvAppend a) {
+  const int vecs = a.D / 8;
+  const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  if (tid < a.B) {
+    const long long n = (long long)max(__ldg(a.seqlens + tid), 0) + a.L_new;
+    a.lens_out[tid] = int(n < INT_MAX ? n : INT_MAX);
+  }
+  const long long cap = (long long)a.pages_per_seq * a.page_size;
+  const long long total = (2 * a.kv_rows + a.q_rows) * vecs;
+  for (long long i = tid; i < total; i += (long long)gridDim.x * blockDim.x) {
+    long long row = i / vecs;
+    const int v = int(i - row * vecs);
+    if (row < 2 * a.kv_rows) {
+      const bool is_k = row < a.kv_rows;
+      if (!is_k) row -= a.kv_rows;
+      const long long b = row / ((long long)a.L_new * a.H_kv);
+      const int tok = int((row / a.H_kv) % a.L_new), hk = int(row % a.H_kv);
+      const long long p = (long long)max(__ldg(a.seqlens + b), 0) + tok;
+      if (p >= cap) continue;
+      const uint16_t* src = (is_k ? a.k_new : a.v_new) + row * a.D;
+      uint4 x = __ldg(reinterpret_cast<const uint4*>(src) + v);
+      if constexpr (ROTARY)
+        if (is_k && 8 * v < a.rotary_dim) x = rotate_vec<DT, INTERLEAVED>(x, src, v, p, a);
+      const long long page = a.table ? (long long)__ldg(a.table + b * a.pages_per_seq + p / a.page_size) : b;
+      uint16_t* dst = (is_k ? a.k_cache : a.v_cache) + ((page * a.page_size + p % a.page_size) * a.H_kv + hk) * a.D;
+      reinterpret_cast<uint4*>(dst)[v] = x;
+    } else if constexpr (ROTARY) {
+      row -= 2 * a.kv_rows;
+      const long long b = row / ((long long)a.Lq * a.H);
+      const int t = int((row / a.H) % a.Lq);
+      const uint16_t* src = a.q + row * a.D;
+      uint4 x = __ldg(reinterpret_cast<const uint4*>(src) + v);
+      if (8 * v < a.rotary_dim)
+        x = rotate_vec<DT, INTERLEAVED>(x, src, v, (long long)max(__ldg(a.seqlens + b), 0) + (a.causal ? t : 0), a);
+      reinterpret_cast<uint4*>(a.q_out + row * a.D)[v] = x;
+    }
+  }
+}
+
 // Launch geometry of KV-cache decode, shared by b200k_fa2_fwd_kvcache and its workspace query.  The 64 rows of a CTA
 // are T tokens x hb query heads of one K/V head's group of G; a group wider than 64 takes nhb head tiles.
 struct KvcacheGrid {
@@ -575,6 +683,110 @@ static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64
   if (tiles > 65535 || B * H_kv > 65535)
     return set_error(B200K_ESHAPE, "%s: %lld (token, head) tiles and %lld (sequence, K/V head) pairs, the grid allows 65535 "
                      "each", fn, (long long)tiles, (long long)(B * H_kv));
+  return B200K_OK;
+}
+
+// Argument checks of b200k_fa2_fwd_kvcache, which b200k_fa2_fwd_kvcache_append shares (before any CUDA call).
+static int kvcache_args(const char* fn, const void* Q, const void* K_cache, const void* V_cache, const void* O,
+                        const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv,
+                        int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq, int dtype) {
+  if (!Q || !K_cache || !V_cache || !O || !cache_seqlens) return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (dtype != B200K_F16 && dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
+  int rc = check_headdim(fn, D);
+  if (rc) return rc;
+  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
+    return set_error(B200K_ESHAPE, "%s: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)", fn,
+                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
+  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
+    return set_error(B200K_ESHAPE, "%s: num_pages * page_size and pages_per_seq * page_size must be <= 2^31 - 1", fn);
+  if ((rc = kvcache_check(fn, B, Lq, H, H_kv, pages_per_seq * page_size))) return rc;
+  if (block_table && page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
+    return set_error(B200K_ESHAPE, "%s: page_size %lld (16, 32, 64 or a multiple of 128)", fn, (long long)page_size);
+  if (!block_table && (num_pages != B || pages_per_seq != 1))
+    return set_error(B200K_ESHAPE, "%s: a contiguous cache (no block table) is num_pages = B pages of page_size = S keys, "
+                     "pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)", fn, (long long)num_pages,
+                     (long long)pages_per_seq);
+  return B200K_OK;
+}
+
+// Everything of a decode call after its workspace check: the decode kernel on `g`'s grid (Q read through a 3-D map,
+// lengths from `seqlens`), then the combine kernel when the call is split.  `part` is the split region of the workspace.
+static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cache, void* O, const int* seqlens,
+                          const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                          int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
+                          const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di) {
+  AttnMask mask;
+  mask.seqlens = seqlens;
+  mask.H = int(H);
+  mask.causal = causal ? 1 : 0;
+  AttnDecode dc;
+  dc.table = block_table;
+  dc.rows = B * Lq * H;
+  dc.Lq = int(Lq);
+  dc.group = int(H / H_kv);
+  dc.hb = g.hb;
+  dc.T = g.T;
+  dc.nhb = g.nhb;
+  dc.page_size = int(page_size);
+  dc.pages_per_seq = int(pages_per_seq);
+  dc.oob = int(num_pages * page_size);
+  if (g.splits > 1) {
+    dc.part = static_cast<float*>(part);
+    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
+  }
+  return run_attn_cfg<1, false, false, true>(dtype, D, [&](auto cfg) {
+    using Cfg = decltype(cfg);
+    // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
+    AttnDecode d = dc;
+    d.box_rows = block_table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
+    const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
+                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
+                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
+    const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
+    const int launched = launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, AttnVarlen(), d, s, di);
+    if (launched || g.splits == 1) return launched;
+    const long long work = d.rows * (D / 2);
+    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
+    B200K_CHECK_CUDA(cudaGetLastError());
+    return B200K_OK;
+  });
+}
+
+// Workspace of b200k_fa2_fwd_kvcache_append, each section on a 256-byte boundary: int32 lengths [B], the rotated Q
+// [B, Lq, H, D] (rotary only), then the split region of kvcache_grid.
+struct AppendLayout {
+  size_t q = 0, part = 0, bytes = 0;
+};
+
+static AppendLayout append_layout(int64_t B, int64_t Lq, int64_t H, int64_t D, bool rotary, const KvcacheGrid& g) {
+  auto up = [](size_t n) { return (n + 255) & ~size_t(255); };
+  AppendLayout l;
+  l.q = up(size_t(B) * sizeof(int));
+  l.part = l.q + (rotary ? up(size_t(B * Lq * H) * size_t(D) * 2) : 0);
+  l.bytes = l.part + g.workspace;
+  return l;
+}
+
+// Checks of the append entry point beyond the decode call's (before any CUDA call).
+static int append_args(const char* fn, const void* Q, const void* K_cache, const void* V_cache, const void* K_new,
+                       const void* V_new, const void* cos, const void* sin, int64_t B, int64_t L_new, int64_t D,
+                       int64_t capacity, int64_t rotary_seqlen, int64_t rotary_dim, const void* workspace) {
+  if (!K_new || !V_new) return set_error(B200K_EARG, "%s: null K_new / V_new", fn);
+  if (!cos != !sin) return set_error(B200K_EARG, "%s: rotary needs both rotary_cos and rotary_sin", fn);
+  if (L_new < 1 || L_new > INT32_MAX || B > INT32_MAX / L_new)
+    return set_error(B200K_ESHAPE, "%s: need L_new >= 1 and B * L_new <= 2^31 - 1 (got L_new=%lld)", fn, (long long)L_new);
+  if (cos && (rotary_dim < 16 || rotary_dim > D || rotary_dim % 16 != 0))
+    return set_error(B200K_ESHAPE, "%s: rotary_dim %lld (a multiple of 16 in [16, D = %lld])", fn, (long long)rotary_dim,
+                     (long long)D);
+  if (cos && rotary_seqlen < capacity)
+    return set_error(B200K_ESHAPE, "%s: rotary_seqlen %lld is below the cache capacity %lld", fn, (long long)rotary_seqlen,
+                     (long long)capacity);
+  const void* aligned[] = {K_new, V_new, cos, sin, Q, K_cache, V_cache, workspace};
+  for (const void* p : aligned)
+    if (reinterpret_cast<uintptr_t>(p) % 16)
+      return set_error(B200K_EALIGN, "%s: K_new, V_new, rotary_cos, rotary_sin, Q, the caches and the workspace must be "
+                       "16-byte aligned", fn);
   return B200K_OK;
 }
 
@@ -687,67 +899,102 @@ extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const v
                                      float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
                                      void* stream) {
   using namespace b200k;
-  if (!Q || !K_cache || !V_cache || !O || !cache_seqlens) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: null pointer");
-  if (dtype != B200K_F16 && dtype != B200K_BF16)
-    return set_error(B200K_EDTYPE, "b200k_fa2_fwd_kvcache: dtype %d not supported (f16, bf16)", dtype);
-  int rc = check_headdim("b200k_fa2_fwd_kvcache", D);
+  const char* fn = "b200k_fa2_fwd_kvcache";
+  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+                        pages_per_seq, dtype);
   if (rc) return rc;
-  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
-    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)",
-                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
-  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
-    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: num_pages * page_size and pages_per_seq * page_size must be "
-                     "<= 2^31 - 1");
-  if ((rc = kvcache_check("b200k_fa2_fwd_kvcache", B, Lq, H, H_kv, pages_per_seq * page_size))) return rc;
-  if (block_table && page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
-    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: page_size %lld (16, 32, 64 or a multiple of 128)",
-                     (long long)page_size);
-  if (!block_table && (num_pages != B || pages_per_seq != 1))
-    return set_error(B200K_ESHAPE, "b200k_fa2_fwd_kvcache: a contiguous cache (no block table) is num_pages = B pages of "
-                     "page_size = S keys, pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)",
-                     (long long)num_pages, (long long)pages_per_seq);
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
   if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
     return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: %zu workspace bytes needed, %zu given", g.workspace,
                      workspace ? workspace_bytes : size_t(0));
+  return kvcache_launch(Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+                        pages_per_seq, scale, dtype, causal, g, workspace, static_cast<cudaStream_t>(stream), di);
+}
+
+extern "C" int b200k_fa2_fwd_kvcache_append_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                                            int64_t max_seqlen_k, int rotary, size_t* bytes) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_fwd_kvcache_append_workspace_bytes";
+  if (!bytes) return set_error(B200K_EARG, "%s: null pointer", fn);
+  int rc = check_headdim(fn, D);
+  if (rc || (rc = kvcache_check(fn, B, Lq, H, H_kv, max_seqlen_k))) return rc;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  *bytes = append_layout(B, Lq, H, D, rotary != 0, kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count)).bytes;
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* V_cache, void* O, const int* cache_seqlens,
+                                            const int* block_table, const void* K_new, const void* V_new, int64_t L_new,
+                                            const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
+                                            int64_t rotary_dim, int rotary_interleaved, int64_t B, int64_t Lq, int64_t H,
+                                            int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size,
+                                            int64_t pages_per_seq, float scale, int dtype, int causal, void* workspace,
+                                            size_t workspace_bytes, void* stream) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_fwd_kvcache_append";
+  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+                        pages_per_seq, dtype);
+  if (rc) return rc;
+  const int64_t capacity = pages_per_seq * page_size;
+  if ((rc = append_args(fn, Q, K_cache, V_cache, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, capacity,
+                        rotary_seqlen, rotary_dim, workspace)))
+    return rc;
+  const bool rotary = rotary_cos != nullptr;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, capacity, di.sm_count);
+  const AppendLayout lay = append_layout(B, Lq, H, D, rotary, g);
+  if (!workspace || workspace_bytes < lay.bytes)
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, lay.bytes,
+                     workspace ? workspace_bytes : size_t(0));
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  AttnMask mask;
-  mask.seqlens = cache_seqlens;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  AttnDecode dc;
-  dc.table = block_table;
-  dc.rows = B * Lq * H;
-  dc.Lq = int(Lq);
-  dc.group = int(H / H_kv);
-  dc.hb = g.hb;
-  dc.T = g.T;
-  dc.nhb = g.nhb;
-  dc.page_size = int(page_size);
-  dc.pages_per_seq = int(pages_per_seq);
-  dc.oob = int(num_pages * page_size);
-  if (g.splits > 1) {
-    dc.part = static_cast<float*>(workspace);
-    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
-  }
-  return run_attn_cfg<1, false, false, true>(dtype, D, [&](auto cfg) {
-    using Cfg = decltype(cfg);
-    // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
-    AttnDecode d = dc;
-    d.box_rows = block_table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
-    const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
-                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
-                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
-    const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
-    const int launched = launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, AttnVarlen(), d, s, di);
-    if (launched || g.splits == 1) return launched;
-    const long long work = d.rows * (D / 2);
-    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  KvAppend a;
+  a.q = static_cast<const uint16_t*>(Q);
+  a.k_new = static_cast<const uint16_t*>(K_new);
+  a.v_new = static_cast<const uint16_t*>(V_new);
+  a.cos = static_cast<const uint16_t*>(rotary_cos);
+  a.sin = static_cast<const uint16_t*>(rotary_sin);
+  a.q_out = rotary ? reinterpret_cast<uint16_t*>(ws + lay.q) : nullptr;
+  a.k_cache = static_cast<uint16_t*>(K_cache);
+  a.v_cache = static_cast<uint16_t*>(V_cache);
+  a.seqlens = cache_seqlens;
+  a.table = block_table;
+  a.lens_out = reinterpret_cast<int*>(ws);
+  a.kv_rows = B * L_new * H_kv;
+  a.q_rows = rotary ? B * Lq * H : 0;
+  a.rotary_seqlen = rotary_seqlen;
+  a.B = int(B);
+  a.L_new = int(L_new);
+  a.Lq = int(Lq);
+  a.H = int(H);
+  a.H_kv = int(H_kv);
+  a.D = int(D);
+  a.page_size = int(page_size);
+  a.pages_per_seq = int(pages_per_seq);
+  a.rotary_dim = rotary ? int(rotary_dim) : 0;
+  a.causal = causal ? 1 : 0;
+  const long long items = (2 * a.kv_rows + a.q_rows) * (D / 8);
+  const long long blocks = ((items > B ? items : B) + 255) / 256;
+  const dim3 grid(unsigned(blocks < 65535 ? blocks : 65535));
+  auto append = [&](auto kern) {
+    kern<<<grid, 256, 0, s>>>(a);
     B200K_CHECK_CUDA(cudaGetLastError());
     return B200K_OK;
-  });
+  };
+  if (dtype == B200K_BF16)
+    rc = !rotary ? append(kvcache_append_kernel<1, false, false>)
+                 : rotary_interleaved ? append(kvcache_append_kernel<1, true, true>) : append(kvcache_append_kernel<1, true, false>);
+  else
+    rc = !rotary ? append(kvcache_append_kernel<0, false, false>)
+                 : rotary_interleaved ? append(kvcache_append_kernel<0, true, true>) : append(kvcache_append_kernel<0, true, false>);
+  if (rc) return rc;
+  // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
+  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
+                        page_size, pages_per_seq, scale, dtype, causal, g, ws + lay.part, s, di);
 }
 
 extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,

@@ -128,7 +128,8 @@ int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, c
                          const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k,
                          int64_t H, int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* stream);
 /* b200k_fa2_fwd_kvcache — attention of the newest Lq query tokens of each sequence against its KV cache (decode,
- * speculative decoding): the forward of flash-attn's flash_attn_with_kvcache, without its append / rotary step.  The
+ * speculative decoding): the forward of flash-attn's flash_attn_with_kvcache (b200k_fa2_fwd_kvcache_append below adds
+ * its append / rotary step).  The
  * same FA-2 kernel in a decode mode: one CTA per (sequence, K/V head) reads each K/V byte once for all the query heads
  * of its group, and a long cache is split across CTAs (the split count is chosen by the library from the shapes and the
  * SM count) and merged by a second kernel in a fixed order, so the result is deterministic.
@@ -161,6 +162,44 @@ int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const void* V_cach
  * unsplit.  Depends on the current device's SM count, so it can fail like any device query. */
 int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                           int64_t max_seqlen_k, size_t* bytes);
+/* b200k_fa2_fwd_kvcache_append — b200k_fa2_fwd_kvcache with flash_attn_with_kvcache's append and rotary steps in the
+ * same call: the new tokens' K / V rows are written into the cache, optionally with rotary embedding on K and Q, and the
+ * attention then runs over each sequence's old keys plus the new ones.  One bandwidth kernel runs before the decode
+ * kernel on `stream`; arguments shared with b200k_fa2_fwd_kvcache mean what they mean there, with every rule it checks.
+ *   K_new, V_new   [B, L_new, H_kv, D] contiguous, Q's dtype, L_new >= 1 (it may differ from Lq).  With base_b =
+ *                  max(cache_seqlens[b], 0), new token i of sequence b is written at cache position p = base_b + i (slot
+ *                  p % page_size of page block_table[b * pages_per_seq + p / page_size], or row p of sequence b without
+ *                  a table).  The caches are updated in place; cache_seqlens is NOT: the caller adds L_new afterwards
+ *   attention      over Lk_b = base_b + L_new keys, with the causal rule of b200k_fa2_fwd_kvcache
+ *   rotary         rotary_cos, rotary_sin: both NULL, or both [rotary_seqlen, rotary_dim / 2] in Q's dtype with
+ *                  rotary_dim % 16 == 0, 16 <= rotary_dim <= D and rotary_seqlen >= pages_per_seq * page_size.  Pair j
+ *                  at position p becomes (x0 c - x1 s, x0 s + x1 c), c = cos[p, j], s = sin[p, j], in fp32 rounded once.
+ *                  rotary_interleaved != 0 pairs columns (2j, 2j + 1), otherwise (j, j + rotary_dim / 2) (GPT-NeoX).
+ *                  New key i is rotated at base_b + i; query token t at base_b + t when causal, at base_b when not.  Only
+ *                  the first rotary_dim columns of K and Q are rotated; the rest, and all of V, are copied bit for bit.
+ *                  Q is not modified: the rotated Q goes to the workspace
+ *   overflow       base_b + L_new > capacity is a caller error; nothing is then written at or past the capacity or
+ *                  outside the sequence's listed pages, and O is the attention over the first capacity keys
+ *   workspace      >= the bytes b200k_fa2_fwd_kvcache_append_workspace_bytes reports (never 0): int32 lengths [B], the
+ *                  rotated Q [B, Lq, H, D] (rotary only), then the split region, each on a 256-byte boundary
+ *   no sync        nothing is read back to the host; the call and the caller's cache_seqlens += L_new can be captured
+ *                  together in a CUDA graph
+ * Errors before any CUDA call: those of b200k_fa2_fwd_kvcache; B200K_EARG when K_new or V_new is NULL or only one of
+ * rotary_cos / rotary_sin is given; B200K_ESHAPE for L_new < 1, B * L_new > INT32_MAX, a bad rotary_dim or rotary_seqlen
+ * below the capacity; B200K_EALIGN unless K_new, V_new, rotary_cos, rotary_sin, Q, the caches and the workspace are
+ * 16-byte aligned.  After the device query: B200K_EARG for a missing or short workspace. */
+int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* V_cache, void* O, const int* cache_seqlens,
+                                 const int* block_table, const void* K_new, const void* V_new, int64_t L_new,
+                                 const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
+                                 int64_t rotary_dim, int rotary_interleaved,
+                                 int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                 int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                 float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
+                                 void* stream);
+/* Workspace the call above needs for these shapes (max_seqlen_k = pages_per_seq * page_size; rotary != 0 when
+ * rotary_cos / rotary_sin are given).  Depends on the current device's SM count. */
+int b200k_fa2_fwd_kvcache_append_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                                 int64_t max_seqlen_k, int rotary, size_t* bytes);
 
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
