@@ -1,8 +1,8 @@
 // Attention forward on Hopper (sm_90a): O = softmax(Q K^T * scale) V, FlashAttention-2 style online softmax, fp32
 // statistics and accumulators in registers, wgmma for both products, TMA + mbarrier rings for Q / K / V.
 //
-// A CTA owns BM = 64 * NWG query rows of one (batch, head) and DV columns of O.  Warpgroup 0 is the producer (one
-// thread issues TMA loads); each consumer warpgroup owns 64 query rows:
+// A CTA owns BM = 64 * NWG query rows and DV columns of O.  Warpgroup 0 is the producer (one thread issues TMA loads);
+// each consumer warpgroup owns 64 query rows:
 //   S  = Q K^T     wgmma m64nBNk16, both operands in shared memory, Q resident for the whole CTA, K streamed in
 //                  64-column chunks of the head dim through a 4-deep ring (so any head dim up to 1024 fits)
 //   P  = exp2(S * scale * log2 e - m)        the S accumulator fragment is, register for register, the A fragment
@@ -12,12 +12,12 @@
 // Head dims above 256 split O into ceil(D / 256) column slices, one per CTA (grid.y); each slice recomputes S.
 // Ragged N and head dims that are not multiples of 64 are zero-filled by TMA (3-D maps: per head) and clipped on the
 // store; padded keys are masked.  Causal CTAs stop at their diagonal tile.
-// Packed variable-length sequences with grouped K/V heads (AttnCfg::VARLEN) run the same main loop; only the tensor
-// maps, the TMA coordinates, the per-CTA key length, the causal diagonal and the epilogue's addressing differ.
-// KV-cache decode (AttnCfg::DECODE) runs it too: a CTA owns the query rows of one K/V head (tokens x grouped heads packed
-// into one 64-row tile), reads K / V through a page table, takes one split of the sequence's KV tiles, and writes either
-// O or fp32 partials that attn_combine_kernel merges.  kvcache_append_kernel, launched before it, writes new K / V rows
-// (K and Q optionally rotated) into the caches and the lengths the decode kernel reads.
+// The layout is the kernel's one mode argument (AttnDense, AttnPacked for packed sequences with grouped K/V heads,
+// AttnDecode): it places the CTA and its TMA boxes, cuts its KV tiles, gives its causal diagonals and stores its rows.
+// In KV-cache decode a CTA owns the query rows of one K/V head (tokens x grouped heads packed into one 64-row tile),
+// reads K / V through a page table, takes one split of the sequence's KV tiles, and writes either O or fp32 partials
+// that attn_combine_kernel merges.  kvcache_append_kernel, launched before it, writes new K / V rows (K and Q
+// optionally rotated) into the caches and the lengths the decode kernel reads.
 #include "abi_common.cuh"
 #include "ptx.cuh"
 
@@ -26,41 +26,10 @@
 
 namespace b200k {
 
-struct AttnMask {
-  const int* seqlens = nullptr;  // int32 [B] valid keys per batch, or null
-  int H = 1;
-  int causal = 0;
-};
-
-// Packed sequences (Cfg::VARLEN): sequence b is tokens [cu_q[b], cu_q[b+1]) of Q / O ([total_q, H, D]) and
-// [cu_k[b], cu_k[b+1]) of K / V ([total_k, H / group, D]); query head h reads K / V head h / group.
-struct AttnVarlen {
-  const int* cu_q = nullptr;
-  const int* cu_k = nullptr;
-  int group = 1;
-  int total_q = 0;
-};
-
-// KV-cache decode (Cfg::DECODE).  Q / O are [B, Lq, H, D]; the caches are [num_pages, page_size, H_kv, D], key j of
-// sequence b at slot j % page_size of page table[b * pages_per_seq + j / page_size] (table null: contiguous cache,
-// sequence b at rows [b * page_size, ...)).  mask.seqlens holds the key counts, mask.H the query heads.  The 64 rows of
-// a CTA are T tokens x hb heads of one group (row r = token r / hb, head r % hb).  With more than one split (gridDim.x)
-// the CTA writes O / l and the row's base-2 log-sum-exp to `part` / `lse` ([split][row][D], [split][row], row =
-// (b * Lq + t) * H + h) instead of O.
-struct AttnDecode {
-  const int* table = nullptr;
-  float* part = nullptr;
-  float* lse = nullptr;
-  long long rows = 0;  // B * Lq * H
-  int Lq = 1, group = 1, hb = 1, T = 1, nhb = 1;
-  int page_size = 1, pages_per_seq = 1, box_rows = 1;
-  int oob = 0;  // a row coordinate past the end of the cache maps: TMA zero-fills the box
-};
-
-template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_, bool VARLEN_ = false, bool DECODE_ = false>  // DT: 0 f16, 1 bf16
+template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_>  // DT: 0 f16, 1 bf16
 struct AttnCfg {
   static constexpr int DT = DT_, DV = DV_, NWG = NWG_, BN = BN_;
-  static constexpr bool V_DN = V_DN_, VARLEN = VARLEN_, DECODE = DECODE_;
+  static constexpr bool V_DN = V_DN_;
   static constexpr int BM = 64 * NWG;
   static constexpr int THREADS = 128 * (NWG + 1);
   static constexpr int KSTAGES = 4, VSTAGES = 2;
@@ -95,73 +64,256 @@ __device__ __forceinline__ uint32_t pack_round(float& lo, float& hi) {
   }
 }
 
-// KV tiles a CTA visits.  q0 is the diagonal of its first row: the key index that row sees last under the causal mask
-// (the row itself, or row + Lk - Lq for packed sequences, which can be negative: no key visible).
+// Row `row` of a 16-bit [rows, D] O from this thread's column pairs of accumulator row h (o[4 i + 2 h], o[4 i + 2 h + 1]
+// hold columns dv0 + 8 i + 2 (lane % 4) and the next), times inv, clipped to D columns (D is even).
 template <class Cfg>
-__device__ __forceinline__ int attn_num_tiles(int q0, int kv_len, const AttnMask& mask) {
-  int nt = (kv_len + Cfg::BN - 1) / Cfg::BN;
-  if constexpr (Cfg::VARLEN) {
-    const int last = q0 + Cfg::BM - 1;
-    if (mask.causal) nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
-  } else {
-    if (mask.causal) nt = min(nt, (q0 + Cfg::BM - 1) / Cfg::BN + 1);
+__device__ __forceinline__ void store_o(void* O, size_t row, int dv0, int D, const float (&o)[Cfg::DV / 2], int h,
+                                        float inv) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < Cfg::DV / 8; ++i) {
+    const int c = dv0 + 8 * i + 2 * (lane & 3);
+    if (c >= D) continue;
+    float x = o[4 * i + 2 * h] * inv, y = o[4 * i + 2 * h + 1] * inv;
+    *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row * size_t(D) + c) = pack_round<Cfg::DT>(x, y);
   }
-  return nt;
 }
 
+// KV tiles [first, end) of a CTA: tile j holds keys [j * BN, (j + 1) * BN) of its sequence.
+struct KvTiles { int first, end; };
+
+// The modes.  Each holds its layout's kernel arguments and provides: Cta, the CTA's coordinates, key count kv_len and
+// first row q0 (its rows are q0 .. q0 + BM - 1 in the numbering diag and store take), which setup fills (false: no rows
+// here; the CTA returns before any barrier exists); tiles, the KV tiles it visits; q_bytes and load_q, the bytes and the
+// box of 64-column chunk c of Q; kv_tile, where KV tile j is, for load_k (chunk c of K) and load_v (all of V); diag,
+// the causal diagonal (last key seen) of row r; zero_v_tail, which only decode fills in; store, the epilogue of row r.
+
+// [B, H, N, D], one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).  CTA (x, y, z) =
+// (query tile, O column slice, batch * H + head).  Rows are numbered within the head, so row r sees keys <= r under the
+// causal mask.
 template <class Cfg>
+struct AttnDense {
+  const int* seqlens;  // int32 [B] valid keys per batch, or null
+  int N, H, causal;
+
+  struct Cta { int bh, q0, dv0, kv_len; };
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    c.bh = blockIdx.z;
+    c.q0 = blockIdx.x * Cfg::BM;
+    c.dv0 = blockIdx.y * Cfg::DV;
+    c.kv_len = seqlens ? min(max(__ldg(seqlens + c.bh / H), 1), N) : N;
+    return true;
+  }
+  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
+    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
+    if (causal) nt = min(nt, (c.q0 + Cfg::BM - 1) / Cfg::BN + 1);
+    return {0, nt};
+  }
+  __device__ __forceinline__ int q_bytes() const { return Cfg::BM * 128; }
+  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.q0, c.bh, kPolicyEvictFirst);
+  }
+  __device__ __forceinline__ int kv_tile(const Cta&, int j) const { return j * Cfg::BN; }
+  __device__ __forceinline__ void load_k(const Cta& c, int key0, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, key0, c.bh, kPolicyEvictNormal);
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, int key0, uint32_t dst, const CUtensorMap* tm, uint32_t bar) const {
+    if constexpr (Cfg::V_DN) {
+#pragma unroll
+      for (int i = 0; i < Cfg::BN / 64; ++i)
+        tma_load_3d(dst + i * Cfg::DV * 128, tm, bar, key0 + i * 64, c.dv0, c.bh, kPolicyEvictNormal);
+    } else {
+#pragma unroll
+      for (int i = 0; i < Cfg::DV / 64; ++i)
+        tma_load_3d(dst + i * Cfg::BN * 128, tm, bar, c.dv0 + i * 64, key0, c.bh, kPolicyEvictNormal);
+    }
+  }
+  __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
+  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
+                                        float, void* O, int D) const {
+    if (r < N) store_o<Cfg>(O, size_t(c.bh) * N + r, c.dv0, D, o, h, inv);
+  }
+};
+
+// Packed sequences: sequence b is tokens [cu_q[b], cu_q[b+1]) of Q / O ([total_q, H, D]) and [cu_k[b], cu_k[b+1]) of
+// K / V ([total_k, H / group, D]); query head h reads K / V head h / group.  The maps are over (D, heads, tokens).  CTA
+// (x, z) = (query tile of the sequence, b * H + head).  Rows are numbered within the sequence; row r sees keys <=
+// r + Lk - Lq under the causal mask (bottom-right aligned).  Its epilogue stores rows of the sequence within tokens [0, total_q), and reloads cu_q
+// rather than keep it in registers through the main loop.
+template <class Cfg>
+struct AttnPacked {
+  static_assert(!Cfg::V_DN, "packed sequences take V as [tokens, heads, D]");
+  const int* cu_q;
+  const int* cu_k;
+  int H, group, total_q, causal;
+
+  struct Cta { int kv_head, q0, q_tok, k_tok, kv_len, shift; };  // q_tok, k_tok: first tokens; shift: Lk - Lq
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    const int b = blockIdx.z / H;
+    c.kv_head = blockIdx.z % H / group;
+    c.q0 = blockIdx.x * Cfg::BM;
+    c.q_tok = __ldg(cu_q + b);
+    const int q_len = __ldg(cu_q + b + 1) - c.q_tok;
+    if (c.q0 >= q_len) return false;
+    c.k_tok = __ldg(cu_k + b);
+    c.kv_len = __ldg(cu_k + b + 1) - c.k_tok;
+    c.shift = c.kv_len - q_len;
+    return true;
+  }
+  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
+    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
+    const int last = c.q0 + c.shift + Cfg::BM - 1;  // can be negative: no key visible
+    if (causal) nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
+    return {0, nt};
+  }
+  __device__ __forceinline__ int q_bytes() const { return Cfg::BM * 128; }
+  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, blockIdx.z % H, c.q_tok + c.q0, kPolicyEvictFirst);
+  }
+  __device__ __forceinline__ int kv_tile(const Cta& c, int j) const { return c.k_tok + j * Cfg::BN; }
+  __device__ __forceinline__ void load_k(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.kv_head, tok, kPolicyEvictNormal);
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar) const {
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, tok, dst + i * Cfg::BN * 128, tm, bar, i);
+  }
+  __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
+  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
+                                        float, void* O, int D) const {
+    const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
+    if (r >= __ldg(cu_q + b + 1) - q_tok) return;
+    const long long tok = (long long)q_tok + r;
+    if (tok < 0 || tok >= total_q) return;
+    store_o<Cfg>(O, size_t(tok) * H + blockIdx.z % H, 0, D, o, h, inv);
+  }
+};
+
+// KV-cache decode.  Q / O are [B, Lq, H, D]; the caches are [num_pages, page_size, H_kv, D], key j of sequence b at
+// slot j % page_size of page table[b * pages_per_seq + j / page_size] (table null: contiguous cache, sequence b at rows
+// [b * page_size, ...)).  CTA (x, y, z) = (split, token tile * nhb + head tile, b * H_kv + K/V head).  Its 64 rows are
+// T tokens x hb heads of one group (row r = token r / hb, head r % hb); row r of token t sees keys <= t + Lk - Lq under
+// the causal mask.  With more than one split (gridDim.x) the CTA writes O / l and the row's base-2 log-sum-exp to
+// `part` / `lse` ([split][row][D], [split][row], row = (b * Lq + t) * H + h) instead of O.
+template <class Cfg>
+struct AttnDecode {
+  static_assert(Cfg::NWG == 1 && !Cfg::V_DN, "decode: one consumer warpgroup, V [keys, heads, D]");
+  const int *seqlens = nullptr, *table = nullptr;  // int32 [B] key counts, block table
+  float *part = nullptr, *lse = nullptr;
+  long long rows = 0;  // B * Lq * H
+  int H = 1, causal = 0;
+  int Lq = 1, group = 1, hb = 1, T = 1, nhb = 1;
+  int page_size = 1, pages_per_seq = 1, box_rows = 1;
+  int oob = 0;  // a row coordinate past the end of the cache maps: TMA zero-fills the box
+
+  struct Cta { int q0, seq, kvh, t0, h0, kv_len, shift; };  // q0 = 0; t0, h0: first token and head; shift: Lk - Lq
+  // cache row of each box of a KV tile: BN / box_rows boxes, one per page when pages are smaller than a tile
+  struct KvRows { int row[Cfg::BN / 16]; };
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    const int h_kv = H / group;
+    c.q0 = 0;
+    c.seq = blockIdx.z / h_kv;
+    c.kvh = blockIdx.z % h_kv;
+    c.t0 = (blockIdx.y / nhb) * T;
+    c.h0 = c.kvh * group + (blockIdx.y % nhb) * hb;
+    c.kv_len = min(max(__ldg(seqlens + c.seq), 0), pages_per_seq * page_size);
+    c.shift = c.kv_len - Lq;
+    return true;
+  }
+  // split s of gridDim.x takes tiles [s * nt / splits, (s + 1) * nt / splits) of this sequence; it may take none
+  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
+    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
+    if (causal) {  // the tile's last token sees keys <= its index + shift
+      const int last = min(c.t0 + T, Lq) - 1 + c.shift;
+      nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
+    }
+    return {int((long long)blockIdx.x * nt / gridDim.x), int((long long)(blockIdx.x + 1) * nt / gridDim.x)};
+  }
+  // the Q box is T tokens x hb heads; rows it reads past the sequence, the group or the tensor are computed and never
+  // stored (zero-filled past the tensor, which TMA still counts in full)
+  __device__ __forceinline__ int q_bytes() const { return T * hb * 128; }
+  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.h0, c.seq * Lq + c.t0, kPolicyEvictFirst);
+  }
+  // A box past the sequence's last page reads outside the map, so the table is read only up to the length.
+  __device__ __forceinline__ KvRows kv_tile(const Cta& c, int j) const {
+    KvRows t;
+#pragma unroll
+    for (int i = 0; i < Cfg::BN / 16; ++i) {
+      const int key = j * Cfg::BN + i * box_rows;
+      if (i * box_rows >= Cfg::BN) break;
+      if (!table) t.row[i] = c.seq * page_size + key;
+      else if (key >= c.kv_len) t.row[i] = oob;
+      else t.row[i] = __ldg(table + size_t(c.seq) * pages_per_seq + key / page_size) * page_size + key % page_size;
+    }
+    return t;
+  }
+  __device__ __forceinline__ void load_k(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+#pragma unroll
+    for (int i = 0; i < Cfg::BN / 16; ++i) {
+      if (i * box_rows >= Cfg::BN) break;
+      tma_load_3d(dst + i * box_rows * 128, tm, bar, chunk * 64, c.kvh, t.row[i], kPolicyEvictNormal);
+    }
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm,
+                                         uint32_t bar) const {
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, t, dst + i * Cfg::BN * 128, tm, bar, i);
+  }
+  __device__ __forceinline__ int diag(const Cta& c, int r) const { return c.t0 + r / hb + c.shift; }
+  // The tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or Inf in
+  // V is NaN in the tensor core, so those V rows are zeroed (K needs nothing: its scores became -inf).
+  __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
+    if (k0 + Cfg::BN <= c.kv_len) return;
+    const int r0 = c.kv_len - k0, words = (Cfg::BN - r0) * 8;  // 16-byte words per 64-column chunk
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i)
+      for (int w = threadIdx.x & 127; w < words; w += 128)
+        asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + i * Cfg::BN * 128 + r0 * 128 + w * 16), "r"(0)
+                     : "memory");
+    fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
+    named_bar_sync(1, 128);
+  }
+  // rows past the box, the sequence or the group are not stored
+  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float m,
+                                        float l, void* O, int D) const {
+    const int tt = r / hb, hh = r % hb;
+    if (tt >= T || c.t0 + tt >= Lq || c.h0 - c.kvh * group + hh >= group) return;
+    const size_t row = (size_t(c.seq) * Lq + c.t0 + tt) * size_t(H) + c.h0 + hh;
+    if (gridDim.x == 1) return store_o<Cfg>(O, row, 0, D, o, h, inv);
+    // one split of several: O / l in fp32 and the base-2 log-sum-exp (-inf: no key seen)
+    const int lane = threadIdx.x & 31;
+    float* dst = part + (size_t(blockIdx.x) * size_t(rows) + row) * size_t(D);
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 8; ++i) {
+      const int col = 8 * i + 2 * (lane & 3);
+      if (col >= D) continue;
+      *reinterpret_cast<float2*>(dst + col) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
+    }
+    if ((lane & 3) == 0) lse[size_t(blockIdx.x) * size_t(rows) + row] = l > 0.f ? m + log2f(l) : -INFINITY;
+  }
+};
+
+template <class Cfg, class Mode>
 __global__ void __launch_bounds__(Cfg::THREADS, 1)
     attn_fwd_wgmma_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmK,
-                          const __grid_constant__ CUtensorMap tmV, void* O, int N, int D, int nqc, float scale_log2,
-                          const AttnMask mask, const AttnVarlen vl, const AttnDecode dc) {
+                          const __grid_constant__ CUtensorMap tmV, void* O, int D, int nqc, float scale_log2,
+                          const Mode md) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DV = Cfg::DV, KST = Cfg::KSTAGES, VST = Cfg::VSTAGES;
-  static_assert(!(Cfg::VARLEN && Cfg::V_DN), "packed sequences take V as [tokens, heads, D]");
-  static_assert(!Cfg::DECODE || (Cfg::NWG == 1 && !Cfg::VARLEN && !Cfg::V_DN), "decode: one consumer warpgroup, V [keys, heads, D]");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u;
   const uint32_t sK = sQ + nqc * BM * 128, sV = sK + KST * Cfg::K_BYTES;
   const uint32_t qbar = sV + VST * Cfg::V_BYTES;
   const uint32_t kfull = qbar + 8, kempty = kfull + 8 * KST, vfull = kempty + 8 * KST, vempty = vfull + 8 * VST;
 
-  // decode: blockIdx.x is the split, blockIdx.y the (token tile, head tile), blockIdx.z the (sequence, K/V head)
-  const int bh = blockIdx.z, q0 = Cfg::DECODE ? 0 : blockIdx.x * BM, dv0 = Cfg::DECODE ? 0 : blockIdx.y * DV;
-  int kv_len = N;
-  // packed sequences: first query and key token of the sequence, and the causal shift Lk - Lq (row r sees keys <= r + shift)
-  int q_tok = 0, k_tok = 0, shift = 0;
-  // decode: sequence, K/V head, first query token of the tile (within the sequence), first query head, first KV tile
-  int seq = 0, kvh = 0, t0 = 0, h0 = 0, j0 = 0;
-  if constexpr (Cfg::VARLEN) {
-    const int b = bh / mask.H;
-    q_tok = __ldg(vl.cu_q + b);
-    const int q_len = __ldg(vl.cu_q + b + 1) - q_tok;
-    if (q0 >= q_len) return;  // no rows of this sequence here; no barrier is initialised yet
-    k_tok = __ldg(vl.cu_k + b);
-    kv_len = __ldg(vl.cu_k + b + 1) - k_tok;
-    shift = kv_len - q_len;
-  } else if constexpr (Cfg::DECODE) {
-    const int h_kv = mask.H / dc.group;
-    seq = bh / h_kv;
-    kvh = bh % h_kv;
-    t0 = (blockIdx.y / dc.nhb) * dc.T;
-    h0 = kvh * dc.group + (blockIdx.y % dc.nhb) * dc.hb;
-    kv_len = min(max(__ldg(mask.seqlens + seq), 0), dc.pages_per_seq * dc.page_size);
-    shift = kv_len - dc.Lq;
-  } else {
-    if (mask.seqlens) kv_len = min(max(__ldg(mask.seqlens + bh / mask.H), 1), N);
-  }
-  int ntiles;
-  if constexpr (Cfg::DECODE) {
-    int nt = (kv_len + BN - 1) / BN;
-    if (mask.causal) {  // the tile's last token sees keys <= its index + shift
-      const int last = min(t0 + dc.T, dc.Lq) - 1 + shift;
-      nt = min(nt, last < 0 ? 0 : last / BN + 1);
-    }
-    // split s of gridDim.x takes tiles [s * nt / splits, (s + 1) * nt / splits) of this sequence; it may take none
-    j0 = int((long long)blockIdx.x * nt / gridDim.x);
-    ntiles = int((long long)(blockIdx.x + 1) * nt / gridDim.x) - j0;
-  } else {
-    ntiles = attn_num_tiles<Cfg>(q0 + shift, kv_len, mask);
-  }
+  typename Mode::Cta cta;
+  if (!md.setup(cta)) return;
+  const KvTiles kv = md.tiles(cta);
   const int wg = threadIdx.x / 128;
 
   if (threadIdx.x == 0) {
@@ -180,74 +332,21 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   if (wg == 0) {
     if (threadIdx.x == 0) {
-      // packed maps are (D, heads, tokens): coordinates (column, head, token) instead of (column, row, batch * head)
-      const int head = bh % mask.H, kv_head = head / vl.group;
-      // decode: the Q box is T tokens x hb heads; rows it reads past the sequence, the group or the tensor are computed
-      // and never stored (zero-filled past the tensor, which TMA still counts in full)
-      mbar_arrive_expect_tx(qbar, Cfg::DECODE ? nqc * dc.T * dc.hb * 128 : nqc * BM * 128);
-      for (int c = 0; c < nqc; ++c) {
-        if constexpr (Cfg::VARLEN) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, head, q_tok + q0, kPolicyEvictFirst);
-        else if constexpr (Cfg::DECODE) tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, h0, seq * dc.Lq + t0, kPolicyEvictFirst);
-        else tma_load_3d(sQ + c * BM * 128, &tmQ, qbar, c * 64, q0, bh, kPolicyEvictFirst);
-      }
+      mbar_arrive_expect_tx(qbar, nqc * md.q_bytes());
+      for (int c = 0; c < nqc; ++c) md.load_q(cta, sQ + c * BM * 128, &tmQ, qbar, c);
       int kc = 0;
-      for (int j = 0; j < ntiles; ++j) {
-        // decode: cache row of each box of KV tile j0 + j (BN / box_rows boxes, one per page when pages are smaller
-        // than a tile).  A box past the sequence's last page reads outside the map, so the table is read only up to the
-        // length.
-        [[maybe_unused]] int crow[BN / 16];
-        if constexpr (Cfg::DECODE) {
-#pragma unroll
-          for (int i = 0; i < BN / 16; ++i) {
-            const int key = (j0 + j) * BN + i * dc.box_rows;
-            if (i * dc.box_rows >= BN) break;
-            if (!dc.table) crow[i] = seq * dc.page_size + key;
-            else if (key >= kv_len) crow[i] = dc.oob;
-            else crow[i] = __ldg(dc.table + size_t(seq) * dc.pages_per_seq + key / dc.page_size) * dc.page_size + key % dc.page_size;
-          }
-        }
+      for (int j = kv.first; j < kv.end; ++j) {
+        const auto t = md.kv_tile(cta, j);
         for (int c = 0; c < nqc; ++c, ++kc) {
           const int s = kc % KST;
           if (kc >= KST) mbar_wait(kempty + 8 * s, ((kc / KST) - 1) & 1);
           mbar_arrive_expect_tx(kfull + 8 * s, Cfg::K_BYTES);
-          if constexpr (Cfg::VARLEN) {
-            tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
-          } else if constexpr (Cfg::DECODE) {
-#pragma unroll
-            for (int i = 0; i < BN / 16; ++i) {
-              if (i * dc.box_rows >= BN) break;
-              tma_load_3d(sK + s * Cfg::K_BYTES + i * dc.box_rows * 128, &tmK, kfull + 8 * s, c * 64, kvh, crow[i],
-                          kPolicyEvictNormal);
-            }
-          } else {
-            tma_load_3d(sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c * 64, j * BN, bh, kPolicyEvictNormal);
-          }
+          md.load_k(cta, t, sK + s * Cfg::K_BYTES, &tmK, kfull + 8 * s, c);
         }
-        const int s = j % VST;
-        if (j >= VST) mbar_wait(vempty + 8 * s, ((j / VST) - 1) & 1);
+        const int n = j - kv.first, s = n % VST;
+        if (n >= VST) mbar_wait(vempty + 8 * s, ((n / VST) - 1) & 1);
         mbar_arrive_expect_tx(vfull + 8 * s, Cfg::V_BYTES);
-        const uint32_t dst = sV + s * Cfg::V_BYTES;
-        if constexpr (Cfg::V_DN) {
-#pragma unroll
-          for (int c = 0; c < BN / 64; ++c)
-            tma_load_3d(dst + c * DV * 128, &tmV, vfull + 8 * s, j * BN + c * 64, dv0, bh, kPolicyEvictNormal);
-        } else {
-#pragma unroll
-          for (int c = 0; c < DV / 64; ++c) {
-            if constexpr (Cfg::VARLEN) {
-              tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, kv_head, k_tok + j * BN, kPolicyEvictNormal);
-            } else if constexpr (Cfg::DECODE) {
-#pragma unroll
-              for (int i = 0; i < BN / 16; ++i) {
-                if (i * dc.box_rows >= BN) break;
-                tma_load_3d(dst + c * BN * 128 + i * dc.box_rows * 128, &tmV, vfull + 8 * s, dv0 + c * 64, kvh, crow[i],
-                            kPolicyEvictNormal);
-              }
-            } else {
-              tma_load_3d(dst + c * BN * 128, &tmV, vfull + 8 * s, dv0 + c * 64, j * BN, bh, kPolicyEvictNormal);
-            }
-          }
-        }
+        md.load_v(cta, t, sV + s * Cfg::V_BYTES, &tmV, vfull + 8 * s);
       }
     }
     return;
@@ -255,21 +354,16 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   const int cw = wg - 1, lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
   const bool leader = (threadIdx.x & 127) == 0;
-  const int row0 = q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
+  const int row0 = cta.q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
   float o[DV / 2];
 #pragma unroll
   for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  // decode: causal diagonal of rows row0 and row0 + 8 (token t0 + r / hb)
-  [[maybe_unused]] int rdiag[2] = {0, 0};
-  if constexpr (Cfg::DECODE) {
-    rdiag[0] = t0 + row0 / dc.hb + shift;
-    rdiag[1] = t0 + (row0 + 8) / dc.hb + shift;
-  }
   mbar_wait(qbar, 0);
 
   int kc = 0;
-  for (int j = 0; j < ntiles; ++j) {
+  for (int j = kv.first; j < kv.end; ++j) {
+    const int n = j - kv.first;  // position in the rings
     // ---- S = Q K^T over the head dim, chunk by chunk
     float s_acc[BN / 2];
 #pragma unroll
@@ -294,11 +388,11 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     fence_regs<BN / 2>(s_acc);
     if (leader) mbar_arrive(kempty + 8 * ((kc - 1) % KST));
 
-    // ---- masks: keys past the valid length, keys after the query row + shift (causal).  The shift is selected at
-    // compile time rather than added as 0, which keeps the dense instantiations' machine code as it was.
-    const int k0 = (Cfg::DECODE ? j0 + j : j) * BN;
-    if (k0 + BN > kv_len ||
-        (mask.causal && k0 + BN - 1 > (Cfg::DECODE ? t0 + shift : (Cfg::VARLEN ? q0 + shift : q0) + cw * 64))) {
+    // ---- masks: keys past the valid length, keys after the row's causal diagonal.  A tile that ends at or before the
+    // diagonal of the warpgroup's first row needs no causal mask.
+    const int k0 = j * BN;
+    if (k0 + BN > cta.kv_len || (md.causal && k0 + BN - 1 > md.diag(cta, cta.q0 + cw * 64))) {
+      const int diag[2] = {md.diag(cta, row0), md.diag(cta, row0 + 8)};
 #pragma unroll
       for (int i = 0; i < BN / 8; ++i)
 #pragma unroll
@@ -306,9 +400,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
           for (int e = 0; e < 2; ++e) {
             const int key = k0 + 8 * i + 2 * (lane & 3) + e;
-            if (key >= kv_len ||
-                (mask.causal && key > (Cfg::DECODE ? rdiag[h] : (Cfg::VARLEN ? row0 + shift : row0) + 8 * h)))
-              s_acc[4 * i + 2 * h + e] = -INFINITY;
+            if (key >= cta.kv_len || (md.causal && key > diag[h])) s_acc[4 * i + 2 * h + e] = -INFINITY;
           }
     }
 
@@ -346,23 +438,10 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
       }
 
     // ---- O += P V
-    const int sv = j % VST;
-    mbar_wait(vfull + 8 * sv, (j / VST) & 1);
+    const int sv = n % VST;
+    mbar_wait(vfull + 8 * sv, (n / VST) & 1);
     const uint32_t vb = sV + sv * Cfg::V_BYTES;
-    if constexpr (Cfg::DECODE) {
-      // the tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or
-      // Inf in V is NaN in the tensor core, so those V rows are zeroed here (K needs nothing: its scores became -inf)
-      if (k0 + BN > kv_len) {
-        const int r0 = kv_len - k0, words = (BN - r0) * 8;  // 16-byte words per 64-column chunk
-#pragma unroll
-        for (int c = 0; c < DV / 64; ++c)
-          for (int i = threadIdx.x & 127; i < words; i += 128)
-            asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + c * BN * 128 + r0 * 128 + i * 16), "r"(0)
-                         : "memory");
-        fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
-        named_bar_sync(1, 128);
-      }
-    }
+    md.zero_v_tail(cta, k0, vb);
     fence_regs<DV / 2>(o);
     wgmma_fence();
 #pragma unroll
@@ -381,55 +460,13 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     if (leader) mbar_arrive(vempty + 8 * sv);
   }
 
-  // ---- epilogue: O / l, clipped to N rows (packed: the sequence's rows and tokens [0, total_q)) and D columns.  Rows
-  // that saw no key have l = 0 and store 0.
-  int q_len = Cfg::DECODE ? BM : N;
-  if constexpr (Cfg::VARLEN) {  // reloaded rather than kept in registers through the main loop
-    const int b = bh / mask.H;
-    q_tok = vl.cu_q[b];
-    q_len = vl.cu_q[b + 1] - q_tok;
-  }
+  // ---- epilogue: O / l; rows that saw no key have l = 0 and store 0
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     float t = l[h];
     t += __shfl_xor_sync(0xffffffffu, t, 1);
     t += __shfl_xor_sync(0xffffffffu, t, 2);
-    const float inv = t > 0.f ? 1.f / t : 0.f;
-    const int r = row0 + 8 * h;
-    if (r >= q_len) continue;
-    size_t row_off;
-    if constexpr (Cfg::DECODE) {
-      // row r is token t0 + r / hb and head h0 + r % hb; rows past the box, the sequence or the group are not stored
-      const int tt = r / dc.hb, hh = r % dc.hb;
-      if (tt >= dc.T || t0 + tt >= dc.Lq || h0 - kvh * dc.group + hh >= dc.group) continue;
-      const size_t row = (size_t(seq) * dc.Lq + t0 + tt) * size_t(mask.H) + h0 + hh;
-      if (gridDim.x > 1) {  // one split of several: O / l in fp32 and the base-2 log-sum-exp (-inf: no key seen)
-        float* dst = dc.part + (size_t(blockIdx.x) * size_t(dc.rows) + row) * size_t(D);
-#pragma unroll
-        for (int i = 0; i < DV / 8; ++i) {
-          const int c = 8 * i + 2 * (lane & 3);
-          if (c >= D) continue;
-          *reinterpret_cast<float2*>(dst + c) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
-        }
-        if ((lane & 3) == 0) dc.lse[size_t(blockIdx.x) * size_t(dc.rows) + row] = t > 0.f ? m[h] + log2f(t) : -INFINITY;
-        continue;
-      }
-      row_off = row * size_t(D);
-    } else if constexpr (Cfg::VARLEN) {
-      const long long tok = (long long)q_tok + r;
-      if (tok < 0 || tok >= vl.total_q) continue;
-      row_off = (size_t(tok) * mask.H + bh % mask.H) * size_t(D);
-    } else {
-      row_off = (size_t(bh) * N + r) * size_t(D);
-    }
-#pragma unroll
-    for (int i = 0; i < DV / 8; ++i) {
-      const int c = dv0 + 8 * i + 2 * (lane & 3);
-      if (c >= D) continue;  // D is even
-      float x = o[4 * i + 2 * h] * inv, y = o[4 * i + 2 * h + 1] * inv;
-      uint32_t* dst = reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row_off + c);
-      *dst = pack_round<Cfg::DT>(x, y);
-    }
+    md.store(cta, row0 + 8 * h, o, h, t > 0.f ? 1.f / t : 0.f, m[h], t, O, D);
   }
 }
 
@@ -448,9 +485,9 @@ static int attn_tmap(CUtensorMap* m, const AttnTensor& t) {
 
 // The launch every mode shares: the shared-memory check, Q / K / V as tensor maps, then the kernel on `grid`.
 // scale <= 0 means 1 / sqrt(D).
-template <class Cfg>
-static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t N, int64_t D, float scale,
-                       const AttnMask& mask, const AttnVarlen& vl, const AttnDecode& dc, cudaStream_t s, const DeviceInfo& di) {
+template <class Cfg, class Mode>
+static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t D, float scale, const Mode& args,
+                       cudaStream_t s, const DeviceInfo& di) {
   const int nqc = int((D + 63) / 64);
   const int smem = Cfg::smem_bytes(nqc);
   if (smem > di.max_smem_optin)
@@ -459,10 +496,10 @@ static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t N
   int rc;
   for (int i = 0; i < 3; ++i)
     if ((rc = attn_tmap(&tm[i], qkv[i]))) return rc;
-  auto kern = attn_fwd_wgmma_kernel<Cfg>;
+  auto kern = attn_fwd_wgmma_kernel<Cfg, Mode>;
   if ((rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem))) return rc;
   if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
-  kern<<<grid, Cfg::THREADS, smem, s>>>(tm[0], tm[1], tm[2], O, int(N), int(D), nqc, scale * 1.4426950408889634f, mask, vl, dc);
+  kern<<<grid, Cfg::THREADS, smem, s>>>(tm[0], tm[1], tm[2], O, int(D), nqc, scale * 1.4426950408889634f, args);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -470,24 +507,25 @@ static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t N
 // Dense [B, H, N, D]: one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).
 template <class Cfg>
 static int launch_dense(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
-                        float scale, const AttnMask& mask, cudaStream_t s, const DeviceInfo& di) {
+                        float scale, const int* seqlens, int causal, cudaStream_t s, const DeviceInfo& di) {
   const int64_t BH = B * H;
   AttnTensor v = {V, BH, N, D, 1, Cfg::BN};
   if (Cfg::V_DN) v = {V, BH, D, N, 1, Cfg::DV};
   const AttnTensor qkv[3] = {{Q, BH, N, D, 1, Cfg::BM}, {K, BH, N, D, 1, Cfg::BN}, v};
   const dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
-  return launch_attn<Cfg>(qkv, grid, O, N, D, scale, mask, AttnVarlen(), AttnDecode(), s, di);
+  const AttnDense<Cfg> args = {seqlens, int(N), int(H), causal ? 1 : 0};
+  return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
 }
 
 // The D <= 128 configurations: BN = 128 keys per tile; O columns DV = 64 for D = 32 / 64, 128 for D = 96 / 128.  V
 // stored [D, N] is built for fp16 only.
-template <int NWG, bool V_DN, bool VARLEN, bool DECODE, class Run>
+template <int NWG, bool V_DN, class Run>
 static int run_attn_cfg(int dtype, int64_t D, Run run) {
   const bool narrow = D <= 64;
   if (dtype != B200K_BF16)
-    return narrow ? run(AttnCfg<0, 64, NWG, 128, V_DN, VARLEN, DECODE>()) : run(AttnCfg<0, 128, NWG, 128, V_DN, VARLEN, DECODE>());
+    return narrow ? run(AttnCfg<0, 64, NWG, 128, V_DN>()) : run(AttnCfg<0, 128, NWG, 128, V_DN>());
   if constexpr (V_DN) return set_error(B200K_EARG, "attention: the [B,H,D,N] V layout is built for fp16 only");
-  else return narrow ? run(AttnCfg<1, 64, NWG, 128, false, VARLEN, DECODE>()) : run(AttnCfg<1, 128, NWG, 128, false, VARLEN, DECODE>());
+  else return narrow ? run(AttnCfg<1, 64, NWG, 128, false>()) : run(AttnCfg<1, 128, NWG, 128, false>());
 }
 
 static int check_headdim(const char* fn, int64_t D) {
@@ -716,35 +754,33 @@ static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cach
                           const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
                           const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di) {
-  AttnMask mask;
-  mask.seqlens = seqlens;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  AttnDecode dc;
-  dc.table = block_table;
-  dc.rows = B * Lq * H;
-  dc.Lq = int(Lq);
-  dc.group = int(H / H_kv);
-  dc.hb = g.hb;
-  dc.T = g.T;
-  dc.nhb = g.nhb;
-  dc.page_size = int(page_size);
-  dc.pages_per_seq = int(pages_per_seq);
-  dc.oob = int(num_pages * page_size);
-  if (g.splits > 1) {
-    dc.part = static_cast<float*>(part);
-    dc.lse = dc.part + size_t(g.splits) * size_t(dc.rows) * size_t(D);
-  }
-  return run_attn_cfg<1, false, false, true>(dtype, D, [&](auto cfg) {
+  return run_attn_cfg<1, false>(dtype, D, [&](auto cfg) {
     using Cfg = decltype(cfg);
+    AttnDecode<Cfg> d;
+    d.seqlens = seqlens;
+    d.table = block_table;
+    d.rows = B * Lq * H;
+    d.H = int(H);
+    d.causal = causal ? 1 : 0;
+    d.Lq = int(Lq);
+    d.group = int(H / H_kv);
+    d.hb = g.hb;
+    d.T = g.T;
+    d.nhb = g.nhb;
+    d.page_size = int(page_size);
+    d.pages_per_seq = int(pages_per_seq);
     // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
-    AttnDecode d = dc;
     d.box_rows = block_table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
+    d.oob = int(num_pages * page_size);
+    if (g.splits > 1) {
+      d.part = static_cast<float*>(part);
+      d.lse = d.part + size_t(g.splits) * size_t(d.rows) * size_t(D);
+    }
     const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
                                {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
                                {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
     const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
-    const int launched = launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, AttnVarlen(), d, s, di);
+    const int launched = launch_attn<Cfg>(qkv, grid, O, D, scale, d, s, di);
     if (launched || g.splits == 1) return launched;
     const long long work = d.rows * (D / 2);
     attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
@@ -799,9 +835,9 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
   if constexpr (DV == 192) {
     using Two = AttnCfg<0, DV, 2, 64, false>;
     if (Two::smem_bytes(int((D + 63) / 64)) <= di.max_smem_optin)
-      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
+      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, s, di);
   }
-  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, AttnMask(), s, di);
+  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, s, di);
 }
 
 }  // namespace b200k
@@ -832,12 +868,8 @@ extern "C" int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* 
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  AttnMask mask;
-  mask.seqlens = seqlens_k;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  auto run = [&](auto cfg) { return launch_dense<decltype(cfg)>(Q, K, V, O, B, H, N, D, scale, mask, s, di); };
-  return v_is_dn ? run_attn_cfg<2, true, false, false>(dtype, D, run) : run_attn_cfg<2, false, false, false>(dtype, D, run);
+  auto run = [&](auto cfg) { return launch_dense<decltype(cfg)>(Q, K, V, O, B, H, N, D, scale, seqlens_k, causal, s, di); };
+  return v_is_dn ? run_attn_cfg<2, true>(dtype, D, run) : run_attn_cfg<2, false>(dtype, D, run);
 }
 
 extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
@@ -865,19 +897,12 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  AttnMask mask;
-  mask.H = int(H);
-  mask.causal = causal ? 1 : 0;
-  AttnVarlen vl;
-  vl.cu_q = cu_seqlens_q;
-  vl.cu_k = cu_seqlens_k;
-  vl.group = int(H / H_kv);
-  vl.total_q = int(total_q);
-  return run_attn_cfg<2, false, true, false>(dtype, D, [&](auto cfg) {
+  return run_attn_cfg<2, false>(dtype, D, [&](auto cfg) {
     using Cfg = decltype(cfg);
     const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1}, {K, total_k, H_kv, D, Cfg::BN, 1}, {V, total_k, H_kv, D, Cfg::BN, 1}};
     const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
-    return launch_attn<Cfg>(qkv, grid, O, 0, D, scale, mask, vl, AttnDecode(), s, di);
+    const AttnPacked<Cfg> args = {cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
+    return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
   });
 }
 

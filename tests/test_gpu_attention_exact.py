@@ -166,7 +166,8 @@ def test_dense_exact(dtype, D, causal, lens):
 @pytest.mark.parametrize("causal", [False, True])
 @pytest.mark.parametrize("D", [32, 64, 96, 128])
 def test_dense_v_stored_dn_exact(D, causal, lens):
-    """V [B,H,D,N] (fp16): AttnCfg<0, 64 / 128, 2, 128, true>, with causal, key padding and N % 128 != 0."""
+    """V [B,H,D,N] (fp16): AttnCfg<0, 64 / 128, 2, 128, true> in the dense mode, with causal, key padding and
+    N % 128 != 0."""
     ops = _ops()
     for N in (1000, 72):
         L = [1, 63, 64, 127, 128, 129, N] if lens else None

@@ -1,0 +1,303 @@
+"""A/B of the attention entry points against an earlier build of the library, in one process: same bits, then time.
+
+A second copy of libb200k.so, built from another git revision, is loaded through ctypes next to the one in the tree, with
+the signatures of b200k._loader.  Every call goes through b200k.ops, pointed at one library or the other, so both builds
+see the same arguments.
+
+  1. Seeded random inputs through both builds; every output (and, for append, both caches) must have the same bits:
+     dense f16 / bf16 at D 32 - 128 (causal, key padding, ragged N), V stored [B,H,D,N], FFPA at D 160 - 1024, packed
+     GQA / MQA with empty sequences, decode on contiguous caches and pages of 16 / 64 / 256 at one split and at many
+     (G = 72 among them: two 64-row head tiles), and append with and without rotary.
+  2. Time per call of each build, alternating, one CUDA graph of `iters` calls per build per round: bench.py's
+     attention shapes (dense (4, 48, 8192, 64) and (4, 64, 8192, 128), FFPA (1, 32, 4096, 512)), packed GQA (4 x 8192
+     tokens, H 64, H_kv 8, D 128, causal) and decode against an 8K cache at B 1 and 64.  Each line gives the median
+     and min - max of both builds and whether the new median lies inside the base's min - max.
+
+The first line names the GPU, its power limit and its maximum SM clock, read in the same run.
+
+    python tools/gpu_ab_attention.py --build-base REV        # CPU is enough: git archive REV -> build_ab/base, make
+    python tools/gpu_ab_attention.py [--base-lib PATH] [--rounds 9]
+"""
+import argparse
+import contextlib
+import ctypes
+import json
+import os
+import sys
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, os.path.join(ROOT, "tools"))
+sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
+from gpu_perf_hgemm import BASE_LIB, build_base, gpu_info  # noqa: E402
+
+
+def load(path):
+    from b200k import _loader
+
+    lib = ctypes.CDLL(os.path.abspath(path))
+    for name, (res, argtypes) in _loader._SIGS.items():
+        fn = getattr(lib, name)
+        fn.restype = res
+        fn.argtypes = argtypes
+    return lib
+
+
+@contextlib.contextmanager
+def using(lib):
+    """b200k.ops calls `lib` inside the block."""
+    from b200k import ops
+
+    saved = ops._lib
+    ops._lib = lib
+    try:
+        yield
+    finally:
+        ops._lib = saved
+
+
+def equal_cases(torch, ops):
+    """(name, run) pairs; run() makes fresh outputs (and caches) from the case's seeded inputs and returns them."""
+    dev = "cuda"
+    cases = []
+
+    def rn(*shape, dt=torch.float16):
+        return torch.randn(*shape, device=dev).to(dt)
+
+    def i32(x):
+        return torch.as_tensor(x, dtype=torch.int32, device=dev)
+
+    for dt in (torch.float16, torch.bfloat16):
+        for D in (32, 64, 96, 128):
+            for causal in (False, True):
+                for pad in (False, True):
+                    torch.manual_seed(D + 2 * causal + 4 * pad)
+                    B, H, N = 3, 4, 1000
+                    q, k, v = [rn(B, H, N, D, dt=dt) for _ in range(3)]
+                    sl = i32([1, 129, 700]) if pad else None
+
+                    def run(q=q, k=k, v=v, sl=sl, causal=causal):
+                        o = torch.full_like(q, float("nan"))
+                        ops.fa2_fwd(q, k, v, o, causal=causal, seqlens_k=sl)
+                        return [o]
+                    cases.append(("dense %s D=%d causal=%d pad=%d" % (str(dt)[6:], D, causal, pad), run))
+    for D in (64, 128):
+        for causal in (False, True):
+            torch.manual_seed(10 + D + causal)
+            q, k = rn(2, 3, 1000, D), rn(2, 3, 1000, D)
+            vt = rn(2, 3, D, 1000)
+            sl = i32([1000, 129])
+
+            def run(q=q, k=k, vt=vt, sl=sl, causal=causal):
+                o = torch.full_like(q, float("nan"))
+                ops.fa2_fwd(q, k, vt, o, v_is_dn=True, causal=causal, seqlens_k=sl)
+                return [o]
+            cases.append(("dense V [D,N] D=%d causal=%d" % (D, causal), run))
+    for D in (160, 192, 256, 288, 512, 544, 1024):
+        torch.manual_seed(D)
+        q, k, v = [rn(1, 3, 777, D) for _ in range(3)]
+
+        def run(q=q, k=k, v=v):
+            o = torch.full_like(q, float("nan"))
+            ops.ffpa_fwd(q, k, v, o)
+            return [o]
+        cases.append(("ffpa D=%d" % D, run))
+    lq, lk = [77, 0, 1, 129, 300, 0, 200, 64, 5], [300, 5, 0, 128, 129, 0, 200, 63, 700]
+    cq, ck = [i32([0] + torch.tensor(x).cumsum(0).tolist()) for x in (lq, lk)]
+    for dt in (torch.float16, torch.bfloat16):
+        for D in (64, 128):
+            for H_kv in (4, 1):
+                for causal in (False, True):
+                    torch.manual_seed(D + H_kv + causal)
+                    q, k, v = rn(sum(lq), 16, D, dt=dt), rn(sum(lk), H_kv, D, dt=dt), rn(sum(lk), H_kv, D, dt=dt)
+
+                    def run(q=q, k=k, v=v, causal=causal):
+                        o = torch.full_like(q, float("nan"))
+                        ops.fa2_fwd_varlen(q, k, v, o, cq, ck, max(lq), causal=causal)
+                        return [o]
+                    cases.append(("packed %s D=%d H=16 H_kv=%d causal=%d" % (str(dt)[6:], D, H_kv, causal), run))
+
+    def paged(kc, vc, ps, seed):
+        """[B, S, H_kv, D] caches as [pages, ps, H_kv, D] under a shuffled table, two pages no table lists."""
+        B, S = kc.shape[:2]
+        pps = S // ps
+        g = torch.Generator().manual_seed(seed)
+        perm = torch.randperm(B * pps + 2, generator=g).to(dev)
+        table = perm[:B * pps].view(B, pps)
+        out = []
+        for c in (kc, vc):
+            p = torch.randn(B * pps + 2, ps, *c.shape[2:], device=dev).to(c.dtype)
+            p[table.reshape(-1)] = c.reshape(B * pps, ps, *c.shape[2:])
+            out.append(p)
+        return out[0], out[1], table.to(torch.int32)
+
+    # decode: (B, Lq, G, H_kv) with one split (B * H_kv CTAs fill the SMs) and with many
+    for dt in (torch.float16, torch.bfloat16):
+        for D in (64, 128):
+            for kind in ("contig", 16, 64, 256):
+                for B, Lq, G, H_kv in ((16, 1, 4, 8), (1, 3, 8, 1), (64, 1, 72, 2), (2, 2, 72, 2)):
+                    for causal in (False, True):
+                        S = 2048
+                        seed = D + B + G + causal + (0 if kind == "contig" else kind)
+                        torch.manual_seed(seed)
+                        q = rn(B, Lq, G * H_kv, D, dt=dt)
+                        kc, vc = rn(B, S, H_kv, D, dt=dt), rn(B, S, H_kv, D, dt=dt)
+                        table = None
+                        if kind != "contig":
+                            kc, vc, table = paged(kc, vc, kind, seed)
+                        lens = i32(torch.randint(0, S + 1, (B,)).tolist())
+                        splits = ops.fa2_fwd_kvcache_workspace_bytes(B, Lq, G * H_kv, H_kv, D, S) > 0
+
+                        def run(q=q, kc=kc, vc=vc, lens=lens, table=table, causal=causal):
+                            o = torch.full_like(q, float("nan"))
+                            ops.fa2_fwd_kvcache(q, kc, vc, o, lens, table, causal=causal)
+                            return [o]
+                        cases.append(("decode %s D=%d %s B=%d Lq=%d G=%d H_kv=%d causal=%d %s" % (
+                            str(dt)[6:], D, kind, B, Lq, G, H_kv, causal, "split" if splits else "one split"), run))
+    for kind in ("contig", 64):
+        for rotary in (None, "neox", "interleaved"):
+            for B, H_kv in ((16, 8), (1, 1)):
+                torch.manual_seed(B + H_kv + (rotary is None))
+                Lq, G, D, S, L_new = 2, 4, 128, 1024, 2
+                q = rn(B, Lq, G * H_kv, D)
+                kc0, vc0 = rn(B, S, H_kv, D), rn(B, S, H_kv, D)
+                table = None
+                if kind != "contig":
+                    kc0, vc0, table = paged(kc0, vc0, kind, B)
+                kn, vn = rn(B, L_new, H_kv, D), rn(B, L_new, H_kv, D)
+                lens = i32(torch.randint(0, S - L_new + 1, (B,)).tolist())
+                rot = {}
+                if rotary:
+                    theta = torch.rand(S, 32, device=dev) * 6.283
+                    rot = dict(rotary_cos=theta.cos().half(), rotary_sin=theta.sin().half(),
+                               rotary_interleaved=rotary == "interleaved")
+
+                def run(q=q, kc0=kc0, vc0=vc0, kn=kn, vn=vn, lens=lens, table=table, rot=rot):
+                    kc, vc = kc0.clone(), vc0.clone()
+                    o = torch.full_like(q, float("nan"))
+                    ops.fa2_fwd_kvcache(q, kc, vc, o, lens, table, causal=True, k=kn, v=vn, **rot)
+                    return [o, kc, vc]
+                cases.append(("append %s rotary=%s B=%d H_kv=%d" % (kind, rotary, B, H_kv), run))
+    return cases
+
+
+def timed_cases(torch, ops):
+    """(name, flop, run) for the timed shapes; run() is one call on preallocated tensors."""
+    dev = "cuda"
+    cases = []
+    for B, H, N, D in ((4, 48, 8192, 64), (4, 64, 8192, 128)):
+        q, k, v = [torch.randn(B, H, N, D, dtype=torch.half, device=dev) for _ in range(3)]
+        o = torch.empty_like(q)
+        cases.append(("dense (%d, %d, %d, %d)" % (B, H, N, D), 4.0 * B * H * N * N * D,
+                      lambda q=q, k=k, v=v, o=o: ops.fa2_fwd(q, k, v, o)))
+    B, H, N, D = 1, 32, 4096, 512
+    q, k, v = [torch.randn(B, H, N, D, dtype=torch.half, device=dev) for _ in range(3)]
+    o = torch.empty_like(q)
+    cases.append(("ffpa (1, 32, 4096, 512)", 4.0 * B * H * N * N * D, lambda q=q, k=k, v=v, o=o: ops.ffpa_fwd(q, k, v, o)))
+    B, N, H, H_kv, D = 4, 8192, 64, 8, 128
+    q = torch.randn(B * N, H, D, dtype=torch.half, device=dev)
+    k, v = [torch.randn(B * N, H_kv, D, dtype=torch.half, device=dev) for _ in range(2)]
+    o = torch.empty_like(q)
+    cu = torch.arange(0, (B + 1) * N, N, dtype=torch.int32, device=dev)
+    cases.append(("packed GQA 4 x 8192 H 64 H_kv 8 D 128 causal", 2.0 * B * H * N * N * D,
+                  lambda q=q, k=k, v=v, o=o: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, N, causal=True)))
+    for B in (1, 64):
+        S, Lq, H, H_kv, D = 8192, 1, 32, 8, 128
+        q = torch.randn(B, Lq, H, D, dtype=torch.half, device=dev)
+        kc, vc = [torch.randn(B, S, H_kv, D, dtype=torch.half, device=dev) for _ in range(2)]
+        o = torch.empty_like(q)
+        lens = torch.full((B,), S, dtype=torch.int32, device=dev)
+        cases.append(("decode B %d Lq 1 H 32 H_kv 8 D 128, 8K cache" % B, 4.0 * B * Lq * H * S * D,
+                      lambda q=q, kc=kc, vc=vc, o=o, lens=lens: ops.fa2_fwd_kvcache(q, kc, vc, o, lens)))
+    return cases
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--build-base", metavar="REV", help="build REV's library into build_ab/base and exit")
+    ap.add_argument("--base-lib", default=BASE_LIB, help="the library to compare against (default: build_ab/base's)")
+    ap.add_argument("--rounds", type=int, default=9)
+    args = ap.parse_args()
+    if args.build_base:
+        build_base(args.build_base)
+        return
+
+    import torch
+
+    if not torch.cuda.is_available():
+        sys.exit("gpu_ab_attention.py needs a CUDA device")
+    from b200k import _loader, ops
+
+    libs = {"base": load(args.base_lib), "new": _loader.lib}
+    info = gpu_info(torch)
+    print(json.dumps(dict(info, base_lib=os.path.relpath(os.path.abspath(args.base_lib), ROOT), rounds=args.rounds)),
+          flush=True)
+
+    bad = 0
+    cases = equal_cases(torch, ops)
+    for name, run in cases:
+        outs = {}
+        for key, lib in libs.items():
+            with using(lib):
+                outs[key] = run()
+        same = all(torch.equal(a, b) for a, b in zip(outs["base"], outs["new"]))
+        bad += not same
+        if not same:
+            print(json.dumps({"case": name, "bit_equal": False}), flush=True)
+    print(json.dumps({"equal_cases": len(cases), "differing": bad}), flush=True)
+
+    slow = 0
+    for name, flop, fn in timed_cases(torch, ops):
+        graphs, iters = {}, None
+        for key, lib in libs.items():
+            with using(lib):
+                fn()
+                torch.cuda.synchronize()
+                if iters is None:  # about 100 ms of work per build per round
+                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+                    e0.record()
+                    for _ in range(3):
+                        fn()
+                    e1.record()
+                    torch.cuda.synchronize()
+                    iters = max(3, min(2000, int(100.0 / (e0.elapsed_time(e1) / 3))))
+                s = torch.cuda.Stream()
+                s.wait_stream(torch.cuda.current_stream())
+                with torch.cuda.stream(s):
+                    fn()  # warm-up on the capture stream
+                torch.cuda.current_stream().wait_stream(s)
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    for _ in range(iters):
+                        fn()
+                graphs[key] = g
+        for g in graphs.values():
+            g.replay()
+        torch.cuda.synchronize()
+        times = {k: [] for k in graphs}
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        for r in range(args.rounds):
+            for key in (("base", "new") if r % 2 == 0 else ("new", "base")):
+                e0.record()
+                graphs[key].replay()
+                e1.record()
+                torch.cuda.synchronize()
+                times[key].append(e0.elapsed_time(e1) * 1e3 / iters)
+        med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
+        inside = min(times["base"]) <= med["new"] <= max(times["base"])
+        slow += med["new"] > max(times["base"])
+        line = {"case": name, "iters_per_round": iters}
+        for k, v in times.items():
+            line[k + "_us"] = round(med[k], 2)
+            line[k + "_min_max_us"] = [round(min(v), 2), round(max(v), 2)]
+            line[k + "_tflops"] = round(flop / (med[k] * 1e-6) * 1e-12, 1)
+        line["new_over_base"] = round(med["new"] / med["base"], 4)
+        line["new_median_inside_base_range"] = inside
+        print(json.dumps(line), flush=True)
+        del graphs
+        torch.cuda.empty_cache()
+    print(json.dumps({"differing_cases": bad, "new_median_above_base_max": slow}), flush=True)
+    sys.exit(1 if bad else 0)
+
+
+if __name__ == "__main__":
+    main()
