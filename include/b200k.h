@@ -65,7 +65,9 @@ int b200k_hgemm_f16(const void* A, const void* B, void* C, int64_t M, int64_t N,
  * fp32 output (wgmma .tf32: the operands' low 13 mantissa bits are ignored by the tensor core, fp32 accumulation) - the
  * H100 counterpart of kernels/sgemm/sgemm_wmma_tf32_stage.cu:L25-420 (sgemm_wmma_m16n16k8_*).
  * K and N must be multiples of 8 (16-bit types) or 4 (fp32).  TF32 wgmma reads K-major operands only, so an fp32 [K,N] B
- * is first transposed into a scratch buffer allocated on `stream` (cudaMallocAsync) and freed after the product. */
+ * is first transposed into a scratch buffer allocated on `stream` (cudaMallocAsync) and freed after the product.  That form
+ * reads B only through the transpose, so its B needs only the 4-byte alignment of a float (A and C must still be 16-byte
+ * aligned); the allocation and free are stream-ordered, so the call can be captured in a CUDA graph. */
 int b200k_gemm(const void* A, const void* B, void* C, int64_t M, int64_t N, int64_t K, int b_is_nk, int dtype, int variant,
                void* stream);
 /* All four storage cases (SURVEY.md 8(f)-4 "TN/NT"): a_is_km != 0 means A is stored transposed, [K,M] row-major (the BLAS

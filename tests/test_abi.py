@@ -42,6 +42,13 @@ def test_argument_validation_happens_before_cuda():
     assert lib.b200k_gemm(one, one, one, 8, 8, 4, 0, L.BF16, 0, None) == L.ESHAPE
     assert lib.b200k_gemm(one, one, one, 8, 8, 8, 0, L.I8, 0, None) == L.EDTYPE
     assert lib.b200k_gemm(None, one, one, 8, 8, 8, 1, L.F32, 0, None) == L.EARG
+    # variant: 0 .. 4 in the low 8 bits, higher bits ignored; 5 is unknown whatever the high bits hold
+    for v in (5, 5 | (0x5A5A << 8)):
+        assert lib.b200k_hgemm_f16(one, one, one, 8, 8, 8, 0, v, None) == L.EARG
+        assert b"variant 5 unknown" in lib.b200k_last_error()
+        for dt in (L.F16, L.BF16, L.F32):
+            assert lib.b200k_gemm(one, one, one, 8, 8, 8, 1, dt, v, None) == L.EARG
+        assert lib.b200k_gemm_ex(one, one, one, 8, 8, 8, 1, 0, L.BF16, v, None) == L.EARG
     # second set of support kernels
     assert lib.b200k_layer_norm(one, one, 0, 8, 1.0, 0.0, 1e-5, L.F32, 1, None) == L.ESHAPE
     assert lib.b200k_mat_transpose_f32(one, None, 4, 4, None) == L.EARG

@@ -215,10 +215,10 @@ def test_gemm_a_stored_transposed_nt_tt(shape, tn, dtype):
 
 @pytest.mark.parametrize("K", [64, 128, 192, 256, 320, 1024])
 @pytest.mark.parametrize("mn", [(512, 256), (1024, 768), (1000, 520), (2048, 2048)])
-def test_512x256_pair_tile_short_k_and_ragged(mn, K):
-    """Short and ragged K (1 ... 16 k-blocks, so the 4-stage ring is filled partly, exactly and many times over), one and
-    several tiles, ragged M / N, NN and TN storage of B; variant values 4 and 2 of the old ABI are accepted and give the
-    same bits as each other and as the TN product (same kernel, same K order)."""
+def test_short_k_fills_the_stage_ring_partly_and_exactly(mn, K):
+    """Short K (1 ... 16 k-blocks of 64, so the 4-stage ring is filled partly, exactly and many times over), one and
+    several 128 x 256 tiles, ragged M / N, NN and TN storage of B; variant values 4 and 2 of the old ABI are accepted and
+    give the same bits as each other and as the TN product (same kernel, same K order)."""
     from b200k import ops
 
     M, N = mn
@@ -238,9 +238,10 @@ def test_512x256_pair_tile_short_k_and_ragged(mn, K):
 
 
 @pytest.mark.parametrize("shape", [(4096, 4096, 1024), (2304, 3072, 512)])
-def test_stream_k_launch_replays_under_cuda_graph(shape):
-    """One GEMM launch captured into a CUDA graph and replayed with new operand contents: nothing launch-specific may be
-    frozen into the graph, so every replay equals an eager call on the same operands, bit for bit."""
+def test_gemm_launch_replays_under_cuda_graph(shape):
+    """One GEMM launch (one 128 x 256 tile per CTA) captured into a CUDA graph and replayed with new contents of A:
+    nothing launch-specific may be frozen into the graph, so every replay equals an eager call on the same operands,
+    bit for bit."""
     from b200k import _loader as L
     from b200k import ops
 
