@@ -1,12 +1,12 @@
-// HBM-roofline support kernels for H100: elementwise add, all-reduce sum, softmax, RMS norm, RoPE, histogram,
-// embedding gather.  Coalesced 128-bit accesses, warp-shuffle reductions, grids sized from the SM count, one pass
-// over HBM wherever the row fits in registers.  No tensor cores (none of this is GEMM shaped).
+// HBM-roofline support kernels for H100: elementwise add, all-reduce sum, softmax, RMS norm, layer norm, RoPE,
+// histogram, embedding gather.  Coalesced 128-bit accesses, warp-shuffle reductions, grids sized from the SM count, one
+// pass over HBM wherever the row fits in registers.  No tensor cores (none of this is GEMM shaped).
 //
 // Replaces (reference file:line)
 //   kernels/elementwise/elementwise.cu:L24-168      kernels/reduce/block_all_reduce.cu:L42-686
 //   kernels/softmax/softmax.cu:L102-391             kernels/rms-norm/rms_norm.cu:L53-366
-//   kernels/rope/rope.cu:L20-69                     kernels/histogram/histogram.cu:L18-48
-//   kernels/embedding/embedding.cu:L16-78
+//   kernels/layer-norm/layer_norm.cu:L48-419        kernels/rope/rope.cu:L20-69
+//   kernels/histogram/histogram.cu:L18-48           kernels/embedding/embedding.cu:L16-78
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
 #include <cuda_fp8.h>
@@ -208,21 +208,12 @@ struct Loader<B200K_I8> {
   __device__ static int one(const int8_t* p) { return int(*p); }
 };
 
-template <typename A>
-__device__ __forceinline__ A warp_sum_t(A v);
-template <>
-__device__ __forceinline__ float warp_sum_t<float>(float v) { return warp_sum(v); }
-template <>
-__device__ __forceinline__ int warp_sum_t<int>(int v) { return warp_sum_i(v); }
-
 template <int DT, bool ACC16, bool EXP /* sum exp(x) instead of x: softmax mode 0 */>
 __global__ void __launch_bounds__(kThreads) reduce_sum_kernel(const void* __restrict__ xin, void* __restrict__ out,
                                                               int64_t n, void* __restrict__ workspace, bool vec_ok) {
   using L = Loader<DT>;
   using A = typename L::acc_t;
   using E = typename L::elem_t;
-  A* partials = reinterpret_cast<A*>(workspace);
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kReduceMaxBlocks * sizeof(float));
   const E* x = reinterpret_cast<const E*>(xin);
   A acc = 0;
   const int64_t stride = int64_t(gridDim.x) * kThreads;
@@ -256,47 +247,13 @@ __global__ void __launch_bounds__(kThreads) reduce_sum_kernel(const void* __rest
     if constexpr (EXP) acc += exp_sub(float(L::one(x + j)), 0.f);
     else acc += L::one(x + j);
   }
-  __shared__ A s_part[kThreads / 32];
-  __shared__ bool s_last;
-  acc = warp_sum_t<A>(acc);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) s_part[warp] = acc;
-  __syncthreads();
-  if (warp == 0) {
-    A v = (lane < kThreads / 32) ? s_part[lane] : A(0);
-    v = warp_sum_t<A>(v);
-    if (lane == 0) {
-      partials[blockIdx.x] = v;
-      __threadfence();
-      const unsigned int t = atomicAdd(ticket, 1u);
-      s_last = (t == gridDim.x - 1);
-    }
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    // fixed-order final sum: thread t adds partials t, t+256, ... then a fixed tree
-    A v = 0;
-    for (int i = threadIdx.x; i < int(gridDim.x); i += kThreads) v += reinterpret_cast<volatile A*>(partials)[i];
-    v = warp_sum_t<A>(v);
-    __syncthreads();
-    if (lane == 0) s_part[warp] = v;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      A r = 0;
-      for (int i = 0; i < kThreads / 32; ++i) r += s_part[i];
-      *reinterpret_cast<A*>(out) = r;
-      *ticket = 0;  // leave the workspace ready for the next call
-    }
-  }
+  grid_sum<A>(acc, static_cast<A*>(out), workspace);
 }
 
 template <int DT, bool EXP>
 static int launch_reduce(const void* x, void* out, int64_t n, int acc_f16, void* ws, cudaStream_t s,
                          const DeviceInfo& di) {
-  using L = Loader<DT>;
-  int grid = grid_for(n / L::N, kThreads * 4, di.sm_count, 8);
-  if (grid > kReduceMaxBlocks) grid = kReduceMaxBlocks;
+  const int grid = reduce_grid(n / Loader<DT>::N, di.sm_count);
   const bool vec_ok = aligned16(x);
   if (acc_f16 && !EXP) reduce_sum_kernel<DT, true, false><<<grid, kThreads, 0, s>>>(x, out, n, ws, vec_ok);
   else reduce_sum_kernel<DT, false, EXP><<<grid, kThreads, 0, s>>>(x, out, n, ws, vec_ok);
@@ -307,12 +264,14 @@ static int launch_reduce(const void* x, void* out, int64_t n, int acc_f16, void*
 // ============================================================================================ row kernels
 // One row is owned by R threads (R = 32, 128 or 256; 256/R rows per CTA).  Each thread keeps up to 32 elements of the
 // row in registers (4 or 8 16-byte vectors), so x is read once and y written once.  Rows longer than 32*R fall back
-// to re-reading x from L2/HBM.
-enum RowOp { OP_SOFTMAX = 0, OP_SAFE_SOFTMAX = 1, OP_RMSNORM = 2, OP_RMSNORM_ACC16 = 3 };
+// to re-reading x from L2/HBM.  Softmax sums exp(x - max) (the safe one finds the max first), RMS norm sums x^2, layer
+// norm sums x for the mean and then (x - mean)^2, like the reference (layer_norm.cu:L62-72).
+enum RowOp { OP_SOFTMAX = 0, OP_SAFE_SOFTMAX = 1, OP_RMSNORM = 2, OP_RMSNORM_ACC16 = 3, OP_LAYERNORM = 4 };
 
 struct RowParams {
   float g, eps;
   int eps_inside_k;
+  float b;             // layer norm: bias
   const float* total;  // softmax mode 0: precomputed sum of exp over the whole tensor
 };
 
@@ -334,7 +293,8 @@ __global__ void __launch_bounds__(kThreads) row_kernel(const T* __restrict__ x, 
     uint4* yv = reinterpret_cast<uint4*>(y + (live ? row : 0) * int64_t(H));
     float v[MAXV * VN];
     float m = -INFINITY, s = 0.f;
-    float ml2 = 0.f;  // m * log2(e) for the safe softmax, 0 for the plain one
+    float ml2 = 0.f;   // m * log2(e) for the safe softmax, 0 for the plain one
+    float mean = 0.f;  // layer norm: the row sum, then its mean
     if (cached) {
 #pragma unroll
       for (int i = 0; i < MAXV; ++i) {
@@ -371,12 +331,15 @@ __global__ void __launch_bounds__(kThreads) row_kernel(const T* __restrict__ x, 
           hs = __hfma(h, h, hs);
         }
         s = __half2float(hs);
+      } else if constexpr (OP == OP_LAYERNORM) {
+#pragma unroll
+        for (int e = 0; e < MAXV * VN; ++e) mean += v[e];
       } else {
 #pragma unroll
         for (int e = 0; e < MAXV * VN; ++e) s = fmaf(v[e], v[e], s);
       }
     } else {
-      // long rows: stream x twice (three times for safe softmax)
+      // long rows: stream x twice (three times for safe softmax and layer norm)
       if constexpr (OP == OP_SAFE_SOFTMAX) {
         for (int vi = t; live && vi < nvec; vi += R) {
           float f[VN];
@@ -393,7 +356,30 @@ __global__ void __launch_bounds__(kThreads) row_kernel(const T* __restrict__ x, 
 #pragma unroll
         for (int e = 0; e < VN; ++e) {
           if constexpr (OP == OP_SAFE_SOFTMAX || OP == OP_SOFTMAX) s += exp_sub(f[e], ml2);
+          else if constexpr (OP == OP_LAYERNORM) mean += f[e];
           else s = fmaf(f[e], f[e], s);
+        }
+      }
+    }
+    if constexpr (OP == OP_LAYERNORM) {  // s = sum of (x - mean)^2, with the centred row kept in registers
+      mean = group_reduce<R, false>(mean, s_red) / float(H);
+      if (cached) {
+#pragma unroll
+        for (int i = 0; i < MAXV; ++i) {
+          const bool in = (t + i * R) < nvec;
+#pragma unroll
+          for (int e = 0; e < VN; ++e) {
+            const float d = in ? v[i * VN + e] - mean : 0.f;
+            v[i * VN + e] = d;
+            s = fmaf(d, d, s);
+          }
+        }
+      } else {
+        for (int vi = t; live && vi < nvec; vi += R) {
+          float f[VN];
+          IO::unpack(xv[vi], f);
+#pragma unroll
+          for (int e = 0; e < VN; ++e) s = fmaf(f[e] - mean, f[e] - mean, s);
         }
       }
     }
@@ -412,7 +398,10 @@ __global__ void __launch_bounds__(kThreads) row_kernel(const T* __restrict__ x, 
         if (live && vi < nvec) {
           float o[VN];
 #pragma unroll
-          for (int e = 0; e < VN; ++e) o[e] = v[i * VN + e] * scale;
+          for (int e = 0; e < VN; ++e) {
+            if constexpr (OP == OP_LAYERNORM) o[e] = fmaf(v[i * VN + e], scale, prm.b);
+            else o[e] = v[i * VN + e] * scale;
+          }
           __stcs(yv + vi, IO::pack(o));
         }
       }
@@ -423,6 +412,7 @@ __global__ void __launch_bounds__(kThreads) row_kernel(const T* __restrict__ x, 
 #pragma unroll
         for (int e = 0; e < VN; ++e) {
           if constexpr (OP == OP_SAFE_SOFTMAX || OP == OP_SOFTMAX) f[e] = exp_sub(f[e], ml2) * scale;
+          else if constexpr (OP == OP_LAYERNORM) f[e] = fmaf(f[e] - mean, scale, prm.b);
           else f[e] = f[e] * scale;
         }
         yv[vi] = IO::pack(f);
@@ -439,15 +429,20 @@ __global__ void __launch_bounds__(kThreads) row_kernel_scalar(const T* __restric
   for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
     const T* xr = x + row * int64_t(H);
     T* yr = y + row * int64_t(H);
-    float m = -INFINITY, s = 0.f;
+    float m = -INFINITY, s = 0.f, mean = 0.f;
     if constexpr (OP == OP_SAFE_SOFTMAX) {
       for (int i = threadIdx.x; i < H; i += kThreads) m = fmaxf(m, float(xr[i]));
       m = group_reduce<kThreads, true>(m, s_red);
+    } else if constexpr (OP == OP_LAYERNORM) {
+      float sum = 0.f;
+      for (int i = threadIdx.x; i < H; i += kThreads) sum += float(xr[i]);
+      mean = group_reduce<kThreads, false>(sum, s_red) / float(H);
     }
     const float ml2 = (OP == OP_SAFE_SOFTMAX) ? m * kLog2e : 0.f;
     for (int i = threadIdx.x; i < H; i += kThreads) {
       const float f = float(xr[i]);
       if constexpr (OP == OP_SAFE_SOFTMAX || OP == OP_SOFTMAX) s += exp_sub(f, ml2);
+      else if constexpr (OP == OP_LAYERNORM) s = fmaf(f - mean, f - mean, s);
       else s = fmaf(f, f, s);
     }
     if (!(OP == OP_SOFTMAX && prm.total != nullptr)) s = group_reduce<kThreads, false>(s, s_red);
@@ -461,6 +456,7 @@ __global__ void __launch_bounds__(kThreads) row_kernel_scalar(const T* __restric
     for (int i = threadIdx.x; i < H; i += kThreads) {
       float f = float(xr[i]);
       if constexpr (OP == OP_SAFE_SOFTMAX || OP == OP_SOFTMAX) f = exp_sub(f, ml2) * scale;
+      else if constexpr (OP == OP_LAYERNORM) f = fmaf(f - mean, scale, prm.b);
       else f = f * scale;
       yr[i] = T(f);
     }
@@ -718,12 +714,12 @@ extern "C" int b200k_softmax(const void* x, void* y, int64_t S, int64_t H, int d
   int rc = get_device_info(&di);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  RowParams prm = {1.f, 0.f, 0, nullptr};
+  RowParams prm = {1.f, 0.f, 0, 0.f, nullptr};
   if (mode == 0) {
     if (dtype != B200K_F32) return set_error(B200K_EDTYPE, "b200k_softmax: whole-tensor mode is f32 only (as in the reference)");
     if (!workspace) return set_error(B200K_EARG, "b200k_softmax: mode 0 needs a workspace");
     // total = sum(exp(x)) over the whole tensor (deterministic two-level reduction), then y = exp(x) / total.
-    float* total = reinterpret_cast<float*>(static_cast<char*>(workspace) + kReduceMaxBlocks * sizeof(float) + 128);
+    float* total = softmax_total(workspace);
     if ((rc = zero_ticket(workspace, s))) return rc;
     if ((rc = launch_reduce<B200K_F32, true>(x, total, S * H, 0, workspace, s, di))) return rc;
     prm.total = total;
@@ -748,12 +744,28 @@ extern "C" int b200k_rms_norm(const void* x, void* y, int64_t N, int64_t K, floa
   int rc = get_device_info(&di);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  RowParams prm = {g, eps, eps_inside_k, nullptr};
+  RowParams prm = {g, eps, eps_inside_k, 0.f, nullptr};
   if (dtype == B200K_F32) return launch_row<float, OP_RMSNORM>(x, y, N, K, prm, s, di);
   if (dtype == B200K_F16)
     return acc_f16 ? launch_row<__half, OP_RMSNORM_ACC16>(x, y, N, K, prm, s, di)
                    : launch_row<__half, OP_RMSNORM>(x, y, N, K, prm, s, di);
   return set_error(B200K_EDTYPE, "b200k_rms_norm: dtype %d not supported (f32, f16)", dtype);
+}
+
+extern "C" int b200k_layer_norm(const void* x, void* y, int64_t N, int64_t K, float g, float b, float eps, int dtype,
+                                int eps_inside_k, void* stream) {
+  if (!x || !y) return set_error(B200K_EARG, "b200k_layer_norm: null pointer");
+  if (N < 1 || K < 1 || K > INT32_MAX) return set_error(B200K_ESHAPE, "b200k_layer_norm: need N >= 1, 1 <= K < 2^31");
+  DeviceInfo di;
+  int rc = get_device_info(&di);
+  if (rc) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const RowParams prm = {g, eps, eps_inside_k, b, nullptr};
+  switch (dtype) {
+    case B200K_F32: return launch_row<float, OP_LAYERNORM>(x, y, N, K, prm, s, di);
+    case B200K_F16: return launch_row<__half, OP_LAYERNORM>(x, y, N, K, prm, s, di);
+    default: return set_error(B200K_EDTYPE, "b200k_layer_norm: dtype %d not supported (f32, f16)", dtype);
+  }
 }
 
 extern "C" int b200k_rope_f32(const void* x, void* out, int64_t seq_len, int64_t hidden, int ref_quirk, void* stream) {

@@ -1,11 +1,12 @@
-// HBM-roofline support kernels, second set (SURVEY.md section 8f-3): the seven activations, layer norm, dot product,
-// fp32 matrix transpose, GEMV.  Same recipe as support_kernels.cu: coalesced 128-bit accesses, several independent
-// loads in flight per thread, grids sized from the SM count, fp32 math on f16 I/O, no tensor cores.
+// HBM-roofline support kernels, second set (SURVEY.md section 8f-3): the seven activations, dot product, matrix
+// transposes, GEMV (layer norm, also of this set, is an op of the row kernel in support_kernels.cu).  Same recipe as
+// support_kernels.cu: coalesced 128-bit accesses, several independent loads in flight per thread, grids sized from the
+// SM count, fp32 math on f16 I/O, no tensor cores.
 //
 // Replaces (reference file:line)
 //   kernels/relu/relu.cu:L21-97              kernels/sigmoid/sigmoid.cu:L24-136        kernels/gelu/gelu.cu:L38-163
 //   kernels/swish/swish.cu:L20-97            kernels/elu/elu.cu:L35-120                kernels/hardswish/hardswish.cu:L36-140
-//   kernels/hardshrink/hardshrink.cu:L33-135 kernels/layer-norm/layer_norm.cu:L48-419  kernels/dot-product/dot_product.cu:L20-184
+//   kernels/hardshrink/hardshrink.cu:L33-135 kernels/dot-product/dot_product.cu:L20-184
 //   kernels/mat-transpose/mat_transpose.cu:L20-278   kernels/sgemv/sgemv.cu:L20-104    kernels/hgemv/hgemv.cu:L24-108
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -102,11 +103,12 @@ static int launch_act2(const void* x, void* y, int64_t n, bool clamp, cudaStream
   const int grid = grid_for(vec ? n / RowIO<T>::N : n, kThreads * 4, di.sm_count, 8);
   const T* xp = static_cast<const T*>(x);
   T* yp = static_cast<T*>(y);
-  // (the f32 sigmoid clamp at +-88.4 cannot change a flush-to-zero fp32 result: skip its two instructions per value)
-  if (clamp && ((OP == B200K_ACT_SIGMOID && sizeof(T) == 2) || OP == B200K_ACT_GELU))
-    activation_kernel<T, OP, true><<<grid, kThreads, 0, s>>>(xp, yp, n, vec);
-  else
-    activation_kernel<T, OP, false><<<grid, kThreads, 0, s>>>(xp, yp, n, vec);
+  auto kernel = activation_kernel<T, OP, false>;
+  // only sigmoid and gelu have a clamp, and the f32 sigmoid one at +-88.4 cannot change a flush-to-zero fp32 result:
+  // skip its two instructions per value
+  if constexpr ((OP == B200K_ACT_SIGMOID && sizeof(T) == 2) || OP == B200K_ACT_GELU)
+    if (clamp) kernel = activation_kernel<T, OP, true>;
+  kernel<<<grid, kThreads, 0, s>>>(xp, yp, n, vec);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -124,155 +126,15 @@ static int launch_act(const void* x, void* y, int64_t n, int op, bool clamp, cud
   }
 }
 
-// ============================================================================================ layer norm
-// One row per R threads with the row cached in registers: x is read once, y written once.  Two group reductions
-// (mean, then the centred sum of squares, like the reference: layer_norm.cu:L62-72).  Rows longer than 32 * R values
-// are re-read from L2 / HBM.
-template <typename T, int R>
-__global__ void __launch_bounds__(kThreads) layer_norm_kernel(const T* __restrict__ x, T* __restrict__ y, int64_t rows,
-                                                              int K, float g, float b, float eps, bool eps_inside_k) {
-  using IO = RowIO<T>;
-  constexpr int VN = IO::N;
-  constexpr int MAXV = 32 / VN;
-  constexpr int ROWS = kThreads / R;
-  __shared__ float s_red[kThreads / 32];
-  const int sub = threadIdx.x / R, t = threadIdx.x % R;
-  const int nvec = K / VN;
-  const bool cached = nvec <= MAXV * R;
-  for (int64_t row = int64_t(blockIdx.x) * ROWS + sub; row < ((rows + ROWS - 1) / ROWS) * ROWS;
-       row += int64_t(gridDim.x) * ROWS) {
-    const bool live = row < rows;  // the whole CTA stays in the loop: group_reduce uses __syncthreads when R > 32
-    const uint4* xv = reinterpret_cast<const uint4*>(x + (live ? row : 0) * int64_t(K));
-    uint4* yv = reinterpret_cast<uint4*>(y + (live ? row : 0) * int64_t(K));
-    float v[MAXV * VN];
-    float s = 0.f;
-    if (cached) {
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int vi = t + i * R;
-        if (live && vi < nvec) {
-          IO::unpack(__ldcs(xv + vi), v + i * VN);
-        } else {
-#pragma unroll
-          for (int e = 0; e < VN; ++e) v[i * VN + e] = 0.f;
-        }
-      }
-#pragma unroll
-      for (int e = 0; e < MAXV * VN; ++e) s += v[e];
-    } else {
-      for (int vi = t; live && vi < nvec; vi += R) {
-        float f[VN];
-        IO::unpack(xv[vi], f);
-#pragma unroll
-        for (int e = 0; e < VN; ++e) s += f[e];
-      }
-    }
-    const float mean = group_reduce<R, false>(s, s_red) / float(K);
-    float q = 0.f;
-    if (cached) {
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const bool in = (t + i * R) < nvec;
-#pragma unroll
-        for (int e = 0; e < VN; ++e) {
-          const float d = in ? v[i * VN + e] - mean : 0.f;
-          v[i * VN + e] = d;
-          q = fmaf(d, d, q);
-        }
-      }
-    } else {
-      for (int vi = t; live && vi < nvec; vi += R) {
-        float f[VN];
-        IO::unpack(xv[vi], f);
-#pragma unroll
-        for (int e = 0; e < VN; ++e) q = fmaf(f[e] - mean, f[e] - mean, q);
-      }
-    }
-    q = group_reduce<R, false>(q, s_red);
-    const float inv_std = rsqrtf(eps_inside_k ? q / (float(K) + eps) : q / float(K) + eps);
-    const float a = inv_std * g;
-    if (cached) {
-#pragma unroll
-      for (int i = 0; i < MAXV; ++i) {
-        const int vi = t + i * R;
-        if (live && vi < nvec) {
-          float o[VN];
-#pragma unroll
-          for (int e = 0; e < VN; ++e) o[e] = fmaf(v[i * VN + e], a, b);
-          __stcs(yv + vi, IO::pack(o));
-        }
-      }
-    } else {
-      for (int vi = t; live && vi < nvec; vi += R) {
-        float f[VN];
-        IO::unpack(xv[vi], f);
-#pragma unroll
-        for (int e = 0; e < VN; ++e) f[e] = fmaf(f[e] - mean, a, b);
-        yv[vi] = IO::pack(f);
-      }
-    }
-  }
-}
-
-// generic fallback: row length not a multiple of the pack, or unaligned
-template <typename T>
-__global__ void __launch_bounds__(kThreads) layer_norm_scalar_kernel(const T* __restrict__ x, T* __restrict__ y,
-                                                                     int64_t rows, int K, float g, float b, float eps,
-                                                                     bool eps_inside_k) {
-  __shared__ float s_red[kThreads / 32];
-  for (int64_t row = blockIdx.x; row < rows; row += gridDim.x) {
-    const T* xr = x + row * int64_t(K);
-    T* yr = y + row * int64_t(K);
-    float s = 0.f;
-    for (int i = threadIdx.x; i < K; i += kThreads) s += float(xr[i]);
-    const float mean = group_reduce<kThreads, false>(s, s_red) / float(K);
-    float q = 0.f;
-    for (int i = threadIdx.x; i < K; i += kThreads) q = fmaf(float(xr[i]) - mean, float(xr[i]) - mean, q);
-    q = group_reduce<kThreads, false>(q, s_red);
-    const float a = rsqrtf(eps_inside_k ? q / (float(K) + eps) : q / float(K) + eps) * g;
-    for (int i = threadIdx.x; i < K; i += kThreads) yr[i] = T(fmaf(float(xr[i]) - mean, a, b));
-    __syncthreads();
-  }
-}
-
-template <typename T>
-static int launch_layer_norm(const void* x, void* y, int64_t rows, int64_t K, float g, float b, float eps, bool inside,
-                             cudaStream_t s, const DeviceInfo& di) {
-  const T* xp = static_cast<const T*>(x);
-  T* yp = static_cast<T*>(y);
-  constexpr int VN = RowIO<T>::N;
-  if (K % VN == 0 && aligned16(x) && aligned16(y)) {
-    if (K <= 32 * 32) {
-      layer_norm_kernel<T, 32><<<grid_for(rows, kThreads / 32, di.sm_count, 16), kThreads, 0, s>>>(xp, yp, rows, int(K), g, b,
-                                                                                                  eps, inside);
-    } else if (K <= 32 * 128) {
-      layer_norm_kernel<T, 128><<<grid_for(rows, kThreads / 128, di.sm_count, 16), kThreads, 0, s>>>(xp, yp, rows, int(K), g,
-                                                                                                    b, eps, inside);
-    } else {
-      layer_norm_kernel<T, 256><<<grid_for(rows, 1, di.sm_count, 16), kThreads, 0, s>>>(xp, yp, rows, int(K), g, b, eps,
-                                                                                       inside);
-    }
-  } else {
-    layer_norm_scalar_kernel<T><<<grid_for(rows, 1, di.sm_count, 16), kThreads, 0, s>>>(xp, yp, rows, int(K), g, b, eps,
-                                                                                       inside);
-  }
-  B200K_CHECK_CUDA(cudaGetLastError());
-  return B200K_OK;
-}
-
 // ============================================================================================ dot product
-// Deterministic two-level reduction (per-CTA partial, the last CTA by ticket adds the partials in index order), as in
-// b200k_block_all_reduce_sum; the reference finishes with atomicAdd(float) in arrival order (dot_product.cu:L52,L76).
-constexpr int kDotMaxBlocks = kReduceMaxBlocks;  // same workspace layout as the all-reduce: partials, then the ticket
-
+// Deterministic two-level reduction (grid_sum), as in b200k_block_all_reduce_sum; the reference finishes with
+// atomicAdd(float) in arrival order (dot_product.cu:L52,L76).
 template <typename T>
 __global__ void __launch_bounds__(kThreads) dot_kernel(const T* __restrict__ a, const T* __restrict__ b,
                                                        float* __restrict__ out, int64_t n, void* __restrict__ workspace,
                                                        bool vec) {
   using IO = RowIO<T>;
   constexpr int VN = IO::N;
-  float* partials = reinterpret_cast<float*>(workspace);
-  unsigned int* ticket = reinterpret_cast<unsigned int*>(reinterpret_cast<char*>(workspace) + kDotMaxBlocks * sizeof(float));
   const int64_t stride = int64_t(gridDim.x) * kThreads;
   float acc[4] = {0.f, 0.f, 0.f, 0.f};
   int64_t done = 0;
@@ -302,118 +164,92 @@ __global__ void __launch_bounds__(kThreads) dot_kernel(const T* __restrict__ a, 
   }
   for (int64_t i = done + int64_t(blockIdx.x) * kThreads + threadIdx.x; i < n; i += stride)
     acc[0] = fmaf(float(a[i]), float(b[i]), acc[0]);
-  float v = (acc[0] + acc[1]) + (acc[2] + acc[3]);
-  __shared__ float s_part[kThreads / 32];
-  __shared__ bool s_last;
-  v = warp_sum(v);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  if (lane == 0) s_part[warp] = v;
-  __syncthreads();
-  if (warp == 0) {
-    float r = (lane < kThreads / 32) ? s_part[lane] : 0.f;
-    r = warp_sum(r);
-    if (lane == 0) {
-      partials[blockIdx.x] = r;
-      __threadfence();
-      s_last = (atomicAdd(ticket, 1u) == gridDim.x - 1);
-    }
-  }
-  __syncthreads();
-  if (s_last) {
-    __threadfence();
-    float r = 0.f;
-    for (int i = threadIdx.x; i < int(gridDim.x); i += kThreads) r += reinterpret_cast<volatile float*>(partials)[i];
-    r = warp_sum(r);
-    __syncthreads();
-    if (lane == 0) s_part[warp] = r;
-    __syncthreads();
-    if (threadIdx.x == 0) {
-      float t = 0.f;
-      for (int i = 0; i < kThreads / 32; ++i) t += s_part[i];
-      *out = t;
-      *ticket = 0;  // leave the workspace ready for the next call
-    }
-  }
+  grid_sum<float>((acc[0] + acc[1]) + (acc[2] + acc[3]), out, workspace);
 }
 
-// ============================================================================================ transpose (fp32)
-// y[N,M] = x[M,N]^T through a 64 x 64 shared-memory tile (row padded by one word: conflict-free both ways); global
-// reads and writes are both full 256-byte row segments.  The reference's 13 entry points differ only in their index
-// arithmetic (mat_transpose.cu:L29-278).
+template <typename T>
+static int launch_dot(const void* a, const void* b, void* out, int64_t n, void* ws, cudaStream_t s,
+                      const DeviceInfo& di) {
+  dot_kernel<T><<<reduce_grid(n / RowIO<T>::N, di.sm_count), kThreads, 0, s>>>(
+      static_cast<const T*>(a), static_cast<const T*>(b), static_cast<float*>(out), n, ws, aligned16(a) && aligned16(b));
+  B200K_CHECK_CUDA(cudaGetLastError());
+  return B200K_OK;
+}
+
+// ============================================================================================ transposes
+// y[b][N,M] = x[b][M,N]^T through a 64 x 64 shared-memory tile (each row padded by one 32-bit word: conflict-free both
+// ways); a warp reads and writes whole tile rows.  The reference's 13 fp32 entry points differ only in their index
+// arithmetic (mat_transpose.cu:L29-278).  The batched 16-bit form serves the drop-in `*_swizzle_qkv` attention entry
+// points for head dims above 128, which receive V as [B,H,D,N] while the FFPA kernel consumes [B,H,N,D].
 constexpr int kTile = 64;
-template <bool VEC4>
-__global__ void __launch_bounds__(kThreads) transpose_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int M,
-                                                                 int N, int tiles_n, int64_t tiles) {
-  __shared__ float tile[kTile][kTile + 1];
-  for (int64_t tidx = blockIdx.x; tidx < tiles; tidx += gridDim.x) {
-    const int tm = int(tidx / tiles_n), tn = int(tidx - int64_t(tm) * tiles_n);
-    const int m0 = tm * kTile, n0 = tn * kTile;
-    if constexpr (VEC4) {
-      // M % 4 == 0, N % 4 == 0, 16-byte aligned bases: 16-byte loads and stores, all four loads of a thread in flight
-      float4 v[4];
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;
-        if (m0 + r < M && n0 + c < N) v[k] = __ldcs(reinterpret_cast<const float4*>(x + int64_t(m0 + r) * N + n0 + c));
-      }
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;
-        tile[r][c] = v[k].x; tile[r][c + 1] = v[k].y; tile[r][c + 2] = v[k].z; tile[r][c + 3] = v[k].w;
-      }
-      __syncthreads();
-#pragma unroll
-      for (int k = 0; k < 4; ++k) {
-        const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;  // r: column of x, c: row of x
-        if (n0 + r < N && m0 + c < M)
-          __stcs(reinterpret_cast<float4*>(y + int64_t(n0 + r) * M + m0 + c),
-                 make_float4(tile[c][r], tile[c + 1][r], tile[c + 2][r], tile[c + 3][r]));
-      }
-    } else {
-      const int tx = threadIdx.x % kTile, ty = threadIdx.x / kTile;  // 64 x 4
-#pragma unroll 4
-      for (int r = ty; r < kTile; r += kThreads / kTile) {
-        const int m = m0 + r, nn = n0 + tx;
-        if (m < M && nn < N) tile[r][tx] = __ldcs(x + int64_t(m) * N + nn);
-      }
-      __syncthreads();
-#pragma unroll 4
-      for (int r = ty; r < kTile; r += kThreads / kTile) {
-        const int nn = n0 + r, m = m0 + tx;
-        if (nn < N && m < M) __stcs(y + int64_t(nn) * M + m, tile[tx][r]);
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// Batched transpose of 16-bit elements: y[b][N,M] = x[b][M,N]^T.  Used by the drop-in `*_swizzle_qkv` attention entry points
-// for head dims above 128, which receive V as [B,H,D,N] while the FFPA kernel consumes [B,H,N,D].  64 x 64 tiles through
-// shared memory (row padded by one 32-bit word), 4-byte global accesses both ways (2 elements), exact.
-__global__ void __launch_bounds__(kThreads) transpose_u16_batched_kernel(const uint16_t* __restrict__ x, uint16_t* __restrict__ y,
-                                                                         int M, int N, int tiles_m, int tiles_n, int64_t tiles) {
-  __shared__ uint16_t tile[kTile][kTile + 2];
+template <typename T>  // float, or uint16_t for any 16-bit type
+__global__ void __launch_bounds__(kThreads) transpose_kernel(const T* __restrict__ x, T* __restrict__ y, int M, int N,
+                                                             int tiles_m, int tiles_n, int64_t tiles) {
+  __shared__ T tile[kTile][kTile + 4 / sizeof(T)];
   const int64_t per_batch = int64_t(tiles_m) * tiles_n;
   for (int64_t tidx = blockIdx.x; tidx < tiles; tidx += gridDim.x) {
     const int64_t b = tidx / per_batch;
     const int t = int(tidx - b * per_batch);
     const int m0 = (t / tiles_n) * kTile, n0 = (t % tiles_n) * kTile;
-    const uint16_t* xb = x + b * int64_t(M) * N;
-    uint16_t* yb = y + b * int64_t(M) * N;
+    const T* xb = x + b * int64_t(M) * N;
+    T* yb = y + b * int64_t(M) * N;
     const int tx = threadIdx.x % kTile, ty = threadIdx.x / kTile;  // 64 x 4
 #pragma unroll 4
     for (int r = ty; r < kTile; r += kThreads / kTile) {
       const int m = m0 + r, nn = n0 + tx;
-      if (m < M && nn < N) tile[r][tx] = xb[int64_t(m) * N + nn];
+      if (m < M && nn < N) tile[r][tx] = __ldcs(xb + int64_t(m) * N + nn);
     }
     __syncthreads();
 #pragma unroll 4
     for (int r = ty; r < kTile; r += kThreads / kTile) {
       const int nn = n0 + r, m = m0 + tx;
-      if (nn < N && m < M) yb[int64_t(nn) * M + m] = tile[tx][r];
+      if (nn < N && m < M) __stcs(yb + int64_t(nn) * M + m, tile[tx][r]);
     }
     __syncthreads();
   }
+}
+
+// fp32 with M % 4 == 0, N % 4 == 0 and 16-byte aligned bases: 16-byte loads and stores, all four loads of a thread in
+// flight
+__global__ void __launch_bounds__(kThreads) transpose_f32x4_kernel(const float* __restrict__ x, float* __restrict__ y,
+                                                                   int M, int N, int tiles_n, int64_t tiles) {
+  __shared__ float tile[kTile][kTile + 1];
+  for (int64_t tidx = blockIdx.x; tidx < tiles; tidx += gridDim.x) {
+    const int tm = int(tidx / tiles_n), tn = int(tidx - int64_t(tm) * tiles_n);
+    const int m0 = tm * kTile, n0 = tn * kTile;
+    float4 v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;
+      if (m0 + r < M && n0 + c < N) v[k] = __ldcs(reinterpret_cast<const float4*>(x + int64_t(m0 + r) * N + n0 + c));
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;
+      tile[r][c] = v[k].x; tile[r][c + 1] = v[k].y; tile[r][c + 2] = v[k].z; tile[r][c + 3] = v[k].w;
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int idx = threadIdx.x + k * kThreads, r = idx >> 4, c = (idx & 15) * 4;  // r: column of x, c: row of x
+      if (n0 + r < N && m0 + c < M)
+        __stcs(reinterpret_cast<float4*>(y + int64_t(n0 + r) * M + m0 + c),
+               make_float4(tile[c][r], tile[c + 1][r], tile[c + 2][r], tile[c + 3][r]));
+    }
+    __syncthreads();
+  }
+}
+
+// Tiles of a batch of M x N matrices and the grid that walks them, one tile per CTA per pass.
+struct TileGrid {
+  int tiles_m, tiles_n;
+  int64_t tiles;
+  int grid;
+};
+static TileGrid tile_grid(int64_t batch, int64_t M, int64_t N, const DeviceInfo& di) {
+  const int tiles_m = int((M + kTile - 1) / kTile), tiles_n = int((N + kTile - 1) / kTile);
+  const int64_t tiles = batch * tiles_m * tiles_n;
+  return {tiles_m, tiles_n, tiles, grid_for(tiles, 1, di.sm_count, 16)};
 }
 
 // ============================================================================================ GEMV
@@ -479,21 +315,6 @@ extern "C" int b200k_activation(const void* x, void* y, int64_t n, int dtype, in
   }
 }
 
-extern "C" int b200k_layer_norm(const void* x, void* y, int64_t N, int64_t K, float g, float b, float eps, int dtype,
-                                int eps_inside_k, void* stream) {
-  if (!x || !y) return set_error(B200K_EARG, "b200k_layer_norm: null pointer");
-  if (N < 1 || K < 1 || K > INT32_MAX) return set_error(B200K_ESHAPE, "b200k_layer_norm: need N >= 1, 1 <= K < 2^31");
-  DeviceInfo di;
-  int rc = get_device_info(&di);
-  if (rc) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  switch (dtype) {
-    case B200K_F32: return launch_layer_norm<float>(x, y, N, K, g, b, eps, eps_inside_k != 0, s, di);
-    case B200K_F16: return launch_layer_norm<__half>(x, y, N, K, g, b, eps, eps_inside_k != 0, s, di);
-    default: return set_error(B200K_EDTYPE, "b200k_layer_norm: dtype %d not supported (f32, f16)", dtype);
-  }
-}
-
 extern "C" int b200k_dot_prod(const void* a, const void* b, void* out, int64_t n, int dtype, void* workspace,
                               void* stream) {
   if (!out || !workspace || ((!a || !b) && n > 0)) return set_error(B200K_EARG, "b200k_dot_prod: null pointer");
@@ -505,20 +326,8 @@ extern "C" int b200k_dot_prod(const void* a, const void* b, void* out, int64_t n
   if (dtype != B200K_F32 && dtype != B200K_F16)
     return set_error(B200K_EDTYPE, "b200k_dot_prod: dtype %d not supported (f32, f16)", dtype);
   if ((rc = zero_ticket(workspace, s))) return rc;
-  const bool vec = aligned16(a) && aligned16(b);
-  if (dtype == B200K_F32) {
-    int grid = grid_for(n / 4, kThreads * 4, di.sm_count, 8);
-    if (grid > kDotMaxBlocks) grid = kDotMaxBlocks;
-    dot_kernel<float><<<grid, kThreads, 0, s>>>(static_cast<const float*>(a), static_cast<const float*>(b),
-                                                static_cast<float*>(out), n, workspace, vec);
-  } else {
-    int grid = grid_for(n / 8, kThreads * 4, di.sm_count, 8);
-    if (grid > kDotMaxBlocks) grid = kDotMaxBlocks;
-    dot_kernel<__half><<<grid, kThreads, 0, s>>>(static_cast<const __half*>(a), static_cast<const __half*>(b),
-                                                 static_cast<float*>(out), n, workspace, vec);
-  }
-  B200K_CHECK_CUDA(cudaGetLastError());
-  return B200K_OK;
+  return dtype == B200K_F32 ? launch_dot<float>(a, b, out, n, workspace, s, di)
+                            : launch_dot<__half>(a, b, out, n, workspace, s, di);
 }
 
 extern "C" int b200k_mat_transpose_f32(const void* x, void* y, int64_t M, int64_t N, void* stream) {
@@ -529,15 +338,13 @@ extern "C" int b200k_mat_transpose_f32(const void* x, void* y, int64_t M, int64_
   int rc = get_device_info(&di);
   if (rc) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  const int tiles_m = int((M + kTile - 1) / kTile), tiles_n = int((N + kTile - 1) / kTile);
-  const int64_t tiles = int64_t(tiles_m) * tiles_n;
-  const int grid = grid_for(tiles, 1, di.sm_count, 16);
+  const TileGrid g = tile_grid(1, M, N, di);
   const float* xp = static_cast<const float*>(x);
   float* yp = static_cast<float*>(y);
   if (M % 4 == 0 && N % 4 == 0 && aligned16(x) && aligned16(y))
-    transpose_f32_kernel<true><<<grid, kThreads, 0, s>>>(xp, yp, int(M), int(N), tiles_n, tiles);
+    transpose_f32x4_kernel<<<g.grid, kThreads, 0, s>>>(xp, yp, int(M), int(N), g.tiles_n, g.tiles);
   else
-    transpose_f32_kernel<false><<<grid, kThreads, 0, s>>>(xp, yp, int(M), int(N), tiles_n, tiles);
+    transpose_kernel<float><<<g.grid, kThreads, 0, s>>>(xp, yp, int(M), int(N), g.tiles_m, g.tiles_n, g.tiles);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }
@@ -549,11 +356,9 @@ extern "C" int b200k_transpose_u16_batched(const void* x, void* y, int64_t batch
   DeviceInfo di;
   int rc = get_device_info(&di);
   if (rc) return rc;
-  const int tiles_m = int((M + kTile - 1) / kTile), tiles_n = int((N + kTile - 1) / kTile);
-  const int64_t tiles = batch * tiles_m * tiles_n;
-  const int grid = grid_for(tiles, 1, di.sm_count, 16);
-  transpose_u16_batched_kernel<<<grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
-      static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y), int(M), int(N), tiles_m, tiles_n, tiles);
+  const TileGrid g = tile_grid(batch, M, N, di);
+  transpose_kernel<uint16_t><<<g.grid, kThreads, 0, static_cast<cudaStream_t>(stream)>>>(
+      static_cast<const uint16_t*>(x), static_cast<uint16_t*>(y), int(M), int(N), g.tiles_m, g.tiles_n, g.tiles);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
 }

@@ -42,9 +42,9 @@ ROW_KERNELS = ("softmax", "rms_norm", "layer_norm")
 
 
 def row(dtype: str, rows: int, H: int, sm: int, aligned: bool = True) -> Plan:
-    """launch_row (softmax modes 1-3 and the normalisation pass of mode 0, rms_norm) and launch_layer_norm: the two
-    launchers make the same choices.  R threads own a row, 256 / R rows per CTA, at most 32 values of the row per
-    thread in registers."""
+    """launch_row, the one launcher of the row kernels (softmax modes 1-3 and the normalisation pass of mode 0,
+    rms_norm, layer_norm).  R threads own a row, 256 / R rows per CTA, at most 32 values of the row per thread in
+    registers."""
     vn = VN[dtype]
     if H % vn == 0 and aligned:
         R = 32 if H <= 32 * 32 else (128 if H <= 32 * 128 else 256)
@@ -52,7 +52,7 @@ def row(dtype: str, rows: int, H: int, sm: int, aligned: bool = True) -> Plan:
         grid = grid_for(rows, rows_per_cta, sm, 16)
         cached = H // vn <= (32 // vn) * R
         return Plan(True, grid, grid * rows_per_cta, "rows", R, cached)
-    grid = grid_for(rows, 1, sm, 16)  # row_kernel_scalar / layer_norm_scalar_kernel: one CTA per row
+    grid = grid_for(rows, 1, sm, 16)  # row_kernel_scalar: one CTA per row
     return Plan(False, grid, grid, "rows")
 
 

@@ -211,42 +211,33 @@ def timed_cases(torch, ops):
     return cases
 
 
-def main():
-    ap = argparse.ArgumentParser()
-    ap.add_argument("--build-base", metavar="REV", help="build REV's library into build_ab/base and exit")
-    ap.add_argument("--base-lib", default=BASE_LIB, help="the library to compare against (default: build_ab/base's)")
-    ap.add_argument("--rounds", type=int, default=9)
-    args = ap.parse_args()
-    if args.build_base:
-        build_base(args.build_base)
-        return
-
+def same_bits(a, b):
+    """Same dtype, shape and bytes: a NaN or a -0 counts like any other value."""
     import torch
 
-    if not torch.cuda.is_available():
-        sys.exit("gpu_ab_attention.py needs a CUDA device")
-    from b200k import _loader, ops
+    raw = [t.contiguous().reshape(-1).view(torch.uint8) for t in (a, b)]
+    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(*raw)
 
-    libs = {"base": load(args.base_lib), "new": _loader.lib}
-    info = gpu_info(torch)
-    print(json.dumps(dict(info, base_lib=os.path.relpath(os.path.abspath(args.base_lib), ROOT), rounds=args.rounds)),
-          flush=True)
 
+def compare_and_time(torch, libs, cases, timed, rounds, unit=("tflops", 1e-12)):
+    """Runs each (name, run) of `cases` through libs["base"] and libs["new"] and prints the ones whose outputs differ
+    in any bit, then times each (name, work, fn) of `timed` (a rate in `unit` = (name, scale) is work / time * scale).
+    Returns (differing cases, timed cases whose new median lies above the base's maximum)."""
     bad = 0
-    cases = equal_cases(torch, ops)
     for name, run in cases:
         outs = {}
         for key, lib in libs.items():
             with using(lib):
                 outs[key] = run()
-        same = all(torch.equal(a, b) for a, b in zip(outs["base"], outs["new"]))
+        same = len(outs["base"]) == len(outs["new"]) and all(same_bits(a, b) for a, b in zip(outs["base"], outs["new"]))
         bad += not same
         if not same:
             print(json.dumps({"case": name, "bit_equal": False}), flush=True)
-    print(json.dumps({"equal_cases": len(cases), "differing": bad}), flush=True)
+    if cases:
+        print(json.dumps({"equal_cases": len(cases), "differing": bad}), flush=True)
 
     slow = 0
-    for name, flop, fn in timed_cases(torch, ops):
+    for name, work, fn in timed:
         graphs, iters = {}, None
         for key, lib in libs.items():
             with using(lib):
@@ -275,7 +266,7 @@ def main():
         torch.cuda.synchronize()
         times = {k: [] for k in graphs}
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        for r in range(args.rounds):
+        for r in range(rounds):
             for key in (("base", "new") if r % 2 == 0 else ("new", "base")):
                 e0.record()
                 graphs[key].replay()
@@ -289,12 +280,37 @@ def main():
         for k, v in times.items():
             line[k + "_us"] = round(med[k], 2)
             line[k + "_min_max_us"] = [round(min(v), 2), round(max(v), 2)]
-            line[k + "_tflops"] = round(flop / (med[k] * 1e-6) * 1e-12, 1)
+            line[k + "_" + unit[0]] = round(work / (med[k] * 1e-6) * unit[1], 1)
         line["new_over_base"] = round(med["new"] / med["base"], 4)
         line["new_median_inside_base_range"] = inside
         print(json.dumps(line), flush=True)
         del graphs
         torch.cuda.empty_cache()
+    return bad, slow
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--build-base", metavar="REV", help="build REV's library into build_ab/base and exit")
+    ap.add_argument("--base-lib", default=BASE_LIB, help="the library to compare against (default: build_ab/base's)")
+    ap.add_argument("--rounds", type=int, default=9)
+    args = ap.parse_args()
+    if args.build_base:
+        build_base(args.build_base)
+        return
+
+    import torch
+
+    if not torch.cuda.is_available():
+        sys.exit("gpu_ab_attention.py needs a CUDA device")
+    from b200k import _loader, ops
+
+    libs = {"base": load(args.base_lib), "new": _loader.lib}
+    info = gpu_info(torch)
+    print(json.dumps(dict(info, base_lib=os.path.relpath(os.path.abspath(args.base_lib), ROOT), rounds=args.rounds)),
+          flush=True)
+
+    bad, slow = compare_and_time(torch, libs, equal_cases(torch, ops), timed_cases(torch, ops), args.rounds)
     print(json.dumps({"differing_cases": bad, "new_median_above_base_max": slow}), flush=True)
     sys.exit(1 if bad else 0)
 
