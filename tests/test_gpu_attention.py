@@ -130,7 +130,7 @@ def test_flash_attn_lib_and_ffpa_drop_in_entry_points():
 @pytest.mark.parametrize("shape", [(4, 48, 8192, 64), (1, 32, 4096, 512), (4, 64, 8192, 128)])
 def test_full_size_properties(shape):
     """BASELINE configs #3 / #4 / #5-shard.  Size-independent properties:
-       (1) V = ones  =>  O == 1 (rows of softmax sum to one), exactly representable in fp16 within 1e-3;
+       (1) V = ones  =>  O == 1 within 1e-3 at full size (test_gpu_attention_graded.py holds constant V to bit equality);
        (2) linearity in V: O(V1 + V2) == O(V1) + O(V2) within tolerance;
        (3) sampled query rows recomputed on the CPU oracle from the full K/V of their head."""
     B, H, N, D = shape

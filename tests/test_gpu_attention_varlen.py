@@ -189,7 +189,8 @@ def test_cuda_graph_capture_and_replay():
 
 
 def test_full_size_gqa_causal_properties():
-    """4 x 8192 tokens, H = 64, H_kv = 8, D = 128, causal: V = 1 gives O = 1, and sampled rows match an fp32 reference
+    """4 x 8192 tokens, H = 64, H_kv = 8, D = 128, causal: V = 1 gives O = 1 (within 1e-3 at this size; the contract, bit
+    equality, is held by test_gpu_attention_graded.py), and sampled rows match an fp32 reference
     computed on the GPU from the full K/V of their sequence and K/V head."""
     B, N, H, H_kv, D = 4, 8192, 64, 8, 128
     torch.manual_seed(21)
