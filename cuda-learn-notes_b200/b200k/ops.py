@@ -162,11 +162,22 @@ def _check_qkvo(q, k, v, o, v_is_dn=False, dtype=torch.float16):
     return B, H, N, D
 
 
+def _check_lse(lse: torch.Tensor, o: torch.Tensor) -> None:
+    """``lse`` must be fp32 of o's shape without its last dim, contiguous, on o's device."""
+    _check_dtype(lse, torch.float32)
+    if tuple(lse.shape) != tuple(o.shape[:-1]):
+        raise RuntimeError("Tensor size mismatch!")
+    _check_cuda_contig(o, lse)
+
+
 def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, variant: int = 0, causal: bool = False,
-            seqlens_k: Optional[torch.Tensor] = None) -> None:
+            seqlens_k: Optional[torch.Tensor] = None, lse: Optional[torch.Tensor] = None) -> None:
     """FA-2 forward, [B,H,N,D] fp16 (the reference's layout and dtype) or bf16.  ``causal`` and ``seqlens_k`` (int32 [B] on
-    the device: valid keys per batch) are the caller-facing options of SURVEY 8(f)-4; the reference has neither."""
+    the device: valid keys per batch) are the caller-facing options of SURVEY 8(f)-4; the reference has neither.
+    ``lse``: an fp32 [B, H, N] tensor that receives each row's softmax log-sum-exp (natural log; see :func:`attn_merge`)."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    if lse is not None:
+        _check_lse(lse, o)
     B, H, N, D = _check_qkvo(q, k, v, o, v_is_dn, dt)
     if D not in FA2_HEADDIMS:
         raise RuntimeError("headdim not support!")
@@ -177,6 +188,12 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
         if seqlens_k.numel() != B:
             raise RuntimeError("Tensor size mismatch!")
         sl = seqlens_k.data_ptr()
+    if lse is not None:
+        with _DeviceGuard(q):
+            L.check(_lib.b200k_fa2_fwd_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), B, H,
+                                           N, D, float(scale) if scale else 0.0, 1 if v_is_dn else 0, _DTYPE_ENUM[dt],
+                                           1 if causal else 0, sl, variant, _stream(q)))
+        return
     with _DeviceGuard(q):
         if dt == torch.float16 and not causal and seqlens_k is None:
             L.check(_lib.b200k_fa2_fwd_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, H, N, D,
@@ -188,12 +205,14 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
 
 
 def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
-                   scale: Optional[float] = None, causal: bool = False) -> None:
+                   scale: Optional[float] = None, causal: bool = False, lse: Optional[torch.Tensor] = None) -> None:
     """FA-2 forward on packed variable-length sequences (the forward of flash-attn's ``flash_attn_varlen_func``).
     q, o [total_q, H, D]; k, v [total_k, H_kv, D] with H % H_kv == 0 (query head h reads K/V head h // (H // H_kv));
     fp16 or bf16.  ``cu_seqlens_q`` / ``cu_seqlens_k``: int32 [B + 1] cumulative token offsets on the device.
     ``max_seqlen_q`` (a Python int, >= every query length) sizes the grid, so nothing is read back to the host.
-    ``causal`` is aligned bottom-right (row r sees keys <= r + Lk - Lq); rows that see no key are 0."""
+    ``causal`` is aligned bottom-right (row r sees keys <= r + Lk - Lq); rows that see no key are 0.
+    ``lse``: an fp32 [total_q, H] tensor that receives each row's softmax log-sum-exp (-inf for a row that sees no key);
+    tokens outside every sequence are left untouched, like o."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     for t in (q, k, v, o):
         _check_dtype(t, dt)
@@ -212,7 +231,16 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
     B = cu_seqlens_q.numel() - 1
     if B < 1 or cu_seqlens_k.numel() != B + 1:
         raise RuntimeError("Tensor size mismatch!")
+    if lse is not None:
+        _check_lse(lse, o)
     _check_cuda_contig(q, k, v, o, cu_seqlens_q, cu_seqlens_k)
+    if lse is not None:
+        with _DeviceGuard(q):
+            L.check(_lib.b200k_fa2_fwd_varlen_lse(
+                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), cu_seqlens_q.data_ptr(),
+                cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
+                float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+        return
     with _DeviceGuard(q):
         L.check(_lib.b200k_fa2_fwd_varlen(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), cu_seqlens_q.data_ptr(),
                                           cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
@@ -238,7 +266,8 @@ def fa2_fwd_kvcache_append_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D
 def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_table: Optional[torch.Tensor] = None,
                     scale: Optional[float] = None, causal: bool = False, *, k: Optional[torch.Tensor] = None,
                     v: Optional[torch.Tensor] = None, rotary_cos: Optional[torch.Tensor] = None,
-                    rotary_sin: Optional[torch.Tensor] = None, rotary_interleaved: bool = True) -> None:
+                    rotary_sin: Optional[torch.Tensor] = None, rotary_interleaved: bool = True,
+                    lse: Optional[torch.Tensor] = None) -> None:
     """Attention of the newest Lq query tokens of each sequence against its KV cache (flash-attn's
     ``flash_attn_with_kvcache``).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
     [B, S, H_kv, D] without ``block_table``, or [num_pages, page_size, H_kv, D] with an int32 ``block_table``
@@ -253,7 +282,10 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
     [rotary_seqlen, rotary_dim / 2] in q's dtype (rotary_dim a multiple of 16, at most D; rotary_seqlen at least the
     capacity) rotate the first rotary_dim columns of k and q: new key i at position cache_seqlens[b] + i, query token t
     at cache_seqlens[b] + t when causal and at cache_seqlens[b] when not.  ``rotary_interleaved`` pairs columns
-    (2j, 2j + 1); otherwise (j, j + rotary_dim / 2), GPT-NeoX style.  q is not modified."""
+    (2j, 2j + 1); otherwise (j, j + rotary_dim / 2), GPT-NeoX style.  q is not modified.
+
+    ``lse``: an fp32 [B, Lq, H] tensor that receives each row's softmax log-sum-exp over the keys it sees (-inf for
+    none), with or without ``k`` / ``v``."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     for t in (q, k_cache, v_cache, o):
         _check_dtype(t, dt)
@@ -282,6 +314,8 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
             raise RuntimeError("Tensor size mismatch!")
         pages_per_seq = block_table.size(1)
         tensors.append(block_table)
+    if lse is not None:
+        _check_lse(lse, o)
     rotary = rotary_cos is not None or rotary_sin is not None
     if k is not None or v is not None or rotary:
         if k is None or v is None:
@@ -305,24 +339,57 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
         with _DeviceGuard(q):
             nbytes = fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, rotary)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-            L.check(_lib.b200k_fa2_fwd_kvcache_append(
-                q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), cache_seqlens.data_ptr(),
-                block_table.data_ptr() if block_table is not None else None, k.data_ptr(), v.data_ptr(), k.size(1),
-                cos.data_ptr() if rotary else None, sin.data_ptr() if rotary else None,
-                cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0, 1 if rotary_interleaved else 0,
-                B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0,
-                _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr(), nbytes, _stream(q)))
+            args = (cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None,
+                    k.data_ptr(), v.data_ptr(), k.size(1), cos.data_ptr() if rotary else None,
+                    sin.data_ptr() if rotary else None, cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0,
+                    1 if rotary_interleaved else 0, B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq,
+                    float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr(), nbytes,
+                    _stream(q))
+            if lse is None:
+                L.check(_lib.b200k_fa2_fwd_kvcache_append(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                          o.data_ptr(), *args))
+            else:
+                L.check(_lib.b200k_fa2_fwd_kvcache_append_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
+                                                              o.data_ptr(), lse.data_ptr(), *args))
         return
     _check_cuda_contig(*tensors)
     with _DeviceGuard(q):
         nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
-        L.check(_lib.b200k_fa2_fwd_kvcache(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
-                                           cache_seqlens.data_ptr(),
-                                           block_table.data_ptr() if block_table is not None else None,
-                                           B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq,
-                                           float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0,
-                                           ws.data_ptr() if ws is not None else None, nbytes, _stream(q)))
+        args = (cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None,
+                B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0,
+                _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr() if ws is not None else None, nbytes, _stream(q))
+        if lse is None:
+            L.check(_lib.b200k_fa2_fwd_kvcache(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), *args))
+        else:
+            L.check(_lib.b200k_fa2_fwd_kvcache_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
+                                                   lse.data_ptr(), *args))
+
+
+def attn_merge(o_parts: torch.Tensor, lse_parts: torch.Tensor, o: torch.Tensor,
+               lse: Optional[torch.Tensor] = None) -> None:
+    """o (and lse) = the attention over the union of S disjoint key sets, from the attention over each: o_parts
+    [S, *o.shape] in o's dtype (fp16 or bf16) and lse_parts [S, *o.shape[:-1]] fp32, as the ``lse=`` outputs of
+    :func:`fa2_fwd`, :func:`fa2_fwd_varlen` and :func:`fa2_fwd_kvcache` give them.  Parts are weighted by
+    exp(lse_s - max) in fp32 and summed in ascending s (deterministic); a part with lse = -inf is skipped, and a row with
+    no part left is 0 with lse -inf.  ``lse`` (fp32, o.shape[:-1]) receives the merged log-sum-exp.  o must not overlap
+    o_parts; o.shape[-1] must be a multiple of 8."""
+    if o.dtype not in (torch.float16, torch.bfloat16):
+        raise RuntimeError("values must be torch::kHalf or torch::kBFloat16")
+    _check_dtype(o_parts, o.dtype)
+    _check_dtype(lse_parts, torch.float32)
+    if o.dim() < 1 or o_parts.dim() != o.dim() + 1 or tuple(o_parts.shape[1:]) != tuple(o.shape):
+        raise RuntimeError("Tensor size mismatch!")
+    S, D = o_parts.size(0), o.size(-1)
+    if tuple(lse_parts.shape) != (S,) + tuple(o.shape[:-1]):
+        raise RuntimeError("Tensor size mismatch!")
+    if lse is not None:
+        _check_lse(lse, o)
+    _check_cuda_contig(o_parts, lse_parts, o)
+    with _DeviceGuard(o):
+        L.check(_lib.b200k_attn_merge(o_parts.data_ptr(), lse_parts.data_ptr(), o.data_ptr(),
+                                      lse.data_ptr() if lse is not None else None, S, o.numel() // D if D else 0, D,
+                                      _DTYPE_ENUM[o.dtype], _stream(o)))
 
 
 def ffpa_fwd(q, k, v, o, scale: Optional[float] = None, variant: int = 0) -> None:

@@ -64,6 +64,12 @@ __device__ __forceinline__ uint32_t pack_round(float& lo, float& hi) {
   }
 }
 
+template <int DT>
+__device__ __forceinline__ float2 unpack2(uint32_t w) {
+  if constexpr (DT == 0) return __half22float2(*reinterpret_cast<const __half2*>(&w));
+  else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
+}
+
 // Row `row` of a 16-bit [rows, D] O from this thread's column pairs of accumulator row h (o[4 i + 2 h], o[4 i + 2 h + 1]
 // hold columns dv0 + 8 i + 2 (lane % 4) and the next), times inv, clipped to D columns (D is even).
 template <class Cfg>
@@ -86,7 +92,8 @@ struct KvTiles { int first, end; };
 // first row q0 (its rows are q0 .. q0 + BM - 1 in the numbering diag and store take), which setup fills (false: no rows
 // here; the CTA returns before any barrier exists); tiles, the KV tiles it visits; q_bytes and load_q, the bytes and the
 // box of 64-column chunk c of Q; kv_tile, where KV tile j is, for load_k (chunk c of K) and load_v (all of V); diag,
-// the causal diagonal (last key seen) of row r; zero_v_tail, which only decode fills in; store, the epilogue of row r.
+// the causal diagonal (last key seen) of row r; zero_v_tail, which only decode fills in; out_row, whether row r is
+// stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.
 
 // [B, H, N, D], one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).  CTA (x, y, z) =
 // (query tile, O column slice, batch * H + head).  Rows are numbered within the head, so row r sees keys <= r under the
@@ -131,9 +138,15 @@ struct AttnDense {
   }
   __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
   __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
+    if (r >= N) return false;
+    row = size_t(c.bh) * N + r;
+    return true;
+  }
   __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
                                         float, void* O, int D) const {
-    if (r < N) store_o<Cfg>(O, size_t(c.bh) * N + r, c.dv0, D, o, h, inv);
+    size_t row;
+    if (out_row(c, r, row)) store_o<Cfg>(O, row, c.dv0, D, o, h, inv);
   }
 };
 
@@ -183,13 +196,18 @@ struct AttnPacked {
   }
   __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
   __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ bool out_row(const Cta&, int r, size_t& row) const {
+    const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
+    if (r >= __ldg(cu_q + b + 1) - q_tok) return false;
+    const long long tok = (long long)q_tok + r;
+    if (tok < 0 || tok >= total_q) return false;
+    row = size_t(tok) * H + blockIdx.z % H;
+    return true;
+  }
   __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
                                         float, void* O, int D) const {
-    const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
-    if (r >= __ldg(cu_q + b + 1) - q_tok) return;
-    const long long tok = (long long)q_tok + r;
-    if (tok < 0 || tok >= total_q) return;
-    store_o<Cfg>(O, size_t(tok) * H + blockIdx.z % H, 0, D, o, h, inv);
+    size_t row;
+    if (out_row(c, r, row)) store_o<Cfg>(O, row, 0, D, o, h, inv);
   }
 };
 
@@ -280,11 +298,16 @@ struct AttnDecode {
     named_bar_sync(1, 128);
   }
   // rows past the box, the sequence or the group are not stored
+  __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
+    const int tt = r / hb, hh = r % hb;
+    if (tt >= T || c.t0 + tt >= Lq || c.h0 - c.kvh * group + hh >= group) return false;
+    row = (size_t(c.seq) * Lq + c.t0 + tt) * size_t(H) + c.h0 + hh;
+    return true;
+  }
   __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float m,
                                         float l, void* O, int D) const {
-    const int tt = r / hb, hh = r % hb;
-    if (tt >= T || c.t0 + tt >= Lq || c.h0 - c.kvh * group + hh >= group) return;
-    const size_t row = (size_t(c.seq) * Lq + c.t0 + tt) * size_t(H) + c.h0 + hh;
+    size_t row;
+    if (!out_row(c, r, row)) return;
     if (gridDim.x == 1) return store_o<Cfg>(O, row, 0, D, o, h, inv);
     // one split of several: O / l in fp32 and the base-2 log-sum-exp (-inf: no key seen)
     const int lane = threadIdx.x & 31;
@@ -296,6 +319,21 @@ struct AttnDecode {
       *reinterpret_cast<float2*>(dst + col) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
     }
     if ((lane & 3) == 0) lse[size_t(blockIdx.x) * size_t(rows) + row] = l > 0.f ? m + log2f(l) : -INFINITY;
+  }
+};
+
+// A mode that also writes each stored row's natural-log log-sum-exp to `lse` (fp32, indexed like the rows of O): m is
+// the row's final running max in base-2 units and l the sum of the rounded P that divides O, so O and lse describe
+// one softmax.  A row that saw no key gets -inf.  Decode takes it only unsplit; split rows are merged by the combine.
+template <class Mode>
+struct WithLse : Mode {
+  float* lse;
+  template <int N>
+  __device__ __forceinline__ void store(const typename Mode::Cta& c, int r, const float (&o)[N], int h, float inv,
+                                        float m, float l, void* O, int D) const {
+    Mode::store(c, r, o, h, inv, m, l, O, D);
+    size_t row;
+    if (Mode::out_row(c, r, row) && (threadIdx.x & 3) == 0) lse[row] = l > 0.f ? (m + log2f(l)) * 0.6931472f : -INFINITY;
   }
 };
 
@@ -505,16 +543,26 @@ static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t D
 }
 
 // Dense [B, H, N, D]: one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).
+// `args` as it is, or with its lse written when `lse` is not null.
+template <class Cfg, class Mode>
+static int launch_mode(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t D, float scale, const Mode& args,
+                       float* lse, cudaStream_t s, const DeviceInfo& di) {
+  if (lse) return launch_attn<Cfg>(qkv, grid, O, D, scale, WithLse<Mode>{args, lse}, s, di);
+  return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
+}
+
+// lse: null, or [B, H, N] fp32 (the D <= 128 configurations only).
 template <class Cfg>
 static int launch_dense(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
-                        float scale, const int* seqlens, int causal, cudaStream_t s, const DeviceInfo& di) {
+                        float scale, const int* seqlens, int causal, float* lse, cudaStream_t s, const DeviceInfo& di) {
   const int64_t BH = B * H;
   AttnTensor v = {V, BH, N, D, 1, Cfg::BN};
   if (Cfg::V_DN) v = {V, BH, D, N, 1, Cfg::DV};
   const AttnTensor qkv[3] = {{Q, BH, N, D, 1, Cfg::BM}, {K, BH, N, D, 1, Cfg::BN}, v};
   const dim3 grid(unsigned((N + Cfg::BM - 1) / Cfg::BM), unsigned((D + Cfg::DV - 1) / Cfg::DV), unsigned(BH));
   const AttnDense<Cfg> args = {seqlens, int(N), int(H), causal ? 1 : 0};
-  return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
+  if constexpr (Cfg::DV <= 128) return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
+  else return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
 }
 
 // The D <= 128 configurations: BN = 128 keys per tile; O columns DV = 64 for D = 32 / 64, 128 for D = 96 / 128.  V
@@ -534,32 +582,63 @@ static int check_headdim(const char* fn, int64_t D) {
   return B200K_OK;
 }
 
-// KV-cache decode with several splits: O[row] = sum_s 2^(lse_s - max) part_s[row] / sum_s 2^(lse_s - max), summed in
-// split order, so the result does not depend on which split finished first.  A split with no key for the row has
-// lse = -inf and adds nothing; a row no split saw a key for is 0.  One thread per (row, column pair).
-template <int DT>
-__global__ void attn_combine_kernel(const float* __restrict__ part, const float* __restrict__ lse, void* O, long long rows,
-                                    int D, int splits) {
-  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x, pairs = D / 2;
+// Merges `splits` partial attentions of each row over disjoint key sets: O[row] = sum_s 2^(t_s - max) part_s[row] /
+// sum_s 2^(t_s - max), summed in ascending s, so the result does not depend on which part finished first.  A part with
+// no key for the row has lse = -inf and adds nothing; a row no part saw a key for is 0.
+//   Part = float     KV-cache decode with several splits: fp32 O / l partials, t_s = lse_s in base 2.  One thread per
+//                    (row, column pair).
+//   Part = uint16_t  b200k_attn_merge: DT partials, t_s = lse_s * log2(e) from a natural-log lse; a part with
+//                    lse_s = -inf is skipped, so whatever its O holds (NaN included) never reaches the result.  One
+//                    thread per (row, 8 columns).
+// LSE: also write the merged natural-log lse of each row to lse_out ([rows]; -inf where no part saw a key).
+template <int DT, class Part = float, bool LSE = false>
+__global__ void attn_combine_kernel(const Part* __restrict__ part, const float* __restrict__ lse, void* O, long long rows,
+                                    int D, int splits, float* __restrict__ lse_out = nullptr) {
+  constexpr bool P16 = sizeof(Part) == 2;
+  constexpr int VEC = P16 ? 8 : 2;
+  const long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x, pairs = D / VEC;
   if (i >= rows * pairs) return;
   const long long row = i / pairs;
-  const int c = 2 * int(i % pairs);
+  const int c = VEC * int(i % pairs);
+  auto t = [&](int s) { return P16 ? lse[s * rows + row] * 1.4426950f : lse[s * rows + row]; };
   float mx = -INFINITY;
-  for (int s = 0; s < splits; ++s) mx = fmaxf(mx, lse[s * rows + row]);
-  float x = 0.f, y = 0.f, den = 0.f;
+  for (int s = 0; s < splits; ++s) mx = fmaxf(mx, t(s));
+  float x[VEC] = {}, den = 0.f;
   if (mx != -INFINITY) {
     for (int s = 0; s < splits; ++s) {
-      const float w = ex2(lse[s * rows + row] - mx);
-      const float2 p = *reinterpret_cast<const float2*>(part + (s * rows + row) * D + c);
-      x = fmaf(w, p.x, x);
-      y = fmaf(w, p.y, y);
+      const float ts = t(s);
+      if (P16 && ts == -INFINITY) continue;
+      const float w = ex2(ts - mx);
+      if constexpr (P16) {
+        const uint4 p = *reinterpret_cast<const uint4*>(part + (s * rows + row) * D + c);
+        const uint32_t pw[4] = {p.x, p.y, p.z, p.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          const float2 f = unpack2<DT>(pw[k]);
+          x[2 * k] = fmaf(w, f.x, x[2 * k]);
+          x[2 * k + 1] = fmaf(w, f.y, x[2 * k + 1]);
+        }
+      } else {
+        const float2 p = *reinterpret_cast<const float2*>(part + (s * rows + row) * D + c);
+        x[0] = fmaf(w, p.x, x[0]);
+        x[1] = fmaf(w, p.y, x[1]);
+      }
       den += w;
     }
   }
   const float inv = den > 0.f ? 1.f / den : 0.f;
-  x *= inv;
-  y *= inv;
-  *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row * D + c) = pack_round<DT>(x, y);
+  uint32_t out[VEC / 2];
+#pragma unroll
+  for (int k = 0; k < VEC / 2; ++k) {
+    x[2 * k] *= inv;
+    x[2 * k + 1] *= inv;
+    out[k] = pack_round<DT>(x[2 * k], x[2 * k + 1]);
+  }
+  uint16_t* dst = static_cast<uint16_t*>(O) + row * D + c;
+  if constexpr (P16) *reinterpret_cast<uint4*>(dst) = make_uint4(out[0], out[1], out[2], out[3]);
+  else *reinterpret_cast<uint32_t*>(dst) = out[0];
+  if constexpr (LSE)
+    if (c == 0) lse_out[row] = den > 0.f ? (mx + log2f(den)) * 0.6931472f : -INFINITY;
 }
 
 // KV-cache append (b200k_fa2_fwd_kvcache_append), in front of the decode kernel.  New token i of sequence b goes to cache
@@ -575,12 +654,6 @@ struct KvAppend {
   long long rotary_seqlen;
   int B, L_new, Lq, H, H_kv, D, page_size, pages_per_seq, rotary_dim, causal;
 };
-
-template <int DT>
-__device__ __forceinline__ float2 unpack2(uint32_t w) {
-  if constexpr (DT == 0) return __half22float2(*reinterpret_cast<const __half2*>(&w));
-  else return __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&w));
-}
 
 // Pair (x0, x1) at position pos becomes (x0 c - x1 s, x0 s + x1 c) in fp32, rounded once.  The products are not left to
 // contraction, so Q and K rows go through the same operations wherever this is inlined.
@@ -749,8 +822,9 @@ static int kvcache_args(const char* fn, const void* Q, const void* K_cache, cons
 }
 
 // Everything of a decode call after its workspace check: the decode kernel on `g`'s grid (Q read through a 3-D map,
-// lengths from `seqlens`), then the combine kernel when the call is split.  `part` is the split region of the workspace.
-static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cache, void* O, const int* seqlens,
+// lengths from `seqlens`), then the combine kernel when the call is split.  `part` is the split region of the workspace;
+// `lse` (null, or [B, Lq, H] fp32) is written by the decode kernel unsplit and by the combine kernel split.
+static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse, const int* seqlens,
                           const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
                           const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di) {
@@ -780,10 +854,15 @@ static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cach
                                {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
                                {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
     const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
+    if (g.splits == 1) return launch_mode<Cfg>(qkv, grid, O, D, scale, d, lse, s, di);
     const int launched = launch_attn<Cfg>(qkv, grid, O, D, scale, d, s, di);
-    if (launched || g.splits == 1) return launched;
+    if (launched) return launched;
     const long long work = d.rows * (D / 2);
-    attn_combine_kernel<Cfg::DT><<<unsigned((work + 255) / 256), 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
+    const unsigned blocks = unsigned((work + 255) / 256);
+    if (lse)
+      attn_combine_kernel<Cfg::DT, float, true><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits, lse);
+    else
+      attn_combine_kernel<Cfg::DT><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
     B200K_CHECK_CUDA(cudaGetLastError());
     return B200K_OK;
   });
@@ -835,9 +914,15 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
   if constexpr (DV == 192) {
     using Two = AttnCfg<0, DV, 2, 64, false>;
     if (Two::smem_bytes(int((D + 63) / 64)) <= di.max_smem_optin)
-      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, s, di);
+      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, nullptr, s, di);
   }
-  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, s, di);
+  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, nullptr, s, di);
+}
+
+// The one check an lse output adds to an attention call (null: no lse).
+static int check_lse(const char* fn, const float* lse) {
+  if (reinterpret_cast<uintptr_t>(lse) % 4) return set_error(B200K_EALIGN, "%s: lse must be 4-byte aligned", fn);
+  return B200K_OK;
 }
 
 }  // namespace b200k
@@ -850,6 +935,12 @@ extern "C" int b200k_fa2_fwd_f16(const void* Q, const void* K, const void* V, vo
 extern "C" int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,
                              int64_t D, float scale, int v_is_dn, int dtype, int causal, const int* seqlens_k, int variant,
                              void* stream) {
+  return b200k_fa2_fwd_lse(Q, K, V, O, nullptr, B, H, N, D, scale, v_is_dn, dtype, causal, seqlens_k, variant, stream);
+}
+
+extern "C" int b200k_fa2_fwd_lse(const void* Q, const void* K, const void* V, void* O, float* lse, int64_t B, int64_t H,
+                                 int64_t N, int64_t D, float scale, int v_is_dn, int dtype, int causal,
+                                 const int* seqlens_k, int variant, void* stream) {
   using namespace b200k;
   (void)variant;  // one configuration per head dim on this architecture
   if (dtype != B200K_F16 && dtype != B200K_BF16)
@@ -865,10 +956,13 @@ extern "C" int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* 
   if (v_is_dn && (N % 8))
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd: V stored [B,H,D,N] needs N %% 8 == 0 (16-byte rows), got N=%lld",
                      (long long)N);
+  if ((rc = check_lse("b200k_fa2_fwd_lse", lse))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  auto run = [&](auto cfg) { return launch_dense<decltype(cfg)>(Q, K, V, O, B, H, N, D, scale, seqlens_k, causal, s, di); };
+  auto run = [&](auto cfg) {
+    return launch_dense<decltype(cfg)>(Q, K, V, O, B, H, N, D, scale, seqlens_k, causal, lse, s, di);
+  };
   return v_is_dn ? run_attn_cfg<2, true>(dtype, D, run) : run_attn_cfg<2, false>(dtype, D, run);
 }
 
@@ -876,6 +970,14 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
                                     const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q,
                                     int64_t total_k, int64_t H, int64_t H_kv, int64_t D, float scale, int dtype,
                                     int causal, void* stream) {
+  return b200k_fa2_fwd_varlen_lse(Q, K, V, O, nullptr, cu_seqlens_q, cu_seqlens_k, B, max_seqlen_q, total_q, total_k, H,
+                                  H_kv, D, scale, dtype, causal, stream);
+}
+
+extern "C" int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void* V, void* O, float* lse,
+                                        const int* cu_seqlens_q, const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q,
+                                        int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv, int64_t D, float scale,
+                                        int dtype, int causal, void* stream) {
   using namespace b200k;
   if (!Q || !K || !V || !O || !cu_seqlens_q || !cu_seqlens_k)
     return set_error(B200K_EARG, "b200k_fa2_fwd_varlen: null pointer");
@@ -894,6 +996,7 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
   if (B > 65535 || H > 65535 || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: B * H = %lld CTAs per query tile, the grid allows 65535",
                      (long long)B * (long long)H);
+  if ((rc = check_lse("b200k_fa2_fwd_varlen_lse", lse))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -902,7 +1005,7 @@ extern "C" int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V,
     const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1}, {K, total_k, H_kv, D, Cfg::BN, 1}, {V, total_k, H_kv, D, Cfg::BN, 1}};
     const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
     const AttnPacked<Cfg> args = {cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
-    return launch_attn<Cfg>(qkv, grid, O, D, scale, args, s, di);
+    return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
   });
 }
 
@@ -923,18 +1026,28 @@ extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const v
                                      int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
                                      float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
                                      void* stream) {
+  return b200k_fa2_fwd_kvcache_lse(Q, K_cache, V_cache, O, nullptr, cache_seqlens, block_table, B, Lq, H, H_kv, D,
+                                   num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace, workspace_bytes,
+                                   stream);
+}
+
+extern "C" int b200k_fa2_fwd_kvcache_lse(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                                         const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq,
+                                         int64_t H, int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size,
+                                         int64_t pages_per_seq, float scale, int dtype, int causal, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
   using namespace b200k;
   const char* fn = "b200k_fa2_fwd_kvcache";
   int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
                         pages_per_seq, dtype);
-  if (rc) return rc;
+  if (rc || (rc = check_lse("b200k_fa2_fwd_kvcache_lse", lse))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
   if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
     return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: %zu workspace bytes needed, %zu given", g.workspace,
                      workspace ? workspace_bytes : size_t(0));
-  return kvcache_launch(Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+  return kvcache_launch(Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
                         pages_per_seq, scale, dtype, causal, g, workspace, static_cast<cudaStream_t>(stream), di);
 }
 
@@ -958,6 +1071,20 @@ extern "C" int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* 
                                             int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size,
                                             int64_t pages_per_seq, float scale, int dtype, int causal, void* workspace,
                                             size_t workspace_bytes, void* stream) {
+  return b200k_fa2_fwd_kvcache_append_lse(Q, K_cache, V_cache, O, nullptr, cache_seqlens, block_table, K_new, V_new, L_new,
+                                          rotary_cos, rotary_sin, rotary_seqlen, rotary_dim, rotary_interleaved, B, Lq, H,
+                                          H_kv, D, num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace,
+                                          workspace_bytes, stream);
+}
+
+extern "C" int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
+                                                const int* cache_seqlens, const int* block_table, const void* K_new,
+                                                const void* V_new, int64_t L_new, const void* rotary_cos,
+                                                const void* rotary_sin, int64_t rotary_seqlen, int64_t rotary_dim,
+                                                int rotary_interleaved, int64_t B, int64_t Lq, int64_t H, int64_t H_kv,
+                                                int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                                float scale, int dtype, int causal, void* workspace,
+                                                size_t workspace_bytes, void* stream) {
   using namespace b200k;
   const char* fn = "b200k_fa2_fwd_kvcache_append";
   int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
@@ -965,7 +1092,8 @@ extern "C" int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* 
   if (rc) return rc;
   const int64_t capacity = pages_per_seq * page_size;
   if ((rc = append_args(fn, Q, K_cache, V_cache, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, capacity,
-                        rotary_seqlen, rotary_dim, workspace)))
+                        rotary_seqlen, rotary_dim, workspace)) ||
+      (rc = check_lse("b200k_fa2_fwd_kvcache_append_lse", lse)))
     return rc;
   const bool rotary = rotary_cos != nullptr;
   DeviceInfo di;
@@ -1018,8 +1146,34 @@ extern "C" int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* 
                  : rotary_interleaved ? append(kvcache_append_kernel<0, true, true>) : append(kvcache_append_kernel<0, true, false>);
   if (rc) return rc;
   // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
-  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
+  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, lse, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
                         page_size, pages_per_seq, scale, dtype, causal, g, ws + lay.part, s, di);
+}
+
+extern "C" int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows,
+                                int64_t D, int dtype, void* stream) {
+  using namespace b200k;
+  if (!O_parts || !lse_parts || !O) return set_error(B200K_EARG, "b200k_attn_merge: null pointer");
+  if (dtype != B200K_F16 && dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "b200k_attn_merge: dtype %d not supported (f16, bf16)", dtype);
+  if (S < 1 || rows < 1 || D < 8 || D % 8 || S > INT32_MAX || D > INT32_MAX || rows > (int64_t(INT32_MAX) << 8) / (D / 8))
+    return set_error(B200K_ESHAPE, "b200k_attn_merge: need S, rows >= 1, D %% 8 == 0 and rows * D / 8 < 2^39 (got S=%lld "
+                     "rows=%lld D=%lld)", (long long)S, (long long)rows, (long long)D);
+  if (reinterpret_cast<uintptr_t>(O_parts) % 16 || reinterpret_cast<uintptr_t>(O) % 16 ||
+      reinterpret_cast<uintptr_t>(lse_parts) % 4 || reinterpret_cast<uintptr_t>(lse) % 4)
+    return set_error(B200K_EALIGN, "b200k_attn_merge: O_parts and O must be 16-byte aligned, lse_parts and lse 4-byte");
+  const long long work = rows * (D / 8);
+  const unsigned blocks = unsigned((work + 255) / 256);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const uint16_t* parts = static_cast<const uint16_t*>(O_parts);
+  auto merge = [&](auto kern) {
+    kern<<<blocks, 256, 0, s>>>(parts, lse_parts, O, rows, int(D), int(S), lse);
+    B200K_CHECK_CUDA(cudaGetLastError());
+    return B200K_OK;
+  };
+  if (dtype == B200K_BF16)
+    return lse ? merge(attn_combine_kernel<1, uint16_t, true>) : merge(attn_combine_kernel<1, uint16_t, false>);
+  return lse ? merge(attn_combine_kernel<0, uint16_t, true>) : merge(attn_combine_kernel<0, uint16_t, false>);
 }
 
 extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,

@@ -203,6 +203,64 @@ int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* V_cache, vo
 int b200k_fa2_fwd_kvcache_append_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                                  int64_t max_seqlen_k, int rotary, size_t* bytes);
 
+/* ------------------------------------------------------------------------------------------------ attention log-sum-exp
+ * The four *_lse calls below are the calls above with `float* lse` inserted right after O; everything else, checks,
+ * messages and return codes included, is the same, and lse == NULL is exactly the call without it (each call above is
+ * its *_lse form with lse = NULL).  They also write the softmax log-sum-exp of each query row (flash-attn's
+ * return_softmax_lse), so that attention results over disjoint key sets can be merged by b200k_attn_merge:
+ *   definition  lse[row] = ln sum_j exp(scale * q_row . k_j) over exactly the keys the row sees (length, key padding,
+ *               causal diagonal, cache length), fp32 in natural-log units.  The kernel forms it as
+ *               (m + log2f(l)) * 0.6931472f, m the row's final running max in base-2 units and l the same sum of rounded
+ *               P that divides O, so O and lse describe one softmax
+ *   empty rows  a row that sees no key gets -inf, the log of an empty sum (flash-attn writes +inf): -inf is what makes
+ *               such a part weigh nothing in a merge
+ *   layout      O's shape without its last dim, contiguous fp32, 4-byte aligned: dense [B, H, N] (as flash-attn), packed
+ *               [total_q, H], decode [B, Lq, H] (flash-attn uses [H, total_q] and [B, H, Lq]).  Every mode then has
+ *               rows = numel(O) / D with lse[row] belonging to O's row `row`, the indexing b200k_attn_merge takes
+ *   stores      lse is written for exactly the rows whose O is written (packed tokens outside every sequence are left
+ *               untouched, like O)
+ *   split       a split decode call writes the merged value (mx + log2f(den)) * ln 2 (or -inf) from its combine kernel;
+ *               the result stays deterministic.  The workspace functions are unchanged: lse needs no workspace
+ * D in {32, 64, 96, 128}; b200k_ffpa_fwd_f16 and b200k_fa2_fwd_f16 have no lse form.  Errors: those of the call without
+ * lse, then B200K_EALIGN for an lse that is not 4-byte aligned (before any CUDA call). */
+int b200k_fa2_fwd_lse(const void* Q, const void* K, const void* V, void* O, float* lse, int64_t B, int64_t H, int64_t N,
+                      int64_t D, float scale, int v_is_dn, int dtype, int causal, const int* seqlens_k, int variant,
+                      void* stream);
+/* Packed sequences (b200k_fa2_fwd_varlen): lse [total_q, H]. */
+int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void* V, void* O, float* lse, const int* cu_seqlens_q,
+                             const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k,
+                             int64_t H, int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* stream);
+/* KV-cache decode (b200k_fa2_fwd_kvcache): lse [B, Lq, H]. */
+int b200k_fa2_fwd_kvcache_lse(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                              const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq, int64_t H,
+                              int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                              float scale, int dtype, int causal, void* workspace, size_t workspace_bytes, void* stream);
+/* KV-cache decode with append (b200k_fa2_fwd_kvcache_append): lse [B, Lq, H], over the old keys plus the new ones. */
+int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
+                                     const int* cache_seqlens, const int* block_table, const void* K_new,
+                                     const void* V_new, int64_t L_new, const void* rotary_cos, const void* rotary_sin,
+                                     int64_t rotary_seqlen, int64_t rotary_dim, int rotary_interleaved,
+                                     int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                     int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                     float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+/* b200k_attn_merge — the attention over the union of S disjoint key sets from the attention over each (cascade /
+ * shared-prefix decode, chunked prefill, keys sharded across devices):
+ *   inputs      O_parts [S, rows, D] in dtype (B200K_F16 or B200K_BF16), lse_parts [S, rows] fp32 natural log, as the
+ *               *_lse calls write them; a dense [B, H, N, D] output is rows = B * H * N
+ *   outputs     O [rows, D] in dtype; lse [rows] fp32 natural log, or NULL.  O must not overlap O_parts
+ *   arithmetic  t_s = lse_s * 1.4426950f, mx = max_s t_s, w_s = 2^(t_s - mx) (ex2.approx.ftz); x = sum_s w_s O_s and
+ *               den = sum_s w_s in fp32, in ascending s; O = dtype(x * (1 / den)), lse = (mx + log2f(den)) * ln 2
+ *   empty parts a part with lse_s = -inf is skipped, so whatever its O holds (NaN included) never reaches the result; a
+ *               row where every part is -inf gets O = 0 and lse = -inf
+ *   guarantees  deterministic; no host sync, so the call can be captured in a CUDA graph.  The split-decode combine of
+ *               b200k_fa2_fwd_kvcache is the same kernel on fp32 base-2 partials
+ * Errors before any CUDA call: B200K_EARG for a null O_parts, lse_parts or O; B200K_EDTYPE; B200K_ESHAPE unless S,
+ * rows >= 1 and D % 8 == 0 (every row a whole number of 16-byte vectors); B200K_EALIGN unless O_parts and O are 16-byte
+ * and lse_parts and lse 4-byte aligned. */
+int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows, int64_t D,
+                     int dtype, void* stream);
+
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
 #define B200K_F32 0

@@ -36,6 +36,8 @@ def load(path):
 
     lib = ctypes.CDLL(os.path.abspath(path))
     for name, (res, argtypes) in _loader._SIGS.items():
+        if not hasattr(lib, name):  # an entry point the other build predates; no case here calls it
+            continue
         fn = getattr(lib, name)
         fn.restype = res
         fn.argtypes = argtypes
