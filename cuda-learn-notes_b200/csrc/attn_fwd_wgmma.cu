@@ -23,6 +23,7 @@
 
 #include <climits>
 #include <cmath>
+#include <initializer_list>
 
 namespace b200k {
 
@@ -582,6 +583,23 @@ static int check_headdim(const char* fn, int64_t D) {
   return B200K_OK;
 }
 
+// Alignment checks of the attention entry points, in order, before any CUDA call: the first pointer that is not a
+// multiple of its byte count is B200K_EALIGN, named in the message.  Null pointers pass (each call checks those it
+// needs).  The rules: Q, K, V, the caches, the new rows, cos / sin and workspaces 16 bytes (TMA maps, 16-byte loads
+// and stores, fp32 partials); O 4 bytes (32-bit stores of column pairs); lse and the int32 arrays 4 bytes.
+struct AlignRule {
+  const void* p;
+  const char* name;
+  unsigned bytes;
+};
+
+static int check_align(const char* fn, std::initializer_list<AlignRule> rules) {
+  for (const AlignRule& r : rules)
+    if (reinterpret_cast<uintptr_t>(r.p) % r.bytes)
+      return set_error(B200K_EALIGN, "%s: %s must be %u-byte aligned", fn, r.name, r.bytes);
+  return B200K_OK;
+}
+
 // Merges `splits` partial attentions of each row over disjoint key sets: O[row] = sum_s 2^(t_s - max) part_s[row] /
 // sum_s 2^(t_s - max), summed in ascending s, so the result does not depend on which part finished first.  A part with
 // no key for the row has lse = -inf and adds nothing; a row no part saw a key for is 0.
@@ -818,7 +836,8 @@ static int kvcache_args(const char* fn, const void* Q, const void* K_cache, cons
     return set_error(B200K_ESHAPE, "%s: a contiguous cache (no block table) is num_pages = B pages of page_size = S keys, "
                      "pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)", fn, (long long)num_pages,
                      (long long)pages_per_seq);
-  return B200K_OK;
+  return check_align(fn, {{Q, "Q", 16}, {K_cache, "K_cache", 16}, {V_cache, "V_cache", 16}, {O, "O", 4},
+                          {cache_seqlens, "cache_seqlens", 4}, {block_table, "block_table", 4}});
 }
 
 // Everything of a decode call after its workspace check: the decode kernel on `g`'s grid (Q read through a 3-D map,
@@ -884,9 +903,9 @@ static AppendLayout append_layout(int64_t B, int64_t Lq, int64_t H, int64_t D, b
 }
 
 // Checks of the append entry point beyond the decode call's (before any CUDA call).
-static int append_args(const char* fn, const void* Q, const void* K_cache, const void* V_cache, const void* K_new,
-                       const void* V_new, const void* cos, const void* sin, int64_t B, int64_t L_new, int64_t D,
-                       int64_t capacity, int64_t rotary_seqlen, int64_t rotary_dim, const void* workspace) {
+static int append_args(const char* fn, const void* K_new, const void* V_new, const void* cos, const void* sin, int64_t B,
+                       int64_t L_new, int64_t D, int64_t capacity, int64_t rotary_seqlen, int64_t rotary_dim,
+                       const void* workspace) {
   if (!K_new || !V_new) return set_error(B200K_EARG, "%s: null K_new / V_new", fn);
   if (!cos != !sin) return set_error(B200K_EARG, "%s: rotary needs both rotary_cos and rotary_sin", fn);
   if (L_new < 1 || L_new > INT32_MAX || B > INT32_MAX / L_new)
@@ -897,12 +916,8 @@ static int append_args(const char* fn, const void* Q, const void* K_cache, const
   if (cos && rotary_seqlen < capacity)
     return set_error(B200K_ESHAPE, "%s: rotary_seqlen %lld is below the cache capacity %lld", fn, (long long)rotary_seqlen,
                      (long long)capacity);
-  const void* aligned[] = {K_new, V_new, cos, sin, Q, K_cache, V_cache, workspace};
-  for (const void* p : aligned)
-    if (reinterpret_cast<uintptr_t>(p) % 16)
-      return set_error(B200K_EALIGN, "%s: K_new, V_new, rotary_cos, rotary_sin, Q, the caches and the workspace must be "
-                       "16-byte aligned", fn);
-  return B200K_OK;
+  return check_align(fn, {{K_new, "K_new", 16}, {V_new, "V_new", 16}, {cos, "rotary_cos", 16}, {sin, "rotary_sin", 16},
+                          {workspace, "workspace", 16}});
 }
 
 // Large head dims: O in column slices of DV = 192 or 256 (as few slices as possible, each a whole number of 64-column
@@ -920,10 +935,7 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
 }
 
 // The one check an lse output adds to an attention call (null: no lse).
-static int check_lse(const char* fn, const float* lse) {
-  if (reinterpret_cast<uintptr_t>(lse) % 4) return set_error(B200K_EALIGN, "%s: lse must be 4-byte aligned", fn);
-  return B200K_OK;
-}
+static int check_lse(const char* fn, const float* lse) { return check_align(fn, {{lse, "lse", 4}}); }
 
 }  // namespace b200k
 
@@ -956,7 +968,10 @@ extern "C" int b200k_fa2_fwd_lse(const void* Q, const void* K, const void* V, vo
   if (v_is_dn && (N % 8))
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd: V stored [B,H,D,N] needs N %% 8 == 0 (16-byte rows), got N=%lld",
                      (long long)N);
-  if ((rc = check_lse("b200k_fa2_fwd_lse", lse))) return rc;
+  if ((rc = check_align("b200k_fa2_fwd", {{Q, "Q", 16}, {K, "K", 16}, {V, "V", 16}, {O, "O", 4},
+                                          {seqlens_k, "seqlens_k", 4}})) ||
+      (rc = check_lse("b200k_fa2_fwd_lse", lse)))
+    return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -996,7 +1011,10 @@ extern "C" int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void
   if (B > 65535 || H > 65535 || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_fa2_fwd_varlen: B * H = %lld CTAs per query tile, the grid allows 65535",
                      (long long)B * (long long)H);
-  if ((rc = check_lse("b200k_fa2_fwd_varlen_lse", lse))) return rc;
+  if ((rc = check_align("b200k_fa2_fwd_varlen", {{Q, "Q", 16}, {K, "K", 16}, {V, "V", 16}, {O, "O", 4},
+                                                 {cu_seqlens_q, "cu_seqlens_q", 4}, {cu_seqlens_k, "cu_seqlens_k", 4}})) ||
+      (rc = check_lse("b200k_fa2_fwd_varlen_lse", lse)))
+    return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1040,7 +1058,9 @@ extern "C" int b200k_fa2_fwd_kvcache_lse(const void* Q, const void* K_cache, con
   const char* fn = "b200k_fa2_fwd_kvcache";
   int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
                         pages_per_seq, dtype);
-  if (rc || (rc = check_lse("b200k_fa2_fwd_kvcache_lse", lse))) return rc;
+  if (rc || (rc = check_align(fn, {{workspace, "workspace", 16}})) ||
+      (rc = check_lse("b200k_fa2_fwd_kvcache_lse", lse)))
+    return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
@@ -1091,8 +1111,8 @@ extern "C" int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, vo
                         pages_per_seq, dtype);
   if (rc) return rc;
   const int64_t capacity = pages_per_seq * page_size;
-  if ((rc = append_args(fn, Q, K_cache, V_cache, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, capacity,
-                        rotary_seqlen, rotary_dim, workspace)) ||
+  if ((rc = append_args(fn, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, capacity, rotary_seqlen, rotary_dim,
+                        workspace)) ||
       (rc = check_lse("b200k_fa2_fwd_kvcache_append_lse", lse)))
     return rc;
   const bool rotary = rotary_cos != nullptr;
@@ -1159,9 +1179,9 @@ extern "C" int b200k_attn_merge(const void* O_parts, const float* lse_parts, voi
   if (S < 1 || rows < 1 || D < 8 || D % 8 || S > INT32_MAX || D > INT32_MAX || rows > (int64_t(INT32_MAX) << 8) / (D / 8))
     return set_error(B200K_ESHAPE, "b200k_attn_merge: need S, rows >= 1, D %% 8 == 0 and rows * D / 8 < 2^39 (got S=%lld "
                      "rows=%lld D=%lld)", (long long)S, (long long)rows, (long long)D);
-  if (reinterpret_cast<uintptr_t>(O_parts) % 16 || reinterpret_cast<uintptr_t>(O) % 16 ||
-      reinterpret_cast<uintptr_t>(lse_parts) % 4 || reinterpret_cast<uintptr_t>(lse) % 4)
-    return set_error(B200K_EALIGN, "b200k_attn_merge: O_parts and O must be 16-byte aligned, lse_parts and lse 4-byte");
+  const int rc = check_align("b200k_attn_merge", {{O_parts, "O_parts", 16}, {lse_parts, "lse_parts", 4}, {O, "O", 16},
+                                                  {lse, "lse", 4}});
+  if (rc) return rc;
   const long long work = rows * (D / 8);
   const unsigned blocks = unsigned((work + 255) / 256);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -1186,9 +1206,9 @@ extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, v
     return set_error(B200K_EHEADDIM, "headdim not support! (b200k_ffpa_fwd_f16: D=%lld; supported 32 .. 1024 step 32)", (long long)D);
   if (B < 1 || H < 1 || N < 1 || N > INT32_MAX || B * H > 65535)
     return set_error(B200K_ESHAPE, "b200k_ffpa_fwd_f16: need B,H,N >= 1 and B*H <= 65535");
+  int rc = check_align("b200k_ffpa_fwd_f16", {{Q, "Q", 16}, {K, "K", 16}, {V, "V", 16}, {O, "O", 4}});
   DeviceInfo di;
-  int rc = get_device_info(&di);
-  if (rc) return rc;
+  if (rc || (rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const int nqc = int((D + 63) / 64), slices = (nqc + 3) / 4, chunks = (nqc + slices - 1) / slices;
   return chunks == 3 ? launch_ffpa<192>(Q, K, V, O, B, H, N, D, scale, s, di)

@@ -5,7 +5,9 @@
  *   - takes DEVICE pointers owned by the caller (never allocates, keeps no state between calls),
  *   - enqueues its kernels on `stream` (a cudaStream_t passed as void*; NULL = legacy default stream, which is
  *     what the reference launches on) and returns without synchronising,
- *   - returns B200K_OK or a negative B200K_E* code; b200k_last_error() gives the message for the calling thread.
+ *   - returns B200K_OK or a negative B200K_E* code; b200k_last_error() gives the message for the calling thread,
+ *   - needs every pointer aligned to its element size (a precondition the caller keeps: torch tensors always do);
+ *     where a call needs more, its comment says so.
  *
  * Each declaration cites the reference interface it replaces (paths relative to the reference repo root).
  * The Python side (cuda-learn-notes_b200/b200k/_loader.py) binds exactly these symbols with ctypes; the
@@ -24,7 +26,7 @@ extern "C" {
 #define B200K_OK 0
 #define B200K_EDTYPE (-1)   /* unsupported dtype / pack enum                         */
 #define B200K_ESHAPE (-2)   /* shape not supported (see each function)               */
-#define B200K_EALIGN (-3)   /* pointer or row pitch not 16-byte aligned              */
+#define B200K_EALIGN (-3)   /* pointer or row pitch below the alignment a call needs */
 #define B200K_EHEADDIM (-4) /* head dim not supported ("headdim not support!")       */
 #define B200K_ECUDA (-5)    /* a CUDA runtime / driver call failed                   */
 #define B200K_EARCH (-6)    /* current device is not compute capability 9.0 (H100)   */
@@ -93,6 +95,8 @@ int b200k_gemm_ex(const void* A, const void* B, void* C, int64_t M, int64_t N, i
  * variant: accepted for source compatibility and ignored; there is one configuration per head dim.  Both entry points run
  *   the same wgmma kernel (csrc/attn_fwd_wgmma.cu); head dims above 256 compute O in column slices of 192 or 256, each
  *   slice recomputing S = Q K^T.
+ * Alignment (every attention call below states its own): Q, K, V 16 bytes, O 4 bytes.  A pointer below its rule is
+ *   B200K_EALIGN, with the argument named in the message, before any CUDA call.
  */
 int b200k_fa2_fwd_f16(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N,
                       int64_t D, float scale, int v_is_dn, int variant, void* stream);
@@ -103,6 +107,7 @@ int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, void* O, int
  *   causal     != 0: query row r attends keys <= r; KV tiles above the diagonal are skipped, not masked
  *   seqlens_k  NULL, or int32 device array [B]: keys >= seqlens_k[b] are masked for batch b (key-padding mask of the
  *              padded [B,H,N,D] layout; 1 <= seqlens_k[b] <= N; every query row is still computed)
+ *   alignment  Q, K, V 16 bytes; O, seqlens_k 4 bytes
  * b200k_fa2_fwd_f16(...) == b200k_fa2_fwd(..., B200K_F16, 0, NULL, ...). */
 int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
                   float scale, int v_is_dn, int dtype, int causal, const int* seqlens_k, int variant, void* stream);
@@ -124,8 +129,10 @@ int b200k_fa2_fwd(const void* Q, const void* K, const void* V, void* O, int64_t 
  *   neighbours the last KV tile of a sequence also reads keys of the next one; they are masked to -inf, so with finite
  *              K/V each sequence's O has the same bits as when computed alone.  A non-finite V in a neighbouring
  *              sequence leaks through as 0 * Inf = NaN (the same contract as the padded keys of b200k_fa2_fwd)
+ *   alignment  Q, K, V 16 bytes; O, cu_seqlens_q, cu_seqlens_k 4 bytes
  * Errors: B200K_EARG for a null pointer, B200K_EDTYPE, B200K_EHEADDIM, and B200K_ESHAPE unless B >= 1, H, H_kv >= 1,
- * H % H_kv == 0, 1 <= max_seqlen_q <= total_q, 1 <= total_q, total_k <= INT32_MAX and B * H <= 65535. */
+ * H % H_kv == 0, 1 <= max_seqlen_q <= total_q, 1 <= total_q, total_k <= INT32_MAX and B * H <= 65535; then
+ * B200K_EALIGN. */
 int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, const int* cu_seqlens_q,
                          const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t total_k,
                          int64_t H, int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* stream);
@@ -151,11 +158,12 @@ int b200k_fa2_fwd_varlen(const void* Q, const void* K, const void* V, void* O, c
  *                  that is 0)
  *   no sync        nothing is read back to the host, so the call can be captured in a CUDA graph and replayed while
  *                  cache_seqlens and block_table change
+ *   alignment      Q, K_cache, V_cache, workspace 16 bytes; O, cache_seqlens, block_table 4 bytes
  * Errors before any CUDA call: B200K_EARG (null pointer), B200K_EDTYPE, B200K_EHEADDIM, B200K_ESHAPE (counts < 1,
  * H % H_kv, page_size, num_pages * page_size or B * Lq > INT32_MAX, grid limits: at most 65535 (token, head) tiles of
- * 64 rows per K/V head and B * H_kv <= 65535; without a table num_pages must be B and pages_per_seq 1).  After the device
- * query (the split count needs the SM count): B200K_EARG when workspace_bytes is below what the workspace function
- * reports. */
+ * 64 rows per K/V head and B * H_kv <= 65535; without a table num_pages must be B and pages_per_seq 1), B200K_EALIGN.
+ * After the device query (the split count needs the SM count): B200K_EARG when workspace_bytes is below what the
+ * workspace function reports. */
 int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const void* V_cache, void* O, const int* cache_seqlens,
                           const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
@@ -186,10 +194,12 @@ int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int6
  *                  rotated Q [B, Lq, H, D] (rotary only), then the split region, each on a 256-byte boundary
  *   no sync        nothing is read back to the host; the call and the caller's cache_seqlens += L_new can be captured
  *                  together in a CUDA graph
+ *   alignment      Q, K_cache, V_cache, K_new, V_new, rotary_cos, rotary_sin, workspace 16 bytes; O, cache_seqlens,
+ *                  block_table 4 bytes
  * Errors before any CUDA call: those of b200k_fa2_fwd_kvcache; B200K_EARG when K_new or V_new is NULL or only one of
  * rotary_cos / rotary_sin is given; B200K_ESHAPE for L_new < 1, B * L_new > INT32_MAX, a bad rotary_dim or rotary_seqlen
- * below the capacity; B200K_EALIGN unless K_new, V_new, rotary_cos, rotary_sin, Q, the caches and the workspace are
- * 16-byte aligned.  After the device query: B200K_EARG for a missing or short workspace. */
+ * below the capacity; B200K_EALIGN.  After the device query, still before the caches are written: B200K_EARG for a
+ * missing or short workspace. */
 int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* V_cache, void* O, const int* cache_seqlens,
                                  const int* block_table, const void* K_new, const void* V_new, int64_t L_new,
                                  const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
@@ -222,7 +232,8 @@ int b200k_fa2_fwd_kvcache_append_workspace_bytes(int64_t B, int64_t Lq, int64_t 
  *   split       a split decode call writes the merged value (mx + log2f(den)) * ln 2 (or -inf) from its combine kernel;
  *               the result stays deterministic.  The workspace functions are unchanged: lse needs no workspace
  * D in {32, 64, 96, 128}; b200k_ffpa_fwd_f16 and b200k_fa2_fwd_f16 have no lse form.  Errors: those of the call without
- * lse, then B200K_EALIGN for an lse that is not 4-byte aligned (before any CUDA call). */
+ * lse, then B200K_EALIGN for an lse that is not 4-byte aligned (before any CUDA call).
+ *   alignment  the pointers of the call without lse as that call states; lse 4 bytes */
 int b200k_fa2_fwd_lse(const void* Q, const void* K, const void* V, void* O, float* lse, int64_t B, int64_t H, int64_t N,
                       int64_t D, float scale, int v_is_dn, int dtype, int causal, const int* seqlens_k, int variant,
                       void* stream);
@@ -256,8 +267,8 @@ int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, void* V_cache
  *   guarantees  deterministic; no host sync, so the call can be captured in a CUDA graph.  The split-decode combine of
  *               b200k_fa2_fwd_kvcache is the same kernel on fp32 base-2 partials
  * Errors before any CUDA call: B200K_EARG for a null O_parts, lse_parts or O; B200K_EDTYPE; B200K_ESHAPE unless S,
- * rows >= 1 and D % 8 == 0 (every row a whole number of 16-byte vectors); B200K_EALIGN unless O_parts and O are 16-byte
- * and lse_parts and lse 4-byte aligned. */
+ * rows >= 1 and D % 8 == 0 (every row a whole number of 16-byte vectors); B200K_EALIGN.
+ *   alignment   O_parts, O 16 bytes (16-byte loads and stores); lse_parts, lse 4 bytes */
 int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows, int64_t D,
                      int dtype, void* stream);
 
