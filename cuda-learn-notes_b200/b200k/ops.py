@@ -392,6 +392,73 @@ def attn_merge(o_parts: torch.Tensor, lse_parts: torch.Tensor, o: torch.Tensor,
                                       _DTYPE_ENUM[o.dtype], _stream(o)))
 
 
+def fa2_bwd_workspace_bytes(B: int, H: int, N: int) -> int:
+    """Workspace bytes :func:`fa2_bwd` needs for these shapes."""
+    n = ctypes.c_size_t(0)
+    L.check(_lib.b200k_fa2_bwd_workspace_bytes(B, H, N, ctypes.byref(n)))
+    return n.value
+
+
+def fa2_bwd(q, k, v, o, lse, do, dq, dk, dv, scale: Optional[float] = None, causal: bool = False,
+            seqlens_k: Optional[torch.Tensor] = None) -> None:
+    """Gradients of :func:`fa2_fwd` (dense [B, H, N, D], fp16 or bf16) into dq, dk, dv: o and ``lse`` (fp32 [B, H, N])
+    are what ``fa2_fwd(q, k, v, o, scale, causal=causal, seqlens_k=seqlens_k, lse=lse)`` wrote, ``do`` the gradient of
+    o.  ``scale``, ``causal`` and ``seqlens_k`` must be the forward's.  Deterministic (no atomics), and nothing is read
+    back to the host, so the call can be captured in a CUDA graph; the workspace is allocated per call on the current
+    stream."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    for t in (q, k, v, o, do, dq, dk, dv):
+        _check_dtype(t, dt)
+    if q.dim() != 4 or any(tuple(t.shape) != tuple(q.shape) for t in (k, v, o, do, dq, dk, dv)):
+        raise RuntimeError("Tensor size mismatch!")
+    B, H, N, D = q.shape
+    if D not in FA2_HEADDIMS:
+        raise RuntimeError("headdim not support!")
+    tensors = [q, k, v, o, lse, do, dq, dk, dv]
+    sl = None
+    if seqlens_k is not None:
+        _check_dtype(seqlens_k, torch.int32)
+        if seqlens_k.numel() != B:
+            raise RuntimeError("Tensor size mismatch!")
+        tensors.append(seqlens_k)
+        sl = seqlens_k.data_ptr()
+    _check_lse(lse, o)
+    _check_cuda_contig(*tensors)
+    with _DeviceGuard(q):
+        nbytes = fa2_bwd_workspace_bytes(B, H, N)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+        L.check(_lib.b200k_fa2_bwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), do.data_ptr(),
+                                   dq.data_ptr(), dk.data_ptr(), dv.data_ptr(), B, H, N, D,
+                                   float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, sl,
+                                   ws.data_ptr(), nbytes, _stream(q)))
+
+
+class _Attention(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, scale, causal, seqlens_k):
+        o = torch.empty_like(q)
+        lse = torch.empty(q.shape[:-1], dtype=torch.float32, device=q.device)
+        fa2_fwd(q, k, v, o, scale, causal=causal, seqlens_k=seqlens_k, lse=lse)
+        ctx.save_for_backward(q, k, v, o, lse)
+        ctx.scale, ctx.causal, ctx.seqlens_k = scale, causal, seqlens_k
+        return o
+
+    @staticmethod
+    def backward(ctx, grad):
+        q, k, v, o, lse = ctx.saved_tensors
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        fa2_bwd(q, k, v, o, lse, grad.contiguous(), dq, dk, dv, ctx.scale, ctx.causal, ctx.seqlens_k)
+        return dq, dk, dv, None, None, None
+
+
+def attention(q, k, v, scale: Optional[float] = None, causal: bool = False,
+              seqlens_k: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """Differentiable attention, dense [B, H, N, D] fp16 or bf16 (D in 32, 64, 96, 128): returns
+    o = softmax(q k^T * scale (masked)) v from :func:`fa2_fwd`, and its backward is :func:`fa2_bwd`, which gives the
+    gradients of q, k and v (``seqlens_k``, int32 [B]: valid keys per batch, is not differentiable)."""
+    return _Attention.apply(q, k, v, scale, causal, seqlens_k)
+
+
 def ffpa_fwd(q, k, v, o, scale: Optional[float] = None, variant: int = 0) -> None:
     B, H, N, D = _check_qkvo(q, k, v, o)
     with _DeviceGuard(q):

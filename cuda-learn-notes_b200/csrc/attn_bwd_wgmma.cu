@@ -1,0 +1,479 @@
+// Attention backward on Hopper (sm_90a), dense [B, H, N, D]: dQ, dK and dV of O = softmax(Q K^T * scale) V from Q, K,
+// V, O, dO and the forward's log-sum-exp (b200k_fa2_fwd_lse), the FlashAttention-2 algorithm with every output element
+// summed in one thread's registers, so the result is deterministic without atomics.  Three kernels, in stream order:
+//   prep    Delta_i = sum_d dO_id O_id and lse_i * log2 e into the workspace (bandwidth kernel, no tensor cores)
+//   dK/dV   one CTA per (64-key tile, b * H + h); K and V resident, Q / dO tiles of 64 rows streamed through a TMA +
+//           mbarrier ring.  One consumer warpgroup owns the 64 keys:
+//             S^T = K Q_i^T, dP^T = V dO_i^T   wgmma_ss, K-major operands
+//             P^T = 2^(S^T scale log2 e - lse_i log2 e), dS^T = P^T (dP^T - Delta_i), in registers
+//             dV += P~^T dO_i, dK += dS~^T Q_i  wgmma_rs (the accumulator fragment of S^T / dP^T is the A fragment),
+//                                               dO_i and Q_i read MN-major as V is in the forward's P V
+//   dQ      one CTA per (128-row query tile, b * H + h), the forward's geometry and its AttnDense addressing; Q and dO
+//           resident, K / V tiles of 64 keys streamed.  Two consumer warpgroups of 64 rows: S = Q K_j^T,
+//           dP = dO V_j^T, P, dS, dQ += dS~ K_j (K read MN-major)
+// P~ and dS~ are P and dS rounded to the 16-bit dtype.  S and dP are computed by both the dK/dV and the dQ kernel:
+// 7 products where an atomic-dQ backward needs 5, the price of determinism.
+// The dK/dV warpgroup holds dK, dV (2 x DP / 2 fp32) and S^T, dP^T (2 x 32): 192 at DP = 128, more than a 384-thread
+// block gives a thread (168), so it runs one consumer warpgroup in a 256-thread block.
+#include "attn_common.cuh"
+
+#include <climits>
+#include <cmath>
+
+namespace b200k {
+
+// The dK/dV kernel's config is AttnCfg<DT, DP, 1, 64, false> (BM = BN = 64, 256 threads), the dQ kernel's
+// AttnCfg<DT, DP, 2, 64, false> (BM = 128 rows, BN = 64 keys, 384 threads).  DP is the head dim padded to whole 64-column
+// chunks (64 for D = 32 / 64, 128 for D = 96 / 128); TMA zero-fills the padding.
+constexpr int kBwdStages = 2;
+
+// Delta[row] = sum_d dO[row, d] O[row, d] and lse2[row] = lse[row] * log2 e, one row per quad of threads, 16-byte loads,
+// each thread's products summed in column order, then across the quad in a fixed order.
+template <int DT>
+__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
+                                                            const float* __restrict__ lse, float* __restrict__ delta,
+                                                            float* __restrict__ lse2, long long rows, int D) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const int t = threadIdx.x & 3, lane = threadIdx.x & 31;
+  // the loop bound is the same for the whole warp (its first thread's index), so the shuffles see every lane
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i - lane < rows * 4; i += stride) {
+    const long long row = i / 4;
+    float acc = 0.f;
+    if (row < rows)
+      for (int v = t; v < D / 8; v += 4) {
+        const uint4 a = __ldg(reinterpret_cast<const uint4*>(O + row * D) + v);
+        const uint4 b = __ldg(reinterpret_cast<const uint4*>(dO + row * D) + v);
+        const uint32_t aw[4] = {a.x, a.y, a.z, a.w}, bw[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int k = 0; k < 4; ++k) {
+          float2 x, y;
+          if constexpr (DT == 0) {
+            x = __half22float2(*reinterpret_cast<const __half2*>(&aw[k]));
+            y = __half22float2(*reinterpret_cast<const __half2*>(&bw[k]));
+          } else {
+            x = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&aw[k]));
+            y = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(&bw[k]));
+          }
+          acc = fmaf(x.x, y.x, acc);
+          acc = fmaf(x.y, y.y, acc);
+        }
+      }
+    acc += __shfl_xor_sync(0xffffffffu, acc, 1);
+    acc += __shfl_xor_sync(0xffffffffu, acc, 2);
+    if (row < rows && t == 0) {
+      delta[row] = acc;
+      lse2[row] = lse[row] * 1.4426950408889634f;
+    }
+  }
+}
+
+// What both main kernels take beyond their tensor maps.
+struct BwdArgs {
+  const float* lse2;   // [B * H * N] lse * log2 e
+  const float* delta;  // [B * H * N]
+  void* dst[2];        // dK / dV kernel: dK, dV; dQ kernel: dQ
+  int D;
+  float scale_log2, scale;
+};
+
+// Rows past a CTA's query rows (ragged N) have zero-filled Q and dO; lse2 = +inf there makes their P exactly 0.
+__device__ __forceinline__ void load_row_stats(const BwdArgs& a, size_t base, int r, int N, float& l2, float& dl) {
+  l2 = r < N ? __ldg(a.lse2 + base + r) : INFINITY;
+  dl = r < N ? __ldg(a.delta + base + r) : 0.f;
+}
+
+// dK, dV of one 64-key tile.  CTA (x, y) = (key tile, b * H + h).  Warpgroup 0 produces (one thread issues TMA),
+// warpgroup 1 computes; thread rows (keys) k0 + 16 warp + lane / 4 and + 8, columns (queries) q0 + 8 j + 2 (lane % 4) + e.
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::THREADS, 1)
+    attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                         const BwdArgs a, const int* seqlens, int N, int H, int causal) {
+  static_assert(Cfg::NWG == 1 && Cfg::BM == 64 && Cfg::BN == 64, "dK/dV: one warpgroup of 64 keys, query tiles of 64");
+  constexpr int DP = Cfg::DV, NC = DP / 64, TILE = 64 * DP * 2, ST = kBwdStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t sK = (smem_u32(smem_raw) + 1023) & ~1023u, sV = sK + TILE, sQ = sV + TILE;  // stage s: Q, then dO
+  const uint32_t kvbar = sQ + ST * 2 * TILE, full = kvbar + 8, empty = full + 8 * ST;
+
+  const int bh = blockIdx.y, k0 = blockIdx.x * 64;
+  const int kv_len = seqlens ? min(max(__ldg(seqlens + bh / H), 1), N) : N;
+  // query tiles that see a key of this tile: all of them, from the one holding row k0 when causal; none past the length
+  const int first = causal ? k0 / 64 : 0, end = k0 < kv_len ? (N + 63) / 64 : first;
+  const int wg = threadIdx.x / 128;
+
+  if (threadIdx.x == 0) {
+    mbar_init(kvbar, 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(full + 8 * s, 1);
+      mbar_init(empty + 8 * s, 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    if (threadIdx.x == 0 && first < end) {
+      mbar_arrive_expect_tx(kvbar, 2 * TILE);
+      for (int c = 0; c < NC; ++c) {
+        tma_load_3d(sK + c * 8192, &tmK, kvbar, c * 64, k0, bh, kPolicyEvictFirst);
+        tma_load_3d(sV + c * 8192, &tmV, kvbar, c * 64, k0, bh, kPolicyEvictFirst);
+      }
+      for (int i = first; i < end; ++i) {
+        const int n = i - first, s = n % ST;
+        if (n >= ST) mbar_wait_nocall(empty + 8 * s, ((n / ST) - 1) & 1);
+        mbar_arrive_expect_tx(full + 8 * s, 2 * TILE);
+        const uint32_t q = sQ + s * 2 * TILE;
+        for (int c = 0; c < NC; ++c) {
+          tma_load_3d(q + c * 8192, &tmQ, full + 8 * s, c * 64, i * 64, bh, kPolicyEvictNormal);
+          tma_load_3d(q + TILE + c * 8192, &tmdO, full + 8 * s, c * 64, i * 64, bh, kPolicyEvictNormal);
+        }
+      }
+    }
+    return;
+  }
+
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
+  const int key0 = k0 + warp * 16 + lane / 4;  // this thread's keys: key0 and key0 + 8
+  const size_t base = size_t(bh) * N;
+  float dk[DP / 2], dv[DP / 2];
+#pragma unroll
+  for (int i = 0; i < DP / 2; ++i) dk[i] = dv[i] = 0.f;
+  if (first < end) mbar_wait_nocall(kvbar, 0);
+
+  for (int i = first; i < end; ++i) {
+    const int n = i - first, s = n % ST, q0 = i * 64;
+    const uint32_t sq = sQ + s * 2 * TILE, sdo = sq + TILE;
+    float st[32], dpt[32];
+#pragma unroll
+    for (int e = 0; e < 32; ++e) st[e] = dpt[e] = 0.f;
+    mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
+    fence_regs<32>(st);
+    fence_regs<32>(dpt);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<Cfg::DT, 64, 0, 0>(st, wgmma_desc(sK + c * 8192 + k * 32, 16, 1024),
+                                    wgmma_desc(sq + c * 8192 + k * 32, 16, 1024), 1);
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<Cfg::DT, 64, 0, 0>(dpt, wgmma_desc(sV + c * 8192 + k * 32, 16, 1024),
+                                    wgmma_desc(sdo + c * 8192 + k * 32, 16, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<32>(st);
+    fence_regs<32>(dpt);
+
+    // masks: keys past the length, and (causal) keys after the query's diagonal.  A masked score becomes -inf (P = 0)
+    // and its dP 0, so nothing a padded key holds reaches dS.
+    if (k0 + 64 > kv_len || (causal && k0 + 63 > q0)) {
+#pragma unroll
+      for (int j = 0; j < 8; ++j)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = key0 + 8 * h, q = q0 + 8 * j + 2 * (lane & 3) + e;
+            if (key >= kv_len || (causal && key > q)) {
+              st[4 * j + 2 * h + e] = -INFINITY;
+              dpt[4 * j + 2 * h + e] = 0.f;
+            }
+          }
+    }
+    uint32_t pa[4][4], da[4][4];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      float l2[2], dl[2];
+#pragma unroll
+      for (int e = 0; e < 2; ++e) load_row_stats(a, base, q0 + 8 * j + 2 * (lane & 3) + e, N, l2[e], dl[e]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float p[2], ds[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          p[e] = ex2(fmaf(st[4 * j + 2 * h + e], a.scale_log2, -l2[e]));
+          ds[e] = p[e] * (dpt[4 * j + 2 * h + e] - dl[e]);
+        }
+        pa[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(p[0], p[1]);
+        da[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(ds[0], ds[1]);
+      }
+    }
+
+    // dV += P~^T dO_i, dK += dS~^T Q_i over the tile's 64 queries
+    fence_regs<DP / 2>(dv);
+    fence_regs<DP / 2>(dk);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dv, pa[kk], wgmma_desc(sdo + kk * 2048, 8192, 1024), 1);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dk, da[kk], wgmma_desc(sq + kk * 2048, 8192, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<DP / 2>(dv);
+    fence_regs<DP / 2>(dk);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)  // the A registers are read by the MMAs until the wait above
+#pragma unroll
+      for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(pa[kk][e]), "+r"(da[kk][e])::"memory");
+    if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * s);
+  }
+
+  // keys past N are not stored; keys past the length (and tiles no query sees) store the zeros they hold
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    const int key = key0 + 8 * h;
+    if (key >= N) continue;
+    store_o<Cfg>(a.dst[0], base + key, 0, a.D, dk, h, a.scale);
+    store_o<Cfg>(a.dst[1], base + key, 0, a.D, dv, h, 1.f);
+  }
+}
+
+// dQ of one query tile, placed and fed by AttnDense (the forward's dense addressing) on CTA (query tile, 0, b * H + h).
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::THREADS, 1)
+    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                       const BwdArgs a, const AttnDense<Cfg> md) {
+  static_assert(Cfg::BN == 64 && !Cfg::V_DN, "dQ: KV tiles of 64 keys, V [N, D]");
+  constexpr int BM = Cfg::BM, BN = Cfg::BN, DP = Cfg::DV, NC = DP / 64, ST = kBwdStages;
+  constexpr int QB = BM * DP * 2, KB = Cfg::V_BYTES;  // a resident Q / dO tile, a streamed K / V tile
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u, sdO = sQ + QB, sKV = sdO + QB;  // stage s: K, then V
+  const uint32_t qbar = sKV + ST * 2 * KB, full = qbar + 8, empty = full + 8 * ST;
+
+  typename AttnDense<Cfg>::Cta cta;
+  md.setup(cta);
+  const KvTiles kv = md.tiles(cta);
+  const int wg = threadIdx.x / 128;
+
+  if (threadIdx.x == 0) {
+    mbar_init(qbar, 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(full + 8 * s, 1);
+      mbar_init(empty + 8 * s, Cfg::NWG);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    if (threadIdx.x == 0) {
+      mbar_arrive_expect_tx(qbar, 2 * NC * md.q_bytes());
+      for (int c = 0; c < NC; ++c) {
+        md.load_q(cta, sQ + c * BM * 128, &tmQ, qbar, c);
+        md.load_q(cta, sdO + c * BM * 128, &tmdO, qbar, c);
+      }
+      for (int j = kv.first; j < kv.end; ++j) {
+        const int n = j - kv.first, s = n % ST;
+        if (n >= ST) mbar_wait_nocall(empty + 8 * s, ((n / ST) - 1) & 1);
+        mbar_arrive_expect_tx(full + 8 * s, 2 * KB);
+        const int key0 = md.kv_tile(cta, j);
+        for (int c = 0; c < NC; ++c) md.load_k(cta, key0, sKV + s * 2 * KB + c * BN * 128, &tmK, full + 8 * s, c);
+        md.load_v(cta, key0, sKV + s * 2 * KB + KB, &tmV, full + 8 * s);
+      }
+    }
+    return;
+  }
+
+  const int cw = wg - 1, lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
+  const int row0 = cta.q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
+  const int N = md.N;
+  float l2[2], dl[2];
+#pragma unroll
+  for (int h = 0; h < 2; ++h) load_row_stats(a, size_t(cta.bh) * N, row0 + 8 * h, N, l2[h], dl[h]);
+  float dq[DP / 2];
+#pragma unroll
+  for (int i = 0; i < DP / 2; ++i) dq[i] = 0.f;
+  mbar_wait_nocall(qbar, 0);
+
+  for (int j = kv.first; j < kv.end; ++j) {
+    const int n = j - kv.first, s = n % ST, k0 = j * BN;
+    const uint32_t sk = sKV + s * 2 * KB, sv = sk + KB;
+    float sa[BN / 2], dp[BN / 2];
+#pragma unroll
+    for (int e = 0; e < BN / 2; ++e) sa[e] = dp[e] = 0.f;
+    mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
+    fence_regs<BN / 2>(sa);
+    fence_regs<BN / 2>(dp);
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<Cfg::DT, BN, 0, 0>(sa, wgmma_desc(sQ + c * BM * 128 + cw * 64 * 128 + k * 32, 16, 1024),
+                                    wgmma_desc(sk + c * BN * 128 + k * 32, 16, 1024), 1);
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        wgmma_ss<Cfg::DT, BN, 0, 0>(dp, wgmma_desc(sdO + c * BM * 128 + cw * 64 * 128 + k * 32, 16, 1024),
+                                    wgmma_desc(sv + c * BN * 128 + k * 32, 16, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<BN / 2>(sa);
+    fence_regs<BN / 2>(dp);
+
+    // the forward's masks: keys past the length, keys after the row's causal diagonal
+    if (k0 + BN > cta.kv_len || (md.causal && k0 + BN - 1 > md.diag(cta, cta.q0 + cw * 64))) {
+      const int diag[2] = {md.diag(cta, row0), md.diag(cta, row0 + 8)};
+#pragma unroll
+      for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            const int key = k0 + 8 * i + 2 * (lane & 3) + e;
+            if (key >= cta.kv_len || (md.causal && key > diag[h])) {
+              sa[4 * i + 2 * h + e] = -INFINITY;
+              dp[4 * i + 2 * h + e] = 0.f;
+            }
+          }
+    }
+    uint32_t da[BN / 16][4];
+#pragma unroll
+    for (int i = 0; i < BN / 8; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float ds[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e)
+          ds[e] = ex2(fmaf(sa[4 * i + 2 * h + e], a.scale_log2, -l2[h])) * (dp[4 * i + 2 * h + e] - dl[h]);
+        da[i / 2][(i & 1) * 2 + h] = pack_round<Cfg::DT>(ds[0], ds[1]);
+      }
+
+    // dQ += dS~ K_j
+    fence_regs<DP / 2>(dq);
+    wgmma_fence();
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk)
+      wgmma_rs<Cfg::DT, DP, 1>(dq, da[kk], wgmma_desc(sk + kk * 2048, BN * 128, 1024), 1);
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs<DP / 2>(dq);
+#pragma unroll
+    for (int kk = 0; kk < BN / 16; ++kk)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(da[kk][e])::"memory");
+    if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * s);
+  }
+
+#pragma unroll
+  for (int h = 0; h < 2; ++h) md.store(cta, row0 + 8 * h, dq, h, a.scale, 0.f, 0.f, a.dst[0], a.D);
+}
+
+// Workspace: Delta, then lse * log2 e, fp32 [B * H * N] each, each on a 256-byte boundary.
+static size_t bwd_section(int64_t rows) { return (size_t(rows) * sizeof(float) + 255) & ~size_t(255); }
+
+static int bwd_shape(const char* fn, int64_t B, int64_t H, int64_t N) {
+  if (B < 1 || H < 1 || N < 1 || N > INT32_MAX || B * H > 65535)
+    return set_error(B200K_ESHAPE, "%s: need B, H, N >= 1, N <= 2^31 - 1 and B * H <= 65535 (got B=%lld H=%lld N=%lld)",
+                     fn, (long long)B, (long long)H, (long long)N);
+  return B200K_OK;
+}
+
+template <class Kern, class... Rest>
+static int bwd_launch(Kern kern, dim3 grid, int threads, int smem, cudaStream_t s, const DeviceInfo& di, const char* fn,
+                      const CUtensorMap (&tm)[4], const BwdArgs& a, Rest... rest) {
+  if (smem > di.max_smem_optin)
+    return set_error(B200K_ESHAPE, "%s: %d bytes of shared memory needed, device allows %d", fn, smem, di.max_smem_optin);
+  int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem);
+  if (rc) return rc;
+  kern<<<grid, threads, smem, s>>>(tm[0], tm[1], tm[2], tm[3], a, rest...);
+  B200K_CHECK_CUDA(cudaGetLastError());
+  return B200K_OK;
+}
+
+template <int DT, int DP>
+static int run_bwd(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO, void* dQ,
+                   void* dK, void* dV, int64_t B, int64_t H, int64_t N, int64_t D, const int* seqlens, int causal,
+                   BwdArgs a, cudaStream_t s, const DeviceInfo& di) {
+  using KvCfg = AttnCfg<DT, DP, 1, 64, false>;
+  using QCfg = AttnCfg<DT, DP, 2, 64, false>;
+  const int64_t BH = B * H;
+  // The prep kernel goes first: its launch makes the device's primary context current on the calling thread, which the
+  // tensor-map encoder (a driver call) needs.  torch runs a backward on an autograd thread of its own, where no CUDA
+  // runtime call may have run yet.
+  const long long rows = BH * N, blocks = (rows * 4 + 255) / 256;
+  attn_bwd_prep_kernel<DT><<<unsigned(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(
+      static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
+      const_cast<float*>(a.lse2), rows, int(D));
+  B200K_CHECK_CUDA(cudaGetLastError());
+  CUtensorMap kv_tm[4], q_tm[4];  // dK/dV kernel: K, V, Q, dO in 64-row boxes; dQ kernel: Q, dO in 128-row boxes, K, V
+  const AttnTensor kv_t[4] = {{K, BH, N, D, 1, 64}, {V, BH, N, D, 1, 64}, {Q, BH, N, D, 1, 64}, {dO, BH, N, D, 1, 64}};
+  const AttnTensor q_t[2] = {{Q, BH, N, D, 1, QCfg::BM}, {dO, BH, N, D, 1, QCfg::BM}};
+  int rc;
+  for (int i = 0; i < 4; ++i)
+    if ((rc = attn_tmap(&kv_tm[i], kv_t[i]))) return rc;
+  for (int i = 0; i < 2; ++i)
+    if ((rc = attn_tmap(&q_tm[i], q_t[i]))) return rc;
+  q_tm[2] = kv_tm[0];
+  q_tm[3] = kv_tm[1];
+  const char* fn = "b200k_fa2_bwd";
+  const int bars = 8 * (1 + 2 * kBwdStages);
+  BwdArgs kva = a;
+  kva.dst[0] = dK;
+  kva.dst[1] = dV;
+  rc = bwd_launch(attn_bwd_dkdv_kernel<KvCfg>, dim3(unsigned((N + 63) / 64), unsigned(BH)), KvCfg::THREADS,
+                  1024 + (2 + 2 * kBwdStages) * 64 * DP * 2 + bars, s, di, fn, kv_tm, kva, seqlens, int(N), int(H),
+                  causal ? 1 : 0);
+  if (rc) return rc;
+  BwdArgs qa = a;
+  qa.dst[0] = dQ;
+  qa.dst[1] = nullptr;
+  const AttnDense<QCfg> md = {seqlens, int(N), int(H), causal ? 1 : 0};
+  return bwd_launch(attn_bwd_dq_kernel<QCfg>, dim3(unsigned((N + QCfg::BM - 1) / QCfg::BM), 1, unsigned(BH)),
+                    QCfg::THREADS, 1024 + 2 * QCfg::BM * DP * 2 + 2 * kBwdStages * QCfg::V_BYTES + bars, s, di, fn, q_tm,
+                    qa, md);
+}
+
+}  // namespace b200k
+
+extern "C" int b200k_fa2_bwd_workspace_bytes(int64_t B, int64_t H, int64_t N, size_t* bytes) {
+  using namespace b200k;
+  if (!bytes) return set_error(B200K_EARG, "b200k_fa2_bwd_workspace_bytes: null pointer");
+  const int rc = bwd_shape("b200k_fa2_bwd_workspace_bytes", B, H, N);
+  if (rc) return rc;
+  *bytes = 2 * bwd_section(B * H * N);
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_bwd(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO,
+                             void* dQ, void* dK, void* dV, int64_t B, int64_t H, int64_t N, int64_t D, float scale,
+                             int dtype, int causal, const int* seqlens_k, void* workspace, size_t workspace_bytes,
+                             void* stream) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_bwd";
+  if (!Q || !K || !V || !O || !lse || !dO || !dQ || !dK || !dV || !workspace)
+    return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (dtype != B200K_F16 && dtype != B200K_BF16) return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
+  int rc = check_headdim(fn, D);
+  if (rc || (rc = bwd_shape(fn, B, H, N))) return rc;
+  if ((rc = check_align(fn, {{Q, "Q", 16}, {K, "K", 16}, {V, "V", 16}, {O, "O", 16}, {dO, "dO", 16},
+                             {workspace, "workspace", 16}, {dQ, "dQ", 4}, {dK, "dK", 4}, {dV, "dV", 4}, {lse, "lse", 4},
+                             {seqlens_k, "seqlens_k", 4}})))
+    return rc;
+  const int64_t rows = B * H * N;
+  const size_t need = 2 * bwd_section(rows);
+  if (workspace_bytes < need)
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, need, workspace_bytes);
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  BwdArgs a;
+  a.delta = static_cast<const float*>(workspace);
+  a.lse2 = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + bwd_section(rows));
+  a.dst[0] = a.dst[1] = nullptr;
+  a.D = int(D);
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  a.scale = scale;
+  a.scale_log2 = scale * 1.4426950408889634f;
+  const bool narrow = D <= 64;
+  if (dtype == B200K_BF16)
+    return narrow ? run_bwd<1, 64>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di)
+                  : run_bwd<1, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
+  return narrow ? run_bwd<0, 64>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di)
+                : run_bwd<0, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
+}

@@ -1,0 +1,159 @@
+// What the attention forward (attn_fwd_wgmma.cu) and backward (attn_bwd_wgmma.cu) share: the kernel configuration, the
+// fp32 -> 16-bit rounding of MMA operands and outputs, the dense [B, H, N, D] addressing, the tensor maps of Q / K / V,
+// and the argument checks of the entry points.
+#pragma once
+#include "abi_common.cuh"
+#include "ptx.cuh"
+
+#include <initializer_list>
+
+namespace b200k {
+
+template <int DT_, int DV_, int NWG_, int BN_, bool V_DN_>  // DT: 0 f16, 1 bf16
+struct AttnCfg {
+  static constexpr int DT = DT_, DV = DV_, NWG = NWG_, BN = BN_;
+  static constexpr bool V_DN = V_DN_;
+  static constexpr int BM = 64 * NWG;
+  static constexpr int THREADS = 128 * (NWG + 1);
+  static constexpr int KSTAGES = 4, VSTAGES = 2;
+  static constexpr int K_BYTES = BN * 128;  // BN keys x 64 head-dim columns
+  static constexpr int V_BYTES = BN * DV * 2;
+  static constexpr int BAR_BYTES = 8 * (1 + 2 * KSTAGES + 2 * VSTAGES);
+  static int smem_bytes(int nqc) { return 1024 + nqc * BM * 128 + KSTAGES * K_BYTES + VSTAGES * V_BYTES + BAR_BYTES; }
+};
+
+__device__ __forceinline__ float ex2(float x) {
+  float y;
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+  return y;
+}
+
+// Two fp32 values -> packed 16-bit pair; `lo` / `hi` come back as the rounded values (so the row sum matches what the
+// tensor core multiplies).
+template <int DT>
+__device__ __forceinline__ uint32_t pack_round(float& lo, float& hi) {
+  if constexpr (DT == 0) {
+    const __half2 h = __floats2half2_rn(lo, hi);
+    const float2 f = __half22float2(h);
+    lo = f.x;
+    hi = f.y;
+    return *reinterpret_cast<const uint32_t*>(&h);
+  } else {
+    const __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
+    const float2 f = __bfloat1622float2(h);
+    lo = f.x;
+    hi = f.y;
+    return *reinterpret_cast<const uint32_t*>(&h);
+  }
+}
+
+// Row `row` of a 16-bit [rows, D] O from this thread's column pairs of accumulator row h (o[4 i + 2 h], o[4 i + 2 h + 1]
+// hold columns dv0 + 8 i + 2 (lane % 4) and the next), times inv, clipped to D columns (D is even).
+template <class Cfg>
+__device__ __forceinline__ void store_o(void* O, size_t row, int dv0, int D, const float (&o)[Cfg::DV / 2], int h,
+                                        float inv) {
+  const int lane = threadIdx.x & 31;
+#pragma unroll
+  for (int i = 0; i < Cfg::DV / 8; ++i) {
+    const int c = dv0 + 8 * i + 2 * (lane & 3);
+    if (c >= D) continue;
+    float x = o[4 * i + 2 * h] * inv, y = o[4 * i + 2 * h + 1] * inv;
+    *reinterpret_cast<uint32_t*>(static_cast<uint16_t*>(O) + row * size_t(D) + c) = pack_round<Cfg::DT>(x, y);
+  }
+}
+
+// KV tiles [first, end) of a CTA: tile j holds keys [j * BN, (j + 1) * BN) of its sequence.
+struct KvTiles { int first, end; };
+
+// [B, H, N, D], one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).  CTA (x, y, z) =
+// (query tile, O column slice, batch * H + head).  Rows are numbered within the head, so row r sees keys <= r under the
+// causal mask.  The modes of the forward are described in attn_fwd_wgmma.cu; the backward's dQ kernel takes this one.
+template <class Cfg>
+struct AttnDense {
+  const int* seqlens;  // int32 [B] valid keys per batch, or null
+  int N, H, causal;
+
+  struct Cta { int bh, q0, dv0, kv_len; };
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    c.bh = blockIdx.z;
+    c.q0 = blockIdx.x * Cfg::BM;
+    c.dv0 = blockIdx.y * Cfg::DV;
+    c.kv_len = seqlens ? min(max(__ldg(seqlens + c.bh / H), 1), N) : N;
+    return true;
+  }
+  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
+    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
+    if (causal) nt = min(nt, (c.q0 + Cfg::BM - 1) / Cfg::BN + 1);
+    return {0, nt};
+  }
+  __device__ __forceinline__ int q_bytes() const { return Cfg::BM * 128; }
+  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.q0, c.bh, kPolicyEvictFirst);
+  }
+  __device__ __forceinline__ int kv_tile(const Cta&, int j) const { return j * Cfg::BN; }
+  __device__ __forceinline__ void load_k(const Cta& c, int key0, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, key0, c.bh, kPolicyEvictNormal);
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, int key0, uint32_t dst, const CUtensorMap* tm, uint32_t bar) const {
+    if constexpr (Cfg::V_DN) {
+#pragma unroll
+      for (int i = 0; i < Cfg::BN / 64; ++i)
+        tma_load_3d(dst + i * Cfg::DV * 128, tm, bar, key0 + i * 64, c.dv0, c.bh, kPolicyEvictNormal);
+    } else {
+#pragma unroll
+      for (int i = 0; i < Cfg::DV / 64; ++i)
+        tma_load_3d(dst + i * Cfg::BN * 128, tm, bar, c.dv0 + i * 64, key0, c.bh, kPolicyEvictNormal);
+    }
+  }
+  __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
+  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
+    if (r >= N) return false;
+    row = size_t(c.bh) * N + r;
+    return true;
+  }
+  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
+                                        float, void* O, int D) const {
+    size_t row;
+    if (out_row(c, r, row)) store_o<Cfg>(O, row, c.dv0, D, o, h, inv);
+  }
+};
+
+// One contiguous 16-bit [d2, d1, d0] tensor read through boxes [box2, box1, 64]: each box row is one 128-byte swizzle row.
+struct AttnTensor {
+  const void* p;
+  int64_t d2, d1, d0;
+  int box2, box1;
+};
+
+static int attn_tmap(CUtensorMap* m, const AttnTensor& t) {
+  const uint64_t dims[3] = {uint64_t(t.d0), uint64_t(t.d1), uint64_t(t.d2)}, strides[2] = {2 * dims[0], 2 * dims[0] * dims[1]};
+  const uint32_t box[3] = {64, uint32_t(t.box1), uint32_t(t.box2)};
+  return make_tmap(m, t.p, 2, 3, dims, strides, box);
+}
+
+static int check_headdim(const char* fn, int64_t D) {
+  if (D != 32 && D != 64 && D != 96 && D != 128)
+    return set_error(B200K_EHEADDIM, "headdim not support! (%s: D=%lld, supported 32/64/96/128)", fn, (long long)D);
+  return B200K_OK;
+}
+
+// Alignment checks of the attention entry points, in order, before any CUDA call: the first pointer that is not a
+// multiple of its byte count is B200K_EALIGN, named in the message.  Null pointers pass (each call checks those it
+// needs).  The rules: Q, K, V, the caches, the new rows, cos / sin and workspaces 16 bytes (TMA maps, 16-byte loads
+// and stores, fp32 partials); O 4 bytes (32-bit stores of column pairs); lse and the int32 arrays 4 bytes.
+struct AlignRule {
+  const void* p;
+  const char* name;
+  unsigned bytes;
+};
+
+static int check_align(const char* fn, std::initializer_list<AlignRule> rules) {
+  for (const AlignRule& r : rules)
+    if (reinterpret_cast<uintptr_t>(r.p) % r.bytes)
+      return set_error(B200K_EALIGN, "%s: %s must be %u-byte aligned", fn, r.name, r.bytes);
+  return B200K_OK;
+}
+
+}  // namespace b200k

@@ -272,6 +272,34 @@ int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, void* V_cache
 int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows, int64_t D,
                      int dtype, void* stream);
 
+/* ------------------------------------------------------------------------------------------------ attention backward
+ * b200k_fa2_bwd — the gradients of b200k_fa2_fwd (flash-attn's backward), dense layout:
+ *   inputs      Q, K, V, O, dO [B, H, N, D] contiguous in dtype (B200K_F16 or B200K_BF16); lse [B, H, N] fp32, natural
+ *               log, as b200k_fa2_fwd_lse wrote it for this O.  D in {32, 64, 96, 128}; scale <= 0 means 1/sqrt(D)
+ *   contract    scale, causal and seqlens_k are those of the forward call that produced O and lse (not checked).  As in
+ *               the forward, seqlens_k[b] is clamped to [1, N]
+ *   outputs     dQ, dK, dV [B, H, N, D] in dtype, every element written once; nothing else outside the workspace is
+ *               written.  dK and dV rows of keys no query sees (at or past seqlens_k[b]) are 0
+ *   arithmetic  fp32 throughout: P = 2^(s * scale * log2 e - lse * log2 e), s = q . k from the tensor core;
+ *               Delta_i = sum_d dO_id O_id from the 16-bit O and dO; dP_ij = dO_i . v_j; dS = P (dP - Delta);
+ *               dV_j = sum_i P~_ij dO_i, dQ_i = scale sum_j dS~_ij k_j, dK_j = scale sum_i dS~_ij q_i, where P~ and dS~ are
+ *               P and dS rounded to dtype (the tensor core's A operand); each output rounded once
+ *   guarantees  deterministic (no atomics, no fp32 accumulation buffer: each output element is summed in one thread's
+ *               registers), so two calls, or a call replayed from a CUDA graph, give the same bits.  No host sync
+ *   workspace   >= b200k_fa2_bwd_workspace_bytes(B, H, N): the per-row Delta, then lse * log2 e, fp32 [B, H, N] each on
+ *               a 256-byte boundary
+ *   cost        S and dP are computed by both the dK/dV and the dQ kernel: 7 matrix products where an atomic-dQ backward
+ *               needs 5
+ *   alignment   Q, K, V, O, dO, workspace 16 bytes; dQ, dK, dV, lse, seqlens_k 4 bytes (32-bit stores and loads)
+ * Errors, all before any CUDA call: B200K_EARG for a null pointer (seqlens_k may be NULL), B200K_EDTYPE,
+ * B200K_EHEADDIM, B200K_ESHAPE unless B, H, N >= 1, N <= INT32_MAX and B * H <= 65535, B200K_EALIGN naming the
+ * argument, then B200K_EARG for a workspace below the size above. */
+int b200k_fa2_bwd(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO,
+                  void* dQ, void* dK, void* dV, int64_t B, int64_t H, int64_t N, int64_t D, float scale, int dtype,
+                  int causal, const int* seqlens_k, void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace bytes b200k_fa2_bwd needs for these shapes (no device query); B200K_ESHAPE as b200k_fa2_bwd. */
+int b200k_fa2_bwd_workspace_bytes(int64_t B, int64_t H, int64_t N, size_t* bytes);
+
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
 #define B200K_F32 0
