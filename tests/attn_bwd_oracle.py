@@ -2,7 +2,7 @@
     s = q k^T * scale, masked (keys >= seqlens_k[b] clamped to [1, N]; causal: key > row), lse = log sum_j exp(s),
     P = exp(s - lse), Delta_i = sum_d dO_id O_id, dP = dO v^T, dS = P (dP - Delta),
     dV = P^T dO, dQ = scale dS k, dK = scale dS^T q.
-Used by test_attention_bwd_cpu.py (against torch.autograd) and test_gpu_attention_bwd.py (against the kernels)."""
+grads_given takes O and lse as inputs instead of forming them.  Used by test_attention_bwd_cpu.py (against torch.autograd) and test_gpu_attention_bwd.py (against the kernels)."""
 from __future__ import annotations
 
 import math
@@ -34,6 +34,20 @@ def forward(q, k, v, scale: Optional[float] = None, causal: bool = False, seqlen
     return torch.softmax(s, -1) @ v, lse
 
 
+def grads_given(q, k, v, o, lse, do, scale: Optional[float] = None, causal: bool = False, seqlens_k=None):
+    """(dq, dk, dv) in fp64 from the explicit formulas with O and lse taken as inputs, as the kernels take them (they
+    need not be the forward of q, k, v): P = exp(s - lse), Delta = rowsum(dO O)."""
+    q, k, v, o, lse, do = (t.double() for t in (q, k, v, o, lse, do))
+    B, H, N, D = q.shape
+    scale = scale if scale else 1.0 / math.sqrt(D)
+    vis = visible(B, N, causal, seqlens_k, q.device)
+    s = ((q @ k.transpose(-1, -2)) * scale).masked_fill(~vis, float("-inf"))
+    p = torch.exp(s - lse.unsqueeze(-1))
+    delta = (do * o).sum(-1, keepdim=True)
+    ds = p * (do @ v.transpose(-1, -2) - delta)
+    return scale * (ds @ k), scale * (ds.transpose(-1, -2) @ q), p.transpose(-1, -2) @ do
+
+
 def grads(q, k, v, do, scale: Optional[float] = None, causal: bool = False, seqlens_k=None):
     """(dq, dk, dv, o, lse) in fp64 from the explicit formulas."""
     q, k, v, do = (t.double() for t in (q, k, v, do))
@@ -42,8 +56,5 @@ def grads(q, k, v, do, scale: Optional[float] = None, causal: bool = False, seql
     vis = visible(B, N, causal, seqlens_k, q.device)
     s = ((q @ k.transpose(-1, -2)) * scale).masked_fill(~vis, float("-inf"))
     lse = torch.logsumexp(s, -1)
-    p = torch.exp(s - lse.unsqueeze(-1))
-    o = p @ v
-    delta = (do * o).sum(-1, keepdim=True)
-    ds = p * (do @ v.transpose(-1, -2) - delta)
-    return scale * (ds @ k), scale * (ds.transpose(-1, -2) @ q), p.transpose(-1, -2) @ do, o, lse
+    o = torch.exp(s - lse.unsqueeze(-1)) @ v
+    return grads_given(q, k, v, o, lse, do, scale, causal, seqlens_k) + (o, lse)
