@@ -78,6 +78,9 @@ _SIGS = {
     "b200k_fa2_bwd": (c_int, [c_void_p] * 9 + [c_int64] * 4 + [c_float, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                                                c_void_p]),
     "b200k_fa2_bwd_workspace_bytes": (c_int, [c_int64] * 3 + [ctypes.POINTER(c_size_t)]),
+    "b200k_fa2_bwd_varlen": (c_int, [c_void_p] * 11 + [c_int64] * 8 + [c_float, c_int, c_int, c_void_p, c_size_t,
+                                                                     c_void_p]),
+    "b200k_fa2_bwd_varlen_workspace_bytes": (c_int, [c_int64] * 2 + [ctypes.POINTER(c_size_t)]),
     "b200k_elementwise_add": (c_int, [c_void_p, c_void_p, c_void_p, c_int64, c_int, c_void_p]),
     "b200k_reduce_workspace_bytes": (c_size_t, []),
     "b200k_block_all_reduce_sum": (c_int, [c_void_p, c_void_p, c_int64, c_int, c_int, c_void_p, c_void_p]),

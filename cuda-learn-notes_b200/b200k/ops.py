@@ -459,6 +459,80 @@ def attention(q, k, v, scale: Optional[float] = None, causal: bool = False,
     return _Attention.apply(q, k, v, scale, causal, seqlens_k)
 
 
+def fa2_bwd_varlen_workspace_bytes(total_q: int, H: int) -> int:
+    """Workspace bytes :func:`fa2_bwd_varlen` needs for these shapes."""
+    n = ctypes.c_size_t(0)
+    L.check(_lib.b200k_fa2_bwd_varlen_workspace_bytes(total_q, H, ctypes.byref(n)))
+    return n.value
+
+
+def fa2_bwd_varlen(q, k, v, o, lse, do, dq, dk, dv, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor,
+                   max_seqlen_q: int, max_seqlen_k: int, scale: Optional[float] = None, causal: bool = False) -> None:
+    """Gradients of :func:`fa2_fwd_varlen` (packed sequences, grouped K/V heads) into dq [total_q, H, D] and dk, dv
+    [total_k, H_kv, D]: o and ``lse`` (fp32 [total_q, H]) are what the forward wrote with ``lse=``, ``do`` the gradient
+    of o.  ``scale``, ``causal`` and the ``cu_seqlens`` must be the forward's; ``max_seqlen_q`` / ``max_seqlen_k``
+    (Python ints, >= every length) size the grids.  dk / dv of a K/V head sum over its query heads; rows of tokens
+    outside every sequence are 0.  Deterministic and graph-capturable; the workspace is allocated per call on the
+    current stream."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    for t in (q, k, v, o, do, dq, dk, dv):
+        _check_dtype(t, dt)
+    if q.dim() != 3 or k.dim() != 3:
+        raise RuntimeError("Tensor size mismatch!")
+    total_q, H, D = q.shape
+    total_k, H_kv = k.size(0), k.size(1)
+    if (tuple(k.shape) != (total_k, H_kv, D) or any(tuple(t.shape) != tuple(k.shape) for t in (v, dk, dv))
+            or any(tuple(t.shape) != tuple(q.shape) for t in (o, do, dq))):
+        raise RuntimeError("Tensor size mismatch!")
+    if H_kv < 1 or H % H_kv:
+        raise RuntimeError("Tensor size mismatch!")
+    if D not in FA2_HEADDIMS:
+        raise RuntimeError("headdim not support!")
+    _check_dtype(cu_seqlens_q, torch.int32)
+    _check_dtype(cu_seqlens_k, torch.int32)
+    B = cu_seqlens_q.numel() - 1
+    if B < 1 or cu_seqlens_k.numel() != B + 1:
+        raise RuntimeError("Tensor size mismatch!")
+    _check_lse(lse, o)
+    _check_cuda_contig(q, k, v, o, lse, do, dq, dk, dv, cu_seqlens_q, cu_seqlens_k)
+    with _DeviceGuard(q):
+        nbytes = fa2_bwd_varlen_workspace_bytes(total_q, H)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
+        L.check(_lib.b200k_fa2_bwd_varlen(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), do.data_ptr(), dq.data_ptr(),
+            dk.data_ptr(), dv.data_ptr(), cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), B, int(max_seqlen_q),
+            int(max_seqlen_k), total_q, total_k, H, H_kv, D, float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
+            1 if causal else 0, ws.data_ptr(), nbytes, _stream(q)))
+
+
+class _AttentionVarlen(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, causal):
+        o = torch.empty_like(q)
+        lse = torch.empty(q.shape[:-1], dtype=torch.float32, device=q.device)
+        fa2_fwd_varlen(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal=causal, lse=lse)
+        ctx.save_for_backward(q, k, v, o, lse, cu_seqlens_q, cu_seqlens_k)
+        ctx.max_seqlen_q, ctx.max_seqlen_k, ctx.scale, ctx.causal = max_seqlen_q, max_seqlen_k, scale, causal
+        return o
+
+    @staticmethod
+    def backward(ctx, grad):
+        q, k, v, o, lse, cu_q, cu_k = ctx.saved_tensors
+        dq, dk, dv = torch.empty_like(q), torch.empty_like(k), torch.empty_like(v)
+        fa2_bwd_varlen(q, k, v, o, lse, grad.contiguous(), dq, dk, dv, cu_q, cu_k, ctx.max_seqlen_q, ctx.max_seqlen_k,
+                       ctx.scale, ctx.causal)
+        return dq, dk, dv, None, None, None, None, None, None
+
+
+def attention_varlen(q, k, v, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
+                     max_seqlen_k: int, scale: Optional[float] = None, causal: bool = False) -> torch.Tensor:
+    """Differentiable packed variable-length attention in ``flash_attn_varlen_func``'s argument order: q [total_q, H, D],
+    k, v [total_k, H_kv, D] (fp16 or bf16, D in 32, 64, 96, 128, H % H_kv == 0), int32 ``cu_seqlens`` [B + 1] on the
+    device.  Returns o from :func:`fa2_fwd_varlen`; its backward is :func:`fa2_bwd_varlen`, which gives the gradients of
+    q, k and v."""
+    return _AttentionVarlen.apply(q, k, v, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, max_seqlen_k, scale, causal)
+
+
 def ffpa_fwd(q, k, v, o, scale: Optional[float] = None, variant: int = 0) -> None:
     B, H, N, D = _check_qkvo(q, k, v, o)
     with _DeviceGuard(q):

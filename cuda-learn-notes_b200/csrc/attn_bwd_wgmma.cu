@@ -1,4 +1,4 @@
-// Attention backward on Hopper (sm_90a), dense [B, H, N, D]: dQ, dK and dV of O = softmax(Q K^T * scale) V from Q, K,
+// Attention backward on Hopper (sm_90a), dense [B, H, N, D] or packed [tokens, H, D] with grouped K/V heads: dQ, dK and dV of O = softmax(Q K^T * scale) V from Q, K,
 // V, O, dO and the forward's log-sum-exp (b200k_fa2_fwd_lse), the FlashAttention-2 algorithm with every output element
 // summed in one thread's registers, so the result is deterministic without atomics.  Three kernels, in stream order:
 //   prep    Delta_i = sum_d dO_id O_id and lse_i * log2 e into the workspace (bandwidth kernel, no tensor cores)
@@ -15,10 +15,14 @@
 // 7 products where an atomic-dQ backward needs 5, the price of determinism.
 // The dK/dV warpgroup holds dK, dV (2 x DP / 2 fp32) and S^T, dP^T (2 x 32): 192 at DP = 128, more than a 384-thread
 // block gives a thread (168), so it runs one consumer warpgroup in a 256-thread block.
+// Packed sequences (b200k_fa2_bwd_varlen) run the same three kernels: the prep also zero-fills the gradients of tokens
+// outside every sequence, a dK/dV CTA owns 64 keys of one K/V head and loops over the query tiles of every query head
+// of its group (so dK / dV sum over the group in registers), and the dQ kernel takes the forward's AttnPacked.
 #include "attn_common.cuh"
 
 #include <climits>
 #include <cmath>
+#include <type_traits>
 
 namespace b200k {
 
@@ -28,11 +32,12 @@ namespace b200k {
 constexpr int kBwdStages = 2;
 
 // Delta[row] = sum_d dO[row, d] O[row, d] and lse2[row] = lse[row] * log2 e, one row per quad of threads, 16-byte loads,
-// each thread's products summed in column order, then across the quad in a fixed order.
-template <int DT>
-__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
-                                                            const float* __restrict__ lse, float* __restrict__ delta,
-                                                            float* __restrict__ lse2, long long rows, int D) {
+// each thread's products summed in column order, then across the quad in a fixed order.  PACKED: a row that sees no key
+// (lse = -inf) gets lse2 = +inf, so its P is exactly 0 against a masked score too (2^(-inf + inf) would be NaN).
+template <int DT, bool PACKED>
+__device__ __forceinline__ void bwd_prep(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
+                                         const float* __restrict__ lse, float* __restrict__ delta,
+                                         float* __restrict__ lse2, long long rows, int D) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const int t = threadIdx.x & 3, lane = threadIdx.x & 31;
   // the loop bound is the same for the whole warp (its first thread's index), so the shuffles see every lane
@@ -62,15 +67,52 @@ __global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const uint16_t* __re
     acc += __shfl_xor_sync(0xffffffffu, acc, 2);
     if (row < rows && t == 0) {
       delta[row] = acc;
-      lse2[row] = lse[row] * 1.4426950408889634f;
+      const float l = lse[row];
+      lse2[row] = PACKED && l == -INFINITY ? INFINITY : l * 1.4426950408889634f;
     }
   }
 }
 
+template <int DT>
+__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
+                                                            const float* __restrict__ lse, float* __restrict__ delta,
+                                                            float* __restrict__ lse2, long long rows, int D) {
+  bwd_prep<DT, false>(O, dO, lse, delta, lse2, rows, D);
+}
+
+// A packed gradient tensor viewed as [total, width] 32-bit words, and its cumulative sequence offsets.
+struct BwdPackedGrad {
+  void* p;
+  const int* cu;
+  long long total, width;
+};
+
+// Zeroes the rows of tokens outside every sequence (before cu[0], from cu[B] on), which no main kernel stores.
+__device__ __forceinline__ void zero_outside(const BwdPackedGrad g, int B) {
+  const long long lo = min(max((long long)__ldg(g.cu), 0ll), g.total), hi = min(max((long long)__ldg(g.cu + B), lo), g.total);
+  const long long n = (lo + g.total - hi) * g.width, stride = (long long)gridDim.x * blockDim.x;
+#pragma unroll 1  // an unrolled loop's 64-bit trip count would be a division: a call
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride)
+    static_cast<uint32_t*>(g.p)[i < lo * g.width ? i : (hi - lo) * g.width + i] = 0u;
+}
+
+// The packed layout's prep: Delta and lse2 of every [total_q * H] row, then the zeros of dQ, dK and dV outside every
+// sequence.
+template <int DT>
+__global__ void __launch_bounds__(256) attn_bwd_packed_prep_kernel(
+    const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO, const float* __restrict__ lse,
+    float* __restrict__ delta, float* __restrict__ lse2, long long rows, int D, int B, const BwdPackedGrad dq,
+    const BwdPackedGrad dk, const BwdPackedGrad dv) {
+  bwd_prep<DT, true>(O, dO, lse, delta, lse2, rows, D);
+  zero_outside(dq, B);
+  zero_outside(dk, B);
+  zero_outside(dv, B);
+}
+
 // What both main kernels take beyond their tensor maps.
 struct BwdArgs {
-  const float* lse2;   // [B * H * N] lse * log2 e
-  const float* delta;  // [B * H * N]
+  const float* lse2;   // [B * H * N] (packed: [total_q * H]) lse * log2 e
+  const float* delta;  // the same rows
   void* dst[2];        // dK / dV kernel: dK, dV; dQ kernel: dQ
   int D;
   float scale_log2, scale;
@@ -231,12 +273,225 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   }
 }
 
-// dQ of one query tile, placed and fed by AttnDense (the forward's dense addressing) on CTA (query tile, 0, b * H + h).
+// Packed (AttnPacked's layout): CTA (x, y) = (key tile of sequence b, b * H_kv + K/V head), which visits the query tiles
+// of each query head h = K/V head * group + g of its group in turn, g ascending.  A query tile that runs past Lq reads
+// the next sequence's rows: their lse2 is +inf, so their P and dS are 0.  Keys past Lk are masked and not stored.  Row r
+// sees keys <= r + Lk - Lq under the causal mask.  The store reloads cu_k rather than keep it through the main loop.
+template <class Cfg>
+struct BwdKeysPacked {
+  const int* cu_q;
+  const int* cu_k;
+  int H, H_kv, group, causal;
+
+  struct Cta { int kvh, k0, kv_len, first, end, q_tok, q_len, shift; };  // q_tok: first query token; shift: Lk - Lq
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    const int b = blockIdx.y / H_kv, k_tok = __ldg(cu_k + b);
+    c.kvh = blockIdx.y % H_kv;
+    c.k0 = blockIdx.x * 64;
+    c.kv_len = __ldg(cu_k + b + 1) - k_tok;
+    if (c.k0 >= c.kv_len) return false;
+    c.q_tok = __ldg(cu_q + b);
+    c.q_len = __ldg(cu_q + b + 1) - c.q_tok;
+    c.shift = c.kv_len - c.q_len;
+    // query tiles that see a key of this tile: from the one holding row k0 - shift when causal, to the last
+    c.first = causal ? max(c.k0 - c.shift, 0) / 64 : 0;
+    c.end = max((c.q_len + 63) / 64, c.first);
+    return true;
+  }
+  __device__ __forceinline__ void load_kv(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                          int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.kvh, __ldg(cu_k + blockIdx.y / H_kv) + c.k0, kPolicyEvictFirst);
+  }
+  __device__ __forceinline__ void load_q(const Cta& c, int g, int i, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.kvh * group + g, c.q_tok + i * 64, kPolicyEvictNormal);
+  }
+  __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
+  __device__ __forceinline__ void row_stats(const BwdArgs& a, const Cta& c, int g, int r, float& l2, float& dl) const {
+    const size_t row = size_t(c.q_tok + r) * H + c.kvh * group + g;
+    l2 = r < c.q_len ? __ldg(a.lse2 + row) : INFINITY;
+    dl = r < c.q_len ? __ldg(a.delta + row) : 0.f;
+  }
+  __device__ __forceinline__ bool key_row(const Cta& c, int k, size_t& row) const {
+    if (k >= c.kv_len) return false;
+    row = size_t(__ldg(cu_k + blockIdx.y / H_kv) + k) * H_kv + c.kvh;
+    return true;
+  }
+};
+
+// Packed dK, dV of one 64-key tile: attn_bwd_dkdv_kernel's geometry and arithmetic, placed and fed by BwdKeysPacked.
+// The query tiles of the group's heads stream through one ring, head by head; dK and dV sum over all of them in this
+// thread's registers.  (The dense kernel keeps its own copy of this body: sharing one template changes ptxas's
+// register allocation of the dense instantiations.)
 template <class Cfg>
 __global__ void __launch_bounds__(Cfg::THREADS, 1)
-    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                       const BwdArgs a, const AttnDense<Cfg> md) {
+    attn_bwd_packed_dkdv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                                const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                                const BwdArgs a, const BwdKeysPacked<Cfg> md) {
+  static_assert(Cfg::NWG == 1 && Cfg::BM == 64 && Cfg::BN == 64, "dK/dV: one warpgroup of 64 keys, query tiles of 64");
+  constexpr int DP = Cfg::DV, NC = DP / 64, TILE = 64 * DP * 2, ST = kBwdStages;
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t sK = (smem_u32(smem_raw) + 1023) & ~1023u, sV = sK + TILE, sQ = sV + TILE;  // stage s: Q, then dO
+  const uint32_t kvbar = sQ + ST * 2 * TILE, full = kvbar + 8, empty = full + 8 * ST;
+
+  typename BwdKeysPacked<Cfg>::Cta c;
+  if (!md.setup(c)) return;
+  const int k0 = c.k0, first = c.first, end = c.end;
+  const int wg = threadIdx.x / 128;
+
+  if (threadIdx.x == 0) {
+    mbar_init(kvbar, 1);
+    for (int s = 0; s < ST; ++s) {
+      mbar_init(full + 8 * s, 1);
+      mbar_init(empty + 8 * s, 1);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+
+  if (wg == 0) {
+    if (threadIdx.x == 0 && first < end) {
+      mbar_arrive_expect_tx(kvbar, 2 * TILE);
+      for (int ch = 0; ch < NC; ++ch) {
+        md.load_kv(c, sK + ch * 8192, &tmK, kvbar, ch);
+        md.load_kv(c, sV + ch * 8192, &tmV, kvbar, ch);
+      }
+      for (int g = 0; g < md.group; ++g)
+        for (int i = first; i < end; ++i) {
+          const int n = g * (end - first) + i - first, s = n % ST;
+          if (n >= ST) mbar_wait_nocall(empty + 8 * s, ((n / ST) - 1) & 1);
+          mbar_arrive_expect_tx(full + 8 * s, 2 * TILE);
+          const uint32_t q = sQ + s * 2 * TILE;
+          for (int ch = 0; ch < NC; ++ch) {
+            md.load_q(c, g, i, q + ch * 8192, &tmQ, full + 8 * s, ch);
+            md.load_q(c, g, i, q + TILE + ch * 8192, &tmdO, full + 8 * s, ch);
+          }
+        }
+    }
+    return;
+  }
+
+  const int lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
+  const int key0 = k0 + warp * 16 + lane / 4;  // this thread's keys: key0 and key0 + 8
+  float dk[DP / 2], dv[DP / 2];
+#pragma unroll
+  for (int i = 0; i < DP / 2; ++i) dk[i] = dv[i] = 0.f;
+  if (first < end) mbar_wait_nocall(kvbar, 0);
+
+  for (int g = 0; g < md.group; ++g)
+    for (int i = first; i < end; ++i) {
+      const int n = g * (end - first) + i - first, s = n % ST, q0 = i * 64;
+      const uint32_t sq = sQ + s * 2 * TILE, sdo = sq + TILE;
+      float st[32], dpt[32];
+#pragma unroll
+      for (int e = 0; e < 32; ++e) st[e] = dpt[e] = 0.f;
+      mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
+      fence_regs<32>(st);
+      fence_regs<32>(dpt);
+      wgmma_fence();
+#pragma unroll
+      for (int ch = 0; ch < NC; ++ch)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss<Cfg::DT, 64, 0, 0>(st, wgmma_desc(sK + ch * 8192 + k * 32, 16, 1024),
+                                      wgmma_desc(sq + ch * 8192 + k * 32, 16, 1024), 1);
+#pragma unroll
+      for (int ch = 0; ch < NC; ++ch)
+#pragma unroll
+        for (int k = 0; k < 4; ++k)
+          wgmma_ss<Cfg::DT, 64, 0, 0>(dpt, wgmma_desc(sV + ch * 8192 + k * 32, 16, 1024),
+                                      wgmma_desc(sdo + ch * 8192 + k * 32, 16, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs<32>(st);
+      fence_regs<32>(dpt);
+
+      // masks: keys past the length, and (causal) keys after the query's diagonal.  A masked score becomes -inf (P = 0)
+      // and its dP 0, so nothing a padded key holds reaches dS.
+      if (k0 + 64 > c.kv_len || (md.causal && k0 + 63 > md.diag(c, q0))) {
+#pragma unroll
+        for (int j = 0; j < 8; ++j)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int e = 0; e < 2; ++e) {
+              const int key = key0 + 8 * h, q = q0 + 8 * j + 2 * (lane & 3) + e;
+              if (key >= c.kv_len || (md.causal && key > md.diag(c, q))) {
+                st[4 * j + 2 * h + e] = -INFINITY;
+                dpt[4 * j + 2 * h + e] = 0.f;
+              }
+            }
+      }
+      uint32_t pa[4][4], da[4][4];
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        float l2[2], dl[2];
+#pragma unroll
+        for (int e = 0; e < 2; ++e) md.row_stats(a, c, g, q0 + 8 * j + 2 * (lane & 3) + e, l2[e], dl[e]);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          float p[2], ds[2];
+#pragma unroll
+          for (int e = 0; e < 2; ++e) {
+            p[e] = ex2(fmaf(st[4 * j + 2 * h + e], a.scale_log2, -l2[e]));
+            ds[e] = p[e] * (dpt[4 * j + 2 * h + e] - dl[e]);
+          }
+          pa[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(p[0], p[1]);
+          da[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(ds[0], ds[1]);
+        }
+      }
+
+      // dV += P~^T dO_i, dK += dS~^T Q_i over the tile's 64 queries
+      fence_regs<DP / 2>(dv);
+      fence_regs<DP / 2>(dk);
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dv, pa[kk], wgmma_desc(sdo + kk * 2048, 8192, 1024), 1);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dk, da[kk], wgmma_desc(sq + kk * 2048, 8192, 1024), 1);
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs<DP / 2>(dv);
+      fence_regs<DP / 2>(dk);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk)  // the A registers are read by the MMAs until the wait above
+#pragma unroll
+        for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(pa[kk][e]), "+r"(da[kk][e])::"memory");
+      if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * s);
+    }
+
+  // keys past the sequence are not stored; tiles no query sees store the zeros they hold
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    size_t row;
+    if (!md.key_row(c, key0 + 8 * h, row)) continue;
+    store_o<Cfg>(a.dst[0], row, 0, a.D, dk, h, a.scale);
+    store_o<Cfg>(a.dst[1], row, 0, a.D, dv, h, 1.f);
+  }
+}
+
+// lse2 and Delta of row r of a dQ CTA: the row the mode stores it to, or padding (+inf, 0) when it stores none (rows
+// past N or past the sequence).
+template <class Mode>
+__device__ __forceinline__ void out_row_stats(const BwdArgs& a, const Mode& md, const typename Mode::Cta& c, int r,
+                                              float& l2, float& dl) {
+  size_t row = 0;
+  const bool in = md.out_row(c, r, row);
+  l2 = in ? __ldg(a.lse2 + row) : INFINITY;
+  dl = in ? __ldg(a.delta + row) : 0.f;
+}
+
+template <class Cfg>
+__device__ __forceinline__ void out_row_stats(const BwdArgs& a, const AttnDense<Cfg>& md,
+                                              const typename AttnDense<Cfg>::Cta& c, int r, float& l2, float& dl) {
+  load_row_stats(a, size_t(c.bh) * md.N, r, md.N, l2, dl);
+}
+
+// dQ of one query tile, placed and fed by the forward's addressing mode (AttnDense or AttnPacked) on CTA (query tile,
+// 0, b * H + h).
+template <class Cfg, class Mode>
+__device__ __forceinline__ void bwd_dq(const CUtensorMap& tmQ, const CUtensorMap& tmdO, const CUtensorMap& tmK,
+                                       const CUtensorMap& tmV, const BwdArgs& a, const Mode& md) {
   static_assert(Cfg::BN == 64 && !Cfg::V_DN, "dQ: KV tiles of 64 keys, V [N, D]");
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DP = Cfg::DV, NC = DP / 64, ST = kBwdStages;
   constexpr int QB = BM * DP * 2, KB = Cfg::V_BYTES;  // a resident Q / dO tile, a streamed K / V tile
@@ -244,8 +499,8 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u, sdO = sQ + QB, sKV = sdO + QB;  // stage s: K, then V
   const uint32_t qbar = sKV + ST * 2 * KB, full = qbar + 8, empty = full + 8 * ST;
 
-  typename AttnDense<Cfg>::Cta cta;
-  md.setup(cta);
+  typename Mode::Cta cta;
+  if (!md.setup(cta)) return;
   const KvTiles kv = md.tiles(cta);
   const int wg = threadIdx.x / 128;
 
@@ -280,10 +535,9 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
   const int cw = wg - 1, lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
   const int row0 = cta.q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
-  const int N = md.N;
   float l2[2], dl[2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) load_row_stats(a, size_t(cta.bh) * N, row0 + 8 * h, N, l2[h], dl[h]);
+  for (int h = 0; h < 2; ++h) out_row_stats(a, md, cta, row0 + 8 * h, l2[h], dl[h]);
   float dq[DP / 2];
 #pragma unroll
   for (int i = 0; i < DP / 2; ++i) dq[i] = 0.f;
@@ -364,6 +618,23 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   for (int h = 0; h < 2; ++h) md.store(cta, row0 + 8 * h, dq, h, a.scale, 0.f, 0.f, a.dst[0], a.D);
 }
 
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::THREADS, 1)
+    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                       const BwdArgs a, const AttnDense<Cfg> md) {
+  bwd_dq<Cfg>(tmQ, tmdO, tmK, tmV, a, md);
+}
+
+// Packed dQ: AttnPacked places the CTA (query tile of the sequence, 0, b * H + h); a tile past the sequence returns.
+template <class Cfg>
+__global__ void __launch_bounds__(Cfg::THREADS, 1)
+    attn_bwd_packed_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                              const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                              const BwdArgs a, const AttnPacked<Cfg> md) {
+  bwd_dq<Cfg>(tmQ, tmdO, tmK, tmV, a, md);
+}
+
 // Workspace: Delta, then lse * log2 e, fp32 [B * H * N] each, each on a 256-byte boundary.
 static size_t bwd_section(int64_t rows) { return (size_t(rows) * sizeof(float) + 255) & ~size_t(255); }
 
@@ -386,6 +657,25 @@ static int bwd_launch(Kern kern, dim3 grid, int threads, int smem, cudaStream_t 
   return B200K_OK;
 }
 
+// The maps of both main kernels: dK/dV kernel K, V, Q, dO in 64-row boxes; dQ kernel Q, dO in 128-row boxes, K, V.
+static int bwd_tmaps(const AttnTensor (&kv_t)[4], const AttnTensor (&q_t)[2], CUtensorMap (&kv_tm)[4],
+                     CUtensorMap (&q_tm)[4]) {
+  int rc;
+  for (int i = 0; i < 4; ++i)
+    if ((rc = attn_tmap(&kv_tm[i], kv_t[i]))) return rc;
+  for (int i = 0; i < 2; ++i)
+    if ((rc = attn_tmap(&q_tm[i], q_t[i]))) return rc;
+  q_tm[2] = kv_tm[0];
+  q_tm[3] = kv_tm[1];
+  return B200K_OK;
+}
+
+constexpr int kBwdBars = 8 * (1 + 2 * kBwdStages);
+template <int DP>
+constexpr int dkdv_smem() { return 1024 + (2 + 2 * kBwdStages) * 64 * DP * 2 + kBwdBars; }
+template <class QCfg>
+constexpr int dq_smem() { return 1024 + 2 * QCfg::BM * QCfg::DV * 2 + 2 * kBwdStages * QCfg::V_BYTES + kBwdBars; }
+
 template <int DT, int DP>
 static int run_bwd(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO, void* dQ,
                    void* dK, void* dV, int64_t B, int64_t H, int64_t N, int64_t D, const int* seqlens, int causal,
@@ -401,32 +691,63 @@ static int run_bwd(const void* Q, const void* K, const void* V, const void* O, c
       static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
       const_cast<float*>(a.lse2), rows, int(D));
   B200K_CHECK_CUDA(cudaGetLastError());
-  CUtensorMap kv_tm[4], q_tm[4];  // dK/dV kernel: K, V, Q, dO in 64-row boxes; dQ kernel: Q, dO in 128-row boxes, K, V
+  CUtensorMap kv_tm[4], q_tm[4];
   const AttnTensor kv_t[4] = {{K, BH, N, D, 1, 64}, {V, BH, N, D, 1, 64}, {Q, BH, N, D, 1, 64}, {dO, BH, N, D, 1, 64}};
   const AttnTensor q_t[2] = {{Q, BH, N, D, 1, QCfg::BM}, {dO, BH, N, D, 1, QCfg::BM}};
-  int rc;
-  for (int i = 0; i < 4; ++i)
-    if ((rc = attn_tmap(&kv_tm[i], kv_t[i]))) return rc;
-  for (int i = 0; i < 2; ++i)
-    if ((rc = attn_tmap(&q_tm[i], q_t[i]))) return rc;
-  q_tm[2] = kv_tm[0];
-  q_tm[3] = kv_tm[1];
+  int rc = bwd_tmaps(kv_t, q_t, kv_tm, q_tm);
+  if (rc) return rc;
   const char* fn = "b200k_fa2_bwd";
-  const int bars = 8 * (1 + 2 * kBwdStages);
   BwdArgs kva = a;
   kva.dst[0] = dK;
   kva.dst[1] = dV;
   rc = bwd_launch(attn_bwd_dkdv_kernel<KvCfg>, dim3(unsigned((N + 63) / 64), unsigned(BH)), KvCfg::THREADS,
-                  1024 + (2 + 2 * kBwdStages) * 64 * DP * 2 + bars, s, di, fn, kv_tm, kva, seqlens, int(N), int(H),
-                  causal ? 1 : 0);
+                  dkdv_smem<DP>(), s, di, fn, kv_tm, kva, seqlens, int(N), int(H), causal ? 1 : 0);
   if (rc) return rc;
   BwdArgs qa = a;
   qa.dst[0] = dQ;
   qa.dst[1] = nullptr;
   const AttnDense<QCfg> md = {seqlens, int(N), int(H), causal ? 1 : 0};
   return bwd_launch(attn_bwd_dq_kernel<QCfg>, dim3(unsigned((N + QCfg::BM - 1) / QCfg::BM), 1, unsigned(BH)),
-                    QCfg::THREADS, 1024 + 2 * QCfg::BM * DP * 2 + 2 * kBwdStages * QCfg::V_BYTES + bars, s, di, fn, q_tm,
-                    qa, md);
+                    QCfg::THREADS, dq_smem<QCfg>(), s, di, fn, q_tm, qa, md);
+}
+
+// The packed layout: the same kernels under BwdKeysPacked / AttnPacked, the maps over (D, heads, tokens), grids sized by
+// the longest sequences.  The prep also zero-fills the gradient rows of tokens outside every sequence.
+template <int DT, int DP>
+static int run_bwd_varlen(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO,
+                          void* dQ, void* dK, void* dV, const int* cu_q, const int* cu_k, int64_t B, int64_t max_q,
+                          int64_t max_k, int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv, int64_t D, int causal,
+                          BwdArgs a, cudaStream_t s, const DeviceInfo& di) {
+  using KvCfg = AttnCfg<DT, DP, 1, 64, false>;
+  using QCfg = AttnCfg<DT, DP, 2, 64, false>;
+  // first, for the reason run_bwd gives
+  const long long rows = total_q * H, blocks = (rows * 4 + 255) / 256;
+  const BwdPackedGrad gq = {dQ, cu_q, total_q, H * D / 2}, gk = {dK, cu_k, total_k, H_kv * D / 2},
+                      gv = {dV, cu_k, total_k, H_kv * D / 2};
+  attn_bwd_packed_prep_kernel<DT><<<unsigned(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(
+      static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
+      const_cast<float*>(a.lse2), rows, int(D), int(B), gq, gk, gv);
+  B200K_CHECK_CUDA(cudaGetLastError());
+  CUtensorMap kv_tm[4], q_tm[4];
+  const AttnTensor kv_t[4] = {{K, total_k, H_kv, D, 64, 1}, {V, total_k, H_kv, D, 64, 1}, {Q, total_q, H, D, 64, 1},
+                              {dO, total_q, H, D, 64, 1}};
+  const AttnTensor q_t[2] = {{Q, total_q, H, D, QCfg::BM, 1}, {dO, total_q, H, D, QCfg::BM, 1}};
+  int rc = bwd_tmaps(kv_t, q_t, kv_tm, q_tm);
+  if (rc) return rc;
+  const char* fn = "b200k_fa2_bwd_varlen";
+  BwdArgs kva = a;
+  kva.dst[0] = dK;
+  kva.dst[1] = dV;
+  const BwdKeysPacked<KvCfg> km = {cu_q, cu_k, int(H), int(H_kv), int(H / H_kv), causal ? 1 : 0};
+  rc = bwd_launch(attn_bwd_packed_dkdv_kernel<KvCfg>, dim3(unsigned((max_k + 63) / 64), unsigned(B * H_kv)),
+                  KvCfg::THREADS, dkdv_smem<DP>(), s, di, fn, kv_tm, kva, km);
+  if (rc) return rc;
+  BwdArgs qa = a;
+  qa.dst[0] = dQ;
+  qa.dst[1] = nullptr;
+  const AttnPacked<QCfg> md = {cu_q, cu_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
+  return bwd_launch(attn_bwd_packed_dq_kernel<QCfg>, dim3(unsigned((max_q + QCfg::BM - 1) / QCfg::BM), 1, unsigned(B * H)),
+                    QCfg::THREADS, dq_smem<QCfg>(), s, di, fn, q_tm, qa, md);
 }
 
 }  // namespace b200k
@@ -476,4 +797,79 @@ extern "C" int b200k_fa2_bwd(const void* Q, const void* K, const void* V, const 
                   : run_bwd<1, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
   return narrow ? run_bwd<0, 64>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di)
                 : run_bwd<0, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
+}
+
+// The checks b200k_fa2_bwd_varlen shares with its workspace query.
+static int bwd_varlen_shape(const char* fn, int64_t B, int64_t max_q, int64_t max_k, int64_t total_q, int64_t total_k,
+                            int64_t H, int64_t H_kv) {
+  using namespace b200k;
+  if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
+    return set_error(B200K_ESHAPE, "%s: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)", fn,
+                     (long long)B, (long long)H, (long long)H_kv);
+  if (total_q > INT32_MAX || total_k > INT32_MAX || max_q < 1 || max_q > total_q || max_k < 1 || max_k > total_k)
+    return set_error(B200K_ESHAPE,
+                     "%s: need 1 <= max_seqlen_q <= total_q <= 2^31 - 1 and 1 <= max_seqlen_k <= total_k <= 2^31 - 1 "
+                     "(got max_seqlen_q=%lld total_q=%lld max_seqlen_k=%lld total_k=%lld)",
+                     fn, (long long)max_q, (long long)total_q, (long long)max_k, (long long)total_k);
+  if (B > 65535 || H > 65535 || B * H > 65535)
+    return set_error(B200K_ESHAPE, "%s: B * H = %lld CTAs per query tile, the grid allows 65535", fn,
+                     (long long)B * (long long)H);
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_bwd_varlen_workspace_bytes(int64_t total_q, int64_t H, size_t* bytes) {
+  using namespace b200k;
+  if (!bytes) return set_error(B200K_EARG, "b200k_fa2_bwd_varlen_workspace_bytes: null pointer");
+  if (total_q < 1 || total_q > INT32_MAX || H < 1 || H > 65535)
+    return set_error(B200K_ESHAPE,
+                     "b200k_fa2_bwd_varlen_workspace_bytes: need 1 <= total_q <= 2^31 - 1 and 1 <= H <= 65535 "
+                     "(got total_q=%lld H=%lld)",
+                     (long long)total_q, (long long)H);
+  *bytes = 2 * bwd_section(total_q * H);
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_bwd_varlen(const void* Q, const void* K, const void* V, const void* O, const float* lse,
+                                    const void* dO, void* dQ, void* dK, void* dV, const int* cu_seqlens_q,
+                                    const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t max_seqlen_k,
+                                    int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv, int64_t D, float scale,
+                                    int dtype, int causal, void* workspace, size_t workspace_bytes, void* stream) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_bwd_varlen";
+  if (!Q || !K || !V || !O || !lse || !dO || !dQ || !dK || !dV || !cu_seqlens_q || !cu_seqlens_k || !workspace)
+    return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (dtype != B200K_F16 && dtype != B200K_BF16) return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
+  int rc = check_headdim(fn, D);
+  if (rc || (rc = bwd_varlen_shape(fn, B, max_seqlen_q, max_seqlen_k, total_q, total_k, H, H_kv))) return rc;
+  if ((rc = check_align(fn, {{Q, "Q", 16}, {K, "K", 16}, {V, "V", 16}, {O, "O", 16}, {dO, "dO", 16},
+                             {workspace, "workspace", 16}, {dQ, "dQ", 4}, {dK, "dK", 4}, {dV, "dV", 4}, {lse, "lse", 4},
+                             {cu_seqlens_q, "cu_seqlens_q", 4}, {cu_seqlens_k, "cu_seqlens_k", 4}})))
+    return rc;
+  const int64_t rows = total_q * H;
+  const size_t need = 2 * bwd_section(rows);
+  if (workspace_bytes < need)
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, need, workspace_bytes);
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  BwdArgs a;
+  a.delta = static_cast<const float*>(workspace);
+  a.lse2 = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + bwd_section(rows));
+  a.dst[0] = a.dst[1] = nullptr;
+  a.D = int(D);
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  a.scale = scale;
+  a.scale_log2 = scale * 1.4426950408889634f;
+  auto run = [&](auto dt, auto dp) {
+    return run_bwd_varlen<decltype(dt)::value, decltype(dp)::value>(
+        Q, K, V, O, lse, dO, dQ, dK, dV, cu_seqlens_q, cu_seqlens_k, B, max_seqlen_q, max_seqlen_k, total_q, total_k, H,
+        H_kv, D, causal, a, s, di);
+  };
+  using F16 = std::integral_constant<int, 0>;
+  using BF16 = std::integral_constant<int, 1>;
+  using P64 = std::integral_constant<int, 64>;
+  using P128 = std::integral_constant<int, 128>;
+  const bool narrow = D <= 64;
+  if (dtype == B200K_BF16) return narrow ? run(BF16(), P64()) : run(BF16(), P128());
+  return narrow ? run(F16(), P64()) : run(F16(), P128());
 }

@@ -1,5 +1,6 @@
 // What the attention forward (attn_fwd_wgmma.cu) and backward (attn_bwd_wgmma.cu) share: the kernel configuration, the
-// fp32 -> 16-bit rounding of MMA operands and outputs, the dense [B, H, N, D] addressing, the tensor maps of Q / K / V,
+// fp32 -> 16-bit rounding of MMA operands and outputs, the dense [B, H, N, D] and packed [tokens, H, D] addressing, the
+// tensor maps of Q / K / V,
 // and the argument checks of the entry points.
 #pragma once
 #include "abi_common.cuh"
@@ -67,7 +68,8 @@ struct KvTiles { int first, end; };
 
 // [B, H, N, D], one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).  CTA (x, y, z) =
 // (query tile, O column slice, batch * H + head).  Rows are numbered within the head, so row r sees keys <= r under the
-// causal mask.  The modes of the forward are described in attn_fwd_wgmma.cu; the backward's dQ kernel takes this one.
+// causal mask.  The modes of the forward are described in attn_fwd_wgmma.cu; the backward's dQ kernel takes this one
+// and AttnPacked.
 template <class Cfg>
 struct AttnDense {
   const int* seqlens;  // int32 [B] valid keys per batch, or null
@@ -117,6 +119,67 @@ struct AttnDense {
                                         float, void* O, int D) const {
     size_t row;
     if (out_row(c, r, row)) store_o<Cfg>(O, row, c.dv0, D, o, h, inv);
+  }
+};
+
+// Packed sequences: sequence b is tokens [cu_q[b], cu_q[b+1]) of Q / O ([total_q, H, D]) and [cu_k[b], cu_k[b+1]) of
+// K / V ([total_k, H / group, D]); query head h reads K / V head h / group.  The maps are over (D, heads, tokens).  CTA
+// (x, z) = (query tile of the sequence, b * H + head).  Rows are numbered within the sequence; row r sees keys <=
+// r + Lk - Lq under the causal mask (bottom-right aligned).  Its epilogue stores rows of the sequence within tokens [0, total_q), and reloads cu_q
+// rather than keep it in registers through the main loop.
+template <class Cfg>
+struct AttnPacked {
+  static_assert(!Cfg::V_DN, "packed sequences take V as [tokens, heads, D]");
+  const int* cu_q;
+  const int* cu_k;
+  int H, group, total_q, causal;
+
+  struct Cta { int kv_head, q0, q_tok, k_tok, kv_len, shift; };  // q_tok, k_tok: first tokens; shift: Lk - Lq
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    const int b = blockIdx.z / H;
+    c.kv_head = blockIdx.z % H / group;
+    c.q0 = blockIdx.x * Cfg::BM;
+    c.q_tok = __ldg(cu_q + b);
+    const int q_len = __ldg(cu_q + b + 1) - c.q_tok;
+    if (c.q0 >= q_len) return false;
+    c.k_tok = __ldg(cu_k + b);
+    c.kv_len = __ldg(cu_k + b + 1) - c.k_tok;
+    c.shift = c.kv_len - q_len;
+    return true;
+  }
+  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
+    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
+    const int last = c.q0 + c.shift + Cfg::BM - 1;  // can be negative: no key visible
+    if (causal) nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
+    return {0, nt};
+  }
+  __device__ __forceinline__ int q_bytes() const { return Cfg::BM * 128; }
+  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, blockIdx.z % H, c.q_tok + c.q0, kPolicyEvictFirst);
+  }
+  __device__ __forceinline__ int kv_tile(const Cta& c, int j) const { return c.k_tok + j * Cfg::BN; }
+  __device__ __forceinline__ void load_k(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.kv_head, tok, kPolicyEvictNormal);
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar) const {
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, tok, dst + i * Cfg::BN * 128, tm, bar, i);
+  }
+  __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
+  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ bool out_row(const Cta&, int r, size_t& row) const {
+    const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
+    if (r >= __ldg(cu_q + b + 1) - q_tok) return false;
+    const long long tok = (long long)q_tok + r;
+    if (tok < 0 || tok >= total_q) return false;
+    row = size_t(tok) * H + blockIdx.z % H;
+    return true;
+  }
+  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
+                                        float, void* O, int D) const {
+    size_t row;
+    if (out_row(c, r, row)) store_o<Cfg>(O, row, 0, D, o, h, inv);
   }
 };
 

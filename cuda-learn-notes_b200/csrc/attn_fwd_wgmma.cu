@@ -36,69 +36,8 @@ __device__ __forceinline__ float2 unpack2(uint32_t w) {
 // here; the CTA returns before any barrier exists); tiles, the KV tiles it visits; q_bytes and load_q, the bytes and the
 // box of 64-column chunk c of Q; kv_tile, where KV tile j is, for load_k (chunk c of K) and load_v (all of V); diag,
 // the causal diagonal (last key seen) of row r; zero_v_tail, which only decode fills in; out_row, whether row r is
-// stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.  The dense mode, AttnDense, is in
-// attn_common.cuh, which the backward shares.
-
-// Packed sequences: sequence b is tokens [cu_q[b], cu_q[b+1]) of Q / O ([total_q, H, D]) and [cu_k[b], cu_k[b+1]) of
-// K / V ([total_k, H / group, D]); query head h reads K / V head h / group.  The maps are over (D, heads, tokens).  CTA
-// (x, z) = (query tile of the sequence, b * H + head).  Rows are numbered within the sequence; row r sees keys <=
-// r + Lk - Lq under the causal mask (bottom-right aligned).  Its epilogue stores rows of the sequence within tokens [0, total_q), and reloads cu_q
-// rather than keep it in registers through the main loop.
-template <class Cfg>
-struct AttnPacked {
-  static_assert(!Cfg::V_DN, "packed sequences take V as [tokens, heads, D]");
-  const int* cu_q;
-  const int* cu_k;
-  int H, group, total_q, causal;
-
-  struct Cta { int kv_head, q0, q_tok, k_tok, kv_len, shift; };  // q_tok, k_tok: first tokens; shift: Lk - Lq
-  __device__ __forceinline__ bool setup(Cta& c) const {
-    const int b = blockIdx.z / H;
-    c.kv_head = blockIdx.z % H / group;
-    c.q0 = blockIdx.x * Cfg::BM;
-    c.q_tok = __ldg(cu_q + b);
-    const int q_len = __ldg(cu_q + b + 1) - c.q_tok;
-    if (c.q0 >= q_len) return false;
-    c.k_tok = __ldg(cu_k + b);
-    c.kv_len = __ldg(cu_k + b + 1) - c.k_tok;
-    c.shift = c.kv_len - q_len;
-    return true;
-  }
-  __device__ __forceinline__ KvTiles tiles(const Cta& c) const {
-    int nt = (c.kv_len + Cfg::BN - 1) / Cfg::BN;
-    const int last = c.q0 + c.shift + Cfg::BM - 1;  // can be negative: no key visible
-    if (causal) nt = min(nt, last < 0 ? 0 : last / Cfg::BN + 1);
-    return {0, nt};
-  }
-  __device__ __forceinline__ int q_bytes() const { return Cfg::BM * 128; }
-  __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
-    tma_load_3d(dst, tm, bar, chunk * 64, blockIdx.z % H, c.q_tok + c.q0, kPolicyEvictFirst);
-  }
-  __device__ __forceinline__ int kv_tile(const Cta& c, int j) const { return c.k_tok + j * Cfg::BN; }
-  __device__ __forceinline__ void load_k(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
-                                         int chunk) const {
-    tma_load_3d(dst, tm, bar, chunk * 64, c.kv_head, tok, kPolicyEvictNormal);
-  }
-  __device__ __forceinline__ void load_v(const Cta& c, int tok, uint32_t dst, const CUtensorMap* tm, uint32_t bar) const {
-#pragma unroll
-    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, tok, dst + i * Cfg::BN * 128, tm, bar, i);
-  }
-  __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
-  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
-  __device__ __forceinline__ bool out_row(const Cta&, int r, size_t& row) const {
-    const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
-    if (r >= __ldg(cu_q + b + 1) - q_tok) return false;
-    const long long tok = (long long)q_tok + r;
-    if (tok < 0 || tok >= total_q) return false;
-    row = size_t(tok) * H + blockIdx.z % H;
-    return true;
-  }
-  __device__ __forceinline__ void store(const Cta& c, int r, const float (&o)[Cfg::DV / 2], int h, float inv, float,
-                                        float, void* O, int D) const {
-    size_t row;
-    if (out_row(c, r, row)) store_o<Cfg>(O, row, 0, D, o, h, inv);
-  }
-};
+// stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.  The dense and packed modes, AttnDense
+// and AttnPacked, are in attn_common.cuh, which the backward shares.
 
 // KV-cache decode.  Q / O are [B, Lq, H, D]; the caches are [num_pages, page_size, H_kv, D], key j of sequence b at
 // slot j % page_size of page table[b * pages_per_seq + j / page_size] (table null: contiguous cache, sequence b at rows

@@ -300,6 +300,44 @@ int b200k_fa2_bwd(const void* Q, const void* K, const void* V, const void* O, co
 /* Workspace bytes b200k_fa2_bwd needs for these shapes (no device query); B200K_ESHAPE as b200k_fa2_bwd. */
 int b200k_fa2_bwd_workspace_bytes(int64_t B, int64_t H, int64_t N, size_t* bytes);
 
+/* b200k_fa2_bwd_varlen — the gradients of b200k_fa2_fwd_varlen (flash-attn's varlen backward): packed sequences with
+ * grouped-query K/V heads, the same kernels and arithmetic as b200k_fa2_bwd:
+ *   inputs      Q, O, dO [total_q, H, D] and K, V [total_k, H_kv, D] contiguous in one dtype (B200K_F16 or B200K_BF16);
+ *               lse [total_q, H] fp32 as b200k_fa2_fwd_varlen_lse wrote it (-inf for a row that sees no key).  D in
+ *               {32, 64, 96, 128}; scale <= 0 means 1/sqrt(D)
+ *   sequences   as b200k_fa2_fwd_varlen: sequence b is tokens [cu_seqlens_q[b], cu_seqlens_q[b+1]) of Q and
+ *               [cu_seqlens_k[b], cu_seqlens_k[b+1]) of K / V; query head h reads K/V head h / (H / H_kv); causal is
+ *               bottom-right (row r sees key j iff j <= r + Lk - Lq).  max_seqlen_q / max_seqlen_k size the grids, so
+ *               nothing is read back to the host; a longer sequence is a caller error
+ *   contract    scale, causal and cu_seqlens_* are those of the forward call that produced O and lse (not checked)
+ *   outputs     dQ [total_q, H, D], dK, dV [total_k, H_kv, D], every element written once; nothing else outside the
+ *               workspace is written.  dK and dV of K/V head k sum over the H / H_kv query heads of its group.  Rows are
+ *               +0 for: dQ of a row that sees no key (Lk = 0, or causal with r + Lk - Lq < 0); dK, dV of a key no query
+ *               sees (Lq = 0, or above every causal diagonal); tokens outside every sequence (before cu_seqlens[0] or at
+ *               or past cu_seqlens[B]), whose gradient is 0
+ *   arithmetic  b200k_fa2_bwd's (P and dS rounded to dtype before their products; dV = dtype(sum), dQ, dK =
+ *               dtype(fp32(sum * scale))); the group sum runs query head ascending, then query tile ascending, in one
+ *               thread's registers
+ *   guarantees  deterministic (no atomics, no fp32 accumulation buffer) and no host sync (CUDA-graph capturable).  With
+ *               H_kv = H and Lq = Lk = N for every sequence, the bits of b200k_fa2_bwd on the same data in the dense
+ *               layout.  With finite inputs, each sequence's gradients have the bits of that sequence passed alone (a
+ *               non-finite value in a neighbouring sequence can reach a row as 0 * Inf, as in the forward)
+ *   workspace   >= b200k_fa2_bwd_varlen_workspace_bytes(total_q, H): Delta, then lse * log2 e, fp32 [total_q, H] each on
+ *               a 256-byte boundary
+ *   alignment   Q, K, V, O, dO, workspace 16 bytes; dQ, dK, dV, lse, cu_seqlens_q, cu_seqlens_k 4 bytes
+ * Errors, all before any CUDA call: B200K_EARG for a null pointer, B200K_EDTYPE, B200K_EHEADDIM, B200K_ESHAPE unless
+ * B, H, H_kv >= 1, H % H_kv == 0, 1 <= max_seqlen_q <= total_q <= INT32_MAX, 1 <= max_seqlen_k <= total_k <= INT32_MAX
+ * and B * H <= 65535 (so B * H_kv <= 65535 too), B200K_EALIGN naming the argument, then B200K_EARG for a workspace
+ * below the size above. */
+int b200k_fa2_bwd_varlen(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO,
+                         void* dQ, void* dK, void* dV, const int* cu_seqlens_q, const int* cu_seqlens_k, int64_t B,
+                         int64_t max_seqlen_q, int64_t max_seqlen_k, int64_t total_q, int64_t total_k, int64_t H,
+                         int64_t H_kv, int64_t D, float scale, int dtype, int causal, void* workspace,
+                         size_t workspace_bytes, void* stream);
+/* Workspace bytes b200k_fa2_bwd_varlen needs (no device query); B200K_ESHAPE unless 1 <= total_q <= INT32_MAX and
+ * 1 <= H <= 65535. */
+int b200k_fa2_bwd_varlen_workspace_bytes(int64_t total_q, int64_t H, size_t* bytes);
+
 /* ------------------------------------------------------------------------------------------------ support kernels
  * HBM-roofline kernels (128-bit vectorised, warp-shuffle reductions, no tensor cores).  dtype enums: */
 #define B200K_F32 0
