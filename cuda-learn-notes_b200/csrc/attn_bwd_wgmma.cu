@@ -16,13 +16,13 @@
 // The dK/dV warpgroup holds dK, dV (2 x DP / 2 fp32) and S^T, dP^T (2 x 32): 192 at DP = 128, more than a 384-thread
 // block gives a thread (168), so it runs one consumer warpgroup in a 256-thread block.
 // Packed sequences (b200k_fa2_bwd_varlen) run the same three kernels: the prep also zero-fills the gradients of tokens
-// outside every sequence, a dK/dV CTA owns 64 keys of one K/V head and loops over the query tiles of every query head
-// of its group (so dK / dV sum over the group in registers), and the dQ kernel takes the forward's AttnPacked.
+// outside every sequence, the dK/dV kernel takes BwdKeysPacked (a CTA owns 64 keys of one K/V head and loops over the
+// query tiles of every query head of its group, so dK / dV sum over the group in registers), and the dQ kernel takes
+// the forward's AttnPacked.
 #include "attn_common.cuh"
 
 #include <climits>
 #include <cmath>
-#include <type_traits>
 
 namespace b200k {
 
@@ -30,14 +30,34 @@ namespace b200k {
 // AttnCfg<DT, DP, 2, 64, false> (BM = 128 rows, BN = 64 keys, 384 threads).  DP is the head dim padded to whole 64-column
 // chunks (64 for D = 32 / 64, 128 for D = 96 / 128); TMA zero-fills the padding.
 constexpr int kBwdStages = 2;
+template <class KvCfg>
+using BwdQCfg = AttnCfg<KvCfg::DT, KvCfg::DV, 2, 64, false>;
+
+// A packed gradient tensor viewed as [total, width] 32-bit words, and its cumulative sequence offsets.
+struct BwdPackedGrad {
+  void* p;
+  const int* cu;
+  long long total, width;
+};
+
+// Zeroes the rows of tokens outside every sequence (before cu[0], from cu[B] on), which no main kernel stores.
+__device__ __forceinline__ void zero_outside(const BwdPackedGrad g, int B) {
+  const long long lo = min(max((long long)__ldg(g.cu), 0ll), g.total), hi = min(max((long long)__ldg(g.cu + B), lo), g.total);
+  const long long n = (lo + g.total - hi) * g.width, stride = (long long)gridDim.x * blockDim.x;
+#pragma unroll 1  // an unrolled loop's 64-bit trip count would be a division: a call
+  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride)
+    static_cast<uint32_t*>(g.p)[i < lo * g.width ? i : (hi - lo) * g.width + i] = 0u;
+}
 
 // Delta[row] = sum_d dO[row, d] O[row, d] and lse2[row] = lse[row] * log2 e, one row per quad of threads, 16-byte loads,
 // each thread's products summed in column order, then across the quad in a fixed order.  PACKED: a row that sees no key
-// (lse = -inf) gets lse2 = +inf, so its P is exactly 0 against a masked score too (2^(-inf + inf) would be NaN).
+// (lse = -inf) gets lse2 = +inf, so its P is exactly 0 against a masked score too (2^(-inf + inf) would be NaN); then
+// the zeros of dQ, dK and dV outside the B sequences.  The dense layout passes no sequences.
 template <int DT, bool PACKED>
-__device__ __forceinline__ void bwd_prep(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
-                                         const float* __restrict__ lse, float* __restrict__ delta,
-                                         float* __restrict__ lse2, long long rows, int D) {
+__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(
+    const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO, const float* __restrict__ lse,
+    float* __restrict__ delta, float* __restrict__ lse2, long long rows, int D, int B, const BwdPackedGrad dq,
+    const BwdPackedGrad dk, const BwdPackedGrad dv) {
   const long long stride = (long long)gridDim.x * blockDim.x;
   const int t = threadIdx.x & 3, lane = threadIdx.x & 31;
   // the loop bound is the same for the whole warp (its first thread's index), so the shuffles see every lane
@@ -71,42 +91,11 @@ __device__ __forceinline__ void bwd_prep(const uint16_t* __restrict__ O, const u
       lse2[row] = PACKED && l == -INFINITY ? INFINITY : l * 1.4426950408889634f;
     }
   }
-}
-
-template <int DT>
-__global__ void __launch_bounds__(256) attn_bwd_prep_kernel(const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO,
-                                                            const float* __restrict__ lse, float* __restrict__ delta,
-                                                            float* __restrict__ lse2, long long rows, int D) {
-  bwd_prep<DT, false>(O, dO, lse, delta, lse2, rows, D);
-}
-
-// A packed gradient tensor viewed as [total, width] 32-bit words, and its cumulative sequence offsets.
-struct BwdPackedGrad {
-  void* p;
-  const int* cu;
-  long long total, width;
-};
-
-// Zeroes the rows of tokens outside every sequence (before cu[0], from cu[B] on), which no main kernel stores.
-__device__ __forceinline__ void zero_outside(const BwdPackedGrad g, int B) {
-  const long long lo = min(max((long long)__ldg(g.cu), 0ll), g.total), hi = min(max((long long)__ldg(g.cu + B), lo), g.total);
-  const long long n = (lo + g.total - hi) * g.width, stride = (long long)gridDim.x * blockDim.x;
-#pragma unroll 1  // an unrolled loop's 64-bit trip count would be a division: a call
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += stride)
-    static_cast<uint32_t*>(g.p)[i < lo * g.width ? i : (hi - lo) * g.width + i] = 0u;
-}
-
-// The packed layout's prep: Delta and lse2 of every [total_q * H] row, then the zeros of dQ, dK and dV outside every
-// sequence.
-template <int DT>
-__global__ void __launch_bounds__(256) attn_bwd_packed_prep_kernel(
-    const uint16_t* __restrict__ O, const uint16_t* __restrict__ dO, const float* __restrict__ lse,
-    float* __restrict__ delta, float* __restrict__ lse2, long long rows, int D, int B, const BwdPackedGrad dq,
-    const BwdPackedGrad dk, const BwdPackedGrad dv) {
-  bwd_prep<DT, true>(O, dO, lse, delta, lse2, rows, D);
-  zero_outside(dq, B);
-  zero_outside(dk, B);
-  zero_outside(dv, B);
+  if constexpr (PACKED) {
+    zero_outside(dq, B);
+    zero_outside(dk, B);
+    zero_outside(dv, B);
+  }
 }
 
 // What both main kernels take beyond their tensor maps.
@@ -118,165 +107,55 @@ struct BwdArgs {
   float scale_log2, scale;
 };
 
-// Rows past a CTA's query rows (ragged N) have zero-filled Q and dO; lse2 = +inf there makes their P exactly 0.
-__device__ __forceinline__ void load_row_stats(const BwdArgs& a, size_t base, int r, int N, float& l2, float& dl) {
-  l2 = r < N ? __ldg(a.lse2 + base + r) : INFINITY;
-  dl = r < N ? __ldg(a.delta + base + r) : 0.f;
-}
+// The addressing modes of the dK/dV kernel.  Each places CTA (x, y) = (key tile, y), loads its K / V tile and its query
+// tiles, and gives the causal diagonal, the row statistics and the store row of a key.  `group` query heads share the
+// CTA's K / V head.
 
-// dK, dV of one 64-key tile.  CTA (x, y) = (key tile, b * H + h).  Warpgroup 0 produces (one thread issues TMA),
-// warpgroup 1 computes; thread rows (keys) k0 + 16 warp + lane / 4 and + 8, columns (queries) q0 + 8 j + 2 (lane % 4) + e.
+// Dense: y = b * H + h.  Every key < N is stored: keys past seqlens_k (clamped to [1, N]) are masked, so they store
+// zeros, and a key tile past it sees no query tile.  Rows past N (ragged N) have zero-filled Q and dO; lse2 = +inf
+// there makes their P exactly 0.
 template <class Cfg>
-__global__ void __launch_bounds__(Cfg::THREADS, 1)
-    attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                         const BwdArgs a, const int* seqlens, int N, int H, int causal) {
-  static_assert(Cfg::NWG == 1 && Cfg::BM == 64 && Cfg::BN == 64, "dK/dV: one warpgroup of 64 keys, query tiles of 64");
-  constexpr int DP = Cfg::DV, NC = DP / 64, TILE = 64 * DP * 2, ST = kBwdStages;
-  extern __shared__ uint8_t smem_raw[];
-  const uint32_t sK = (smem_u32(smem_raw) + 1023) & ~1023u, sV = sK + TILE, sQ = sV + TILE;  // stage s: Q, then dO
-  const uint32_t kvbar = sQ + ST * 2 * TILE, full = kvbar + 8, empty = full + 8 * ST;
+struct BwdKeysDense {
+  static constexpr int group = 1;
+  const int* seqlens;  // int32 [B] valid keys per batch, or null
+  int N, H, causal;
 
-  const int bh = blockIdx.y, k0 = blockIdx.x * 64;
-  const int kv_len = seqlens ? min(max(__ldg(seqlens + bh / H), 1), N) : N;
-  // query tiles that see a key of this tile: all of them, from the one holding row k0 when causal; none past the length
-  const int first = causal ? k0 / 64 : 0, end = k0 < kv_len ? (N + 63) / 64 : first;
-  const int wg = threadIdx.x / 128;
-
-  if (threadIdx.x == 0) {
-    mbar_init(kvbar, 1);
-    for (int s = 0; s < ST; ++s) {
-      mbar_init(full + 8 * s, 1);
-      mbar_init(empty + 8 * s, 1);
-    }
-    fence_mbar_init();
+  struct Cta { int bh, k0, kv_len, first, end; };
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    c.bh = blockIdx.y;
+    c.k0 = blockIdx.x * 64;
+    c.kv_len = seqlens ? min(max(__ldg(seqlens + c.bh / H), 1), N) : N;
+    // query tiles that see a key of this tile: all of them, from the one holding row k0 when causal; none past the length
+    c.first = causal ? c.k0 / 64 : 0;
+    c.end = c.k0 < c.kv_len ? (N + 63) / 64 : c.first;
+    return true;
   }
-  __syncthreads();
-
-  if (wg == 0) {
-    if (threadIdx.x == 0 && first < end) {
-      mbar_arrive_expect_tx(kvbar, 2 * TILE);
-      for (int c = 0; c < NC; ++c) {
-        tma_load_3d(sK + c * 8192, &tmK, kvbar, c * 64, k0, bh, kPolicyEvictFirst);
-        tma_load_3d(sV + c * 8192, &tmV, kvbar, c * 64, k0, bh, kPolicyEvictFirst);
-      }
-      for (int i = first; i < end; ++i) {
-        const int n = i - first, s = n % ST;
-        if (n >= ST) mbar_wait_nocall(empty + 8 * s, ((n / ST) - 1) & 1);
-        mbar_arrive_expect_tx(full + 8 * s, 2 * TILE);
-        const uint32_t q = sQ + s * 2 * TILE;
-        for (int c = 0; c < NC; ++c) {
-          tma_load_3d(q + c * 8192, &tmQ, full + 8 * s, c * 64, i * 64, bh, kPolicyEvictNormal);
-          tma_load_3d(q + TILE + c * 8192, &tmdO, full + 8 * s, c * 64, i * 64, bh, kPolicyEvictNormal);
-        }
-      }
-    }
-    return;
+  __device__ __forceinline__ void load_kv(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                          int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, c.k0, c.bh, kPolicyEvictFirst);
   }
-
-  const int lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
-  const int key0 = k0 + warp * 16 + lane / 4;  // this thread's keys: key0 and key0 + 8
-  const size_t base = size_t(bh) * N;
-  float dk[DP / 2], dv[DP / 2];
-#pragma unroll
-  for (int i = 0; i < DP / 2; ++i) dk[i] = dv[i] = 0.f;
-  if (first < end) mbar_wait_nocall(kvbar, 0);
-
-  for (int i = first; i < end; ++i) {
-    const int n = i - first, s = n % ST, q0 = i * 64;
-    const uint32_t sq = sQ + s * 2 * TILE, sdo = sq + TILE;
-    float st[32], dpt[32];
-#pragma unroll
-    for (int e = 0; e < 32; ++e) st[e] = dpt[e] = 0.f;
-    mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
-    fence_regs<32>(st);
-    fence_regs<32>(dpt);
-    wgmma_fence();
-#pragma unroll
-    for (int c = 0; c < NC; ++c)
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_ss<Cfg::DT, 64, 0, 0>(st, wgmma_desc(sK + c * 8192 + k * 32, 16, 1024),
-                                    wgmma_desc(sq + c * 8192 + k * 32, 16, 1024), 1);
-#pragma unroll
-    for (int c = 0; c < NC; ++c)
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        wgmma_ss<Cfg::DT, 64, 0, 0>(dpt, wgmma_desc(sV + c * 8192 + k * 32, 16, 1024),
-                                    wgmma_desc(sdo + c * 8192 + k * 32, 16, 1024), 1);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs<32>(st);
-    fence_regs<32>(dpt);
-
-    // masks: keys past the length, and (causal) keys after the query's diagonal.  A masked score becomes -inf (P = 0)
-    // and its dP 0, so nothing a padded key holds reaches dS.
-    if (k0 + 64 > kv_len || (causal && k0 + 63 > q0)) {
-#pragma unroll
-      for (int j = 0; j < 8; ++j)
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const int key = key0 + 8 * h, q = q0 + 8 * j + 2 * (lane & 3) + e;
-            if (key >= kv_len || (causal && key > q)) {
-              st[4 * j + 2 * h + e] = -INFINITY;
-              dpt[4 * j + 2 * h + e] = 0.f;
-            }
-          }
-    }
-    uint32_t pa[4][4], da[4][4];
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      float l2[2], dl[2];
-#pragma unroll
-      for (int e = 0; e < 2; ++e) load_row_stats(a, base, q0 + 8 * j + 2 * (lane & 3) + e, N, l2[e], dl[e]);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        float p[2], ds[2];
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          p[e] = ex2(fmaf(st[4 * j + 2 * h + e], a.scale_log2, -l2[e]));
-          ds[e] = p[e] * (dpt[4 * j + 2 * h + e] - dl[e]);
-        }
-        pa[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(p[0], p[1]);
-        da[j / 2][(j & 1) * 2 + h] = pack_round<Cfg::DT>(ds[0], ds[1]);
-      }
-    }
-
-    // dV += P~^T dO_i, dK += dS~^T Q_i over the tile's 64 queries
-    fence_regs<DP / 2>(dv);
-    fence_regs<DP / 2>(dk);
-    wgmma_fence();
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dv, pa[kk], wgmma_desc(sdo + kk * 2048, 8192, 1024), 1);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk) wgmma_rs<Cfg::DT, DP, 1>(dk, da[kk], wgmma_desc(sq + kk * 2048, 8192, 1024), 1);
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs<DP / 2>(dv);
-    fence_regs<DP / 2>(dk);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk)  // the A registers are read by the MMAs until the wait above
-#pragma unroll
-      for (int e = 0; e < 4; ++e) asm volatile("" : "+r"(pa[kk][e]), "+r"(da[kk][e])::"memory");
-    if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * s);
+  __device__ __forceinline__ void load_q(const Cta& c, int, int i, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    tma_load_3d(dst, tm, bar, chunk * 64, i * 64, c.bh, kPolicyEvictNormal);
   }
-
-  // keys past N are not stored; keys past the length (and tiles no query sees) store the zeros they hold
-#pragma unroll
-  for (int h = 0; h < 2; ++h) {
-    const int key = key0 + 8 * h;
-    if (key >= N) continue;
-    store_o<Cfg>(a.dst[0], base + key, 0, a.D, dk, h, a.scale);
-    store_o<Cfg>(a.dst[1], base + key, 0, a.D, dv, h, 1.f);
+  __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
+  __device__ __forceinline__ void row_stats(const BwdArgs& a, const Cta& c, int, int r, float& l2, float& dl) const {
+    const size_t base = size_t(c.bh) * N;
+    l2 = r < N ? __ldg(a.lse2 + base + r) : INFINITY;
+    dl = r < N ? __ldg(a.delta + base + r) : 0.f;
   }
-}
+  __device__ __forceinline__ bool key_row(const Cta& c, int k, size_t& row) const {
+    if (k >= N) return false;
+    row = size_t(c.bh) * N + k;
+    return true;
+  }
+};
 
-// Packed (AttnPacked's layout): CTA (x, y) = (key tile of sequence b, b * H_kv + K/V head), which visits the query tiles
-// of each query head h = K/V head * group + g of its group in turn, g ascending.  A query tile that runs past Lq reads
-// the next sequence's rows: their lse2 is +inf, so their P and dS are 0.  Keys past Lk are masked and not stored.  Row r
-// sees keys <= r + Lk - Lq under the causal mask.  The store reloads cu_k rather than keep it through the main loop.
+// Packed (AttnPacked's layout): y = b * H_kv + K/V head; the CTA visits the query tiles of each query head
+// h = K/V head * group + g of its group in turn, g ascending.  A key tile past Lk returns.  A query tile that runs past
+// Lq reads the next sequence's rows: their lse2 is +inf, so their P and dS are 0.  Keys past Lk are masked and not
+// stored.  Row r sees keys <= r + Lk - Lq under the causal mask.  The store reloads cu_k rather than keep it through the
+// main loop.
 template <class Cfg>
 struct BwdKeysPacked {
   const int* cu_q;
@@ -319,22 +198,22 @@ struct BwdKeysPacked {
   }
 };
 
-// Packed dK, dV of one 64-key tile: attn_bwd_dkdv_kernel's geometry and arithmetic, placed and fed by BwdKeysPacked.
-// The query tiles of the group's heads stream through one ring, head by head; dK and dV sum over all of them in this
-// thread's registers.  (The dense kernel keeps its own copy of this body: sharing one template changes ptxas's
-// register allocation of the dense instantiations.)
-template <class Cfg>
+// dK, dV of one 64-key tile, placed and fed by Mode (BwdKeysDense or BwdKeysPacked).  Warpgroup 0 produces (one thread
+// issues TMA), warpgroup 1 computes; thread rows (keys) k0 + 16 warp + lane / 4 and + 8, columns (queries)
+// q0 + 8 j + 2 (lane % 4) + e.  The query tiles of the group's heads stream through one ring, head by head; dK and dV
+// sum over all of them in this thread's registers.
+template <class Cfg, class Mode>
 __global__ void __launch_bounds__(Cfg::THREADS, 1)
-    attn_bwd_packed_dkdv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                                const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                                const BwdArgs a, const BwdKeysPacked<Cfg> md) {
+    attn_bwd_dkdv_kernel(const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                         const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                         const BwdArgs a, const Mode md) {
   static_assert(Cfg::NWG == 1 && Cfg::BM == 64 && Cfg::BN == 64, "dK/dV: one warpgroup of 64 keys, query tiles of 64");
   constexpr int DP = Cfg::DV, NC = DP / 64, TILE = 64 * DP * 2, ST = kBwdStages;
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sK = (smem_u32(smem_raw) + 1023) & ~1023u, sV = sK + TILE, sQ = sV + TILE;  // stage s: Q, then dO
   const uint32_t kvbar = sQ + ST * 2 * TILE, full = kvbar + 8, empty = full + 8 * ST;
 
-  typename BwdKeysPacked<Cfg>::Cta c;
+  typename Mode::Cta c;
   if (!md.setup(c)) return;
   const int k0 = c.k0, first = c.first, end = c.end;
   const int wg = threadIdx.x / 128;
@@ -460,7 +339,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
       if ((threadIdx.x & 127) == 0) mbar_arrive(empty + 8 * s);
     }
 
-  // keys past the sequence are not stored; tiles no query sees store the zeros they hold
+  // keys the mode does not store are skipped; tiles no query sees store the zeros they hold
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     size_t row;
@@ -470,28 +349,13 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
   }
 }
 
-// lse2 and Delta of row r of a dQ CTA: the row the mode stores it to, or padding (+inf, 0) when it stores none (rows
-// past N or past the sequence).
-template <class Mode>
-__device__ __forceinline__ void out_row_stats(const BwdArgs& a, const Mode& md, const typename Mode::Cta& c, int r,
-                                              float& l2, float& dl) {
-  size_t row = 0;
-  const bool in = md.out_row(c, r, row);
-  l2 = in ? __ldg(a.lse2 + row) : INFINITY;
-  dl = in ? __ldg(a.delta + row) : 0.f;
-}
-
-template <class Cfg>
-__device__ __forceinline__ void out_row_stats(const BwdArgs& a, const AttnDense<Cfg>& md,
-                                              const typename AttnDense<Cfg>::Cta& c, int r, float& l2, float& dl) {
-  load_row_stats(a, size_t(c.bh) * md.N, r, md.N, l2, dl);
-}
-
 // dQ of one query tile, placed and fed by the forward's addressing mode (AttnDense or AttnPacked) on CTA (query tile,
-// 0, b * H + h).
+// 0, b * H + h); a packed tile past the sequence returns.
 template <class Cfg, class Mode>
-__device__ __forceinline__ void bwd_dq(const CUtensorMap& tmQ, const CUtensorMap& tmdO, const CUtensorMap& tmK,
-                                       const CUtensorMap& tmV, const BwdArgs& a, const Mode& md) {
+__global__ void __launch_bounds__(Cfg::THREADS, 1)
+    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
+                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
+                       const BwdArgs a, const Mode md) {
   static_assert(Cfg::BN == 64 && !Cfg::V_DN, "dQ: KV tiles of 64 keys, V [N, D]");
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DP = Cfg::DV, NC = DP / 64, ST = kBwdStages;
   constexpr int QB = BM * DP * 2, KB = Cfg::V_BYTES;  // a resident Q / dO tile, a streamed K / V tile
@@ -535,9 +399,15 @@ __device__ __forceinline__ void bwd_dq(const CUtensorMap& tmQ, const CUtensorMap
 
   const int cw = wg - 1, lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
   const int row0 = cta.q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
+  // lse2 and Delta of the row the mode stores, or padding (+inf, 0) for a row it does not (past N or the sequence)
   float l2[2], dl[2];
 #pragma unroll
-  for (int h = 0; h < 2; ++h) out_row_stats(a, md, cta, row0 + 8 * h, l2[h], dl[h]);
+  for (int h = 0; h < 2; ++h) {
+    size_t row = 0;
+    const bool in = md.out_row(cta, row0 + 8 * h, row);
+    l2[h] = in ? __ldg(a.lse2 + row) : INFINITY;
+    dl[h] = in ? __ldg(a.delta + row) : 0.f;
+  }
   float dq[DP / 2];
 #pragma unroll
   for (int i = 0; i < DP / 2; ++i) dq[i] = 0.f;
@@ -618,25 +488,31 @@ __device__ __forceinline__ void bwd_dq(const CUtensorMap& tmQ, const CUtensorMap
   for (int h = 0; h < 2; ++h) md.store(cta, row0 + 8 * h, dq, h, a.scale, 0.f, 0.f, a.dst[0], a.D);
 }
 
-template <class Cfg>
-__global__ void __launch_bounds__(Cfg::THREADS, 1)
-    attn_bwd_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                       const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                       const BwdArgs a, const AttnDense<Cfg> md) {
-  bwd_dq<Cfg>(tmQ, tmdO, tmK, tmV, a, md);
-}
-
-// Packed dQ: AttnPacked places the CTA (query tile of the sequence, 0, b * H + h); a tile past the sequence returns.
-template <class Cfg>
-__global__ void __launch_bounds__(Cfg::THREADS, 1)
-    attn_bwd_packed_dq_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmdO,
-                              const __grid_constant__ CUtensorMap tmK, const __grid_constant__ CUtensorMap tmV,
-                              const BwdArgs a, const AttnPacked<Cfg> md) {
-  bwd_dq<Cfg>(tmQ, tmdO, tmK, tmV, a, md);
-}
-
-// Workspace: Delta, then lse * log2 e, fp32 [B * H * N] each, each on a 256-byte boundary.
+// Workspace: Delta, then lse * log2 e, fp32 [rows] each, each on a 256-byte boundary.
 static size_t bwd_section(int64_t rows) { return (size_t(rows) * sizeof(float) + 255) & ~size_t(255); }
+
+// Checks that the workspace holds both sections of `rows` rows, and fills `a` with them, D and the scale (scale <= 0
+// means 1 / sqrt(D)).  Each main kernel's launch sets dst.
+static int bwd_args(const char* fn, int64_t rows, int64_t D, float scale, void* workspace, size_t workspace_bytes,
+                    BwdArgs& a) {
+  const size_t need = 2 * bwd_section(rows);
+  if (workspace_bytes < need)
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, need, workspace_bytes);
+  a.delta = static_cast<const float*>(workspace);
+  a.lse2 = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + bwd_section(rows));
+  a.dst[0] = a.dst[1] = nullptr;
+  a.D = int(D);
+  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
+  a.scale = scale;
+  a.scale_log2 = scale * 1.4426950408889634f;
+  return B200K_OK;
+}
+
+// The prep kernel's grid: a quad of threads per row, at most 2^20 blocks of 256.
+static unsigned bwd_prep_blocks(long long rows) {
+  const long long blocks = (rows * 4 + 255) / 256;
+  return unsigned(blocks < (1 << 20) ? blocks : (1 << 20));
+}
 
 static int bwd_shape(const char* fn, int64_t B, int64_t H, int64_t N) {
   if (B < 1 || H < 1 || N < 1 || N > INT32_MAX || B * H > 65535)
@@ -645,28 +521,23 @@ static int bwd_shape(const char* fn, int64_t B, int64_t H, int64_t N) {
   return B200K_OK;
 }
 
-template <class Kern, class... Rest>
+// The configurations: dtype, and DP = 64 for D = 32 / 64, 128 for D = 96 / 128.  `run` gets the dK/dV kernel's.
+template <class Run>
+static int run_bwd_cfg(int dtype, int64_t D, Run run) {
+  const bool narrow = D <= 64;
+  if (dtype == B200K_BF16) return narrow ? run(AttnCfg<1, 64, 1, 64, false>()) : run(AttnCfg<1, 128, 1, 64, false>());
+  return narrow ? run(AttnCfg<0, 64, 1, 64, false>()) : run(AttnCfg<0, 128, 1, 64, false>());
+}
+
+template <class Kern, class Mode>
 static int bwd_launch(Kern kern, dim3 grid, int threads, int smem, cudaStream_t s, const DeviceInfo& di, const char* fn,
-                      const CUtensorMap (&tm)[4], const BwdArgs& a, Rest... rest) {
+                      const CUtensorMap (&tm)[4], const BwdArgs& a, const Mode& md) {
   if (smem > di.max_smem_optin)
     return set_error(B200K_ESHAPE, "%s: %d bytes of shared memory needed, device allows %d", fn, smem, di.max_smem_optin);
   int rc = ensure_dynamic_smem(reinterpret_cast<const void*>(kern), di.device, smem);
   if (rc) return rc;
-  kern<<<grid, threads, smem, s>>>(tm[0], tm[1], tm[2], tm[3], a, rest...);
+  kern<<<grid, threads, smem, s>>>(tm[0], tm[1], tm[2], tm[3], a, md);
   B200K_CHECK_CUDA(cudaGetLastError());
-  return B200K_OK;
-}
-
-// The maps of both main kernels: dK/dV kernel K, V, Q, dO in 64-row boxes; dQ kernel Q, dO in 128-row boxes, K, V.
-static int bwd_tmaps(const AttnTensor (&kv_t)[4], const AttnTensor (&q_t)[2], CUtensorMap (&kv_tm)[4],
-                     CUtensorMap (&q_tm)[4]) {
-  int rc;
-  for (int i = 0; i < 4; ++i)
-    if ((rc = attn_tmap(&kv_tm[i], kv_t[i]))) return rc;
-  for (int i = 0; i < 2; ++i)
-    if ((rc = attn_tmap(&q_tm[i], q_t[i]))) return rc;
-  q_tm[2] = kv_tm[0];
-  q_tm[3] = kv_tm[1];
   return B200K_OK;
 }
 
@@ -676,78 +547,32 @@ constexpr int dkdv_smem() { return 1024 + (2 + 2 * kBwdStages) * 64 * DP * 2 + k
 template <class QCfg>
 constexpr int dq_smem() { return 1024 + 2 * QCfg::BM * QCfg::DV * 2 + 2 * kBwdStages * QCfg::V_BYTES + kBwdBars; }
 
-template <int DT, int DP>
-static int run_bwd(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO, void* dQ,
-                   void* dK, void* dV, int64_t B, int64_t H, int64_t N, int64_t D, const int* seqlens, int causal,
-                   BwdArgs a, cudaStream_t s, const DeviceInfo& di) {
-  using KvCfg = AttnCfg<DT, DP, 1, 64, false>;
-  using QCfg = AttnCfg<DT, DP, 2, 64, false>;
-  const int64_t BH = B * H;
-  // The prep kernel goes first: its launch makes the device's primary context current on the calling thread, which the
-  // tensor-map encoder (a driver call) needs.  torch runs a backward on an autograd thread of its own, where no CUDA
-  // runtime call may have run yet.
-  const long long rows = BH * N, blocks = (rows * 4 + 255) / 256;
-  attn_bwd_prep_kernel<DT><<<unsigned(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(
-      static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
-      const_cast<float*>(a.lse2), rows, int(D));
-  B200K_CHECK_CUDA(cudaGetLastError());
+// The main kernels of both layouts: the dK/dV kernel under `km` on `kv_grid`, reading K, V, Q, dO through maps of
+// 64-row boxes (kv_t), then the dQ kernel under `qm` on `q_grid`, reading Q, dO in 128-row boxes (q_t) and the same
+// K, V.  The prep kernel goes first: its launch makes the device's primary context current on the calling thread,
+// which the tensor-map encoder (a driver call) needs.  torch runs a backward on an autograd thread of its own, where
+// no CUDA runtime call may have run yet.
+template <class KvCfg, class KvMode, class QMode>
+static int bwd_main(const char* fn, const AttnTensor (&kv_t)[4], const AttnTensor (&q_t)[2], const KvMode& km,
+                    dim3 kv_grid, const QMode& qm, dim3 q_grid, BwdArgs a, void* dQ, void* dK, void* dV, cudaStream_t s,
+                    const DeviceInfo& di) {
+  using QCfg = BwdQCfg<KvCfg>;
   CUtensorMap kv_tm[4], q_tm[4];
-  const AttnTensor kv_t[4] = {{K, BH, N, D, 1, 64}, {V, BH, N, D, 1, 64}, {Q, BH, N, D, 1, 64}, {dO, BH, N, D, 1, 64}};
-  const AttnTensor q_t[2] = {{Q, BH, N, D, 1, QCfg::BM}, {dO, BH, N, D, 1, QCfg::BM}};
-  int rc = bwd_tmaps(kv_t, q_t, kv_tm, q_tm);
+  int rc;
+  for (int i = 0; i < 4; ++i)
+    if ((rc = attn_tmap(&kv_tm[i], kv_t[i]))) return rc;
+  for (int i = 0; i < 2; ++i)
+    if ((rc = attn_tmap(&q_tm[i], q_t[i]))) return rc;
+  q_tm[2] = kv_tm[0];
+  q_tm[3] = kv_tm[1];
+  a.dst[0] = dK;
+  a.dst[1] = dV;
+  rc = bwd_launch(attn_bwd_dkdv_kernel<KvCfg, KvMode>, kv_grid, KvCfg::THREADS, dkdv_smem<KvCfg::DV>(), s, di, fn, kv_tm,
+                  a, km);
   if (rc) return rc;
-  const char* fn = "b200k_fa2_bwd";
-  BwdArgs kva = a;
-  kva.dst[0] = dK;
-  kva.dst[1] = dV;
-  rc = bwd_launch(attn_bwd_dkdv_kernel<KvCfg>, dim3(unsigned((N + 63) / 64), unsigned(BH)), KvCfg::THREADS,
-                  dkdv_smem<DP>(), s, di, fn, kv_tm, kva, seqlens, int(N), int(H), causal ? 1 : 0);
-  if (rc) return rc;
-  BwdArgs qa = a;
-  qa.dst[0] = dQ;
-  qa.dst[1] = nullptr;
-  const AttnDense<QCfg> md = {seqlens, int(N), int(H), causal ? 1 : 0};
-  return bwd_launch(attn_bwd_dq_kernel<QCfg>, dim3(unsigned((N + QCfg::BM - 1) / QCfg::BM), 1, unsigned(BH)),
-                    QCfg::THREADS, dq_smem<QCfg>(), s, di, fn, q_tm, qa, md);
-}
-
-// The packed layout: the same kernels under BwdKeysPacked / AttnPacked, the maps over (D, heads, tokens), grids sized by
-// the longest sequences.  The prep also zero-fills the gradient rows of tokens outside every sequence.
-template <int DT, int DP>
-static int run_bwd_varlen(const void* Q, const void* K, const void* V, const void* O, const float* lse, const void* dO,
-                          void* dQ, void* dK, void* dV, const int* cu_q, const int* cu_k, int64_t B, int64_t max_q,
-                          int64_t max_k, int64_t total_q, int64_t total_k, int64_t H, int64_t H_kv, int64_t D, int causal,
-                          BwdArgs a, cudaStream_t s, const DeviceInfo& di) {
-  using KvCfg = AttnCfg<DT, DP, 1, 64, false>;
-  using QCfg = AttnCfg<DT, DP, 2, 64, false>;
-  // first, for the reason run_bwd gives
-  const long long rows = total_q * H, blocks = (rows * 4 + 255) / 256;
-  const BwdPackedGrad gq = {dQ, cu_q, total_q, H * D / 2}, gk = {dK, cu_k, total_k, H_kv * D / 2},
-                      gv = {dV, cu_k, total_k, H_kv * D / 2};
-  attn_bwd_packed_prep_kernel<DT><<<unsigned(blocks < (1 << 20) ? blocks : (1 << 20)), 256, 0, s>>>(
-      static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
-      const_cast<float*>(a.lse2), rows, int(D), int(B), gq, gk, gv);
-  B200K_CHECK_CUDA(cudaGetLastError());
-  CUtensorMap kv_tm[4], q_tm[4];
-  const AttnTensor kv_t[4] = {{K, total_k, H_kv, D, 64, 1}, {V, total_k, H_kv, D, 64, 1}, {Q, total_q, H, D, 64, 1},
-                              {dO, total_q, H, D, 64, 1}};
-  const AttnTensor q_t[2] = {{Q, total_q, H, D, QCfg::BM, 1}, {dO, total_q, H, D, QCfg::BM, 1}};
-  int rc = bwd_tmaps(kv_t, q_t, kv_tm, q_tm);
-  if (rc) return rc;
-  const char* fn = "b200k_fa2_bwd_varlen";
-  BwdArgs kva = a;
-  kva.dst[0] = dK;
-  kva.dst[1] = dV;
-  const BwdKeysPacked<KvCfg> km = {cu_q, cu_k, int(H), int(H_kv), int(H / H_kv), causal ? 1 : 0};
-  rc = bwd_launch(attn_bwd_packed_dkdv_kernel<KvCfg>, dim3(unsigned((max_k + 63) / 64), unsigned(B * H_kv)),
-                  KvCfg::THREADS, dkdv_smem<DP>(), s, di, fn, kv_tm, kva, km);
-  if (rc) return rc;
-  BwdArgs qa = a;
-  qa.dst[0] = dQ;
-  qa.dst[1] = nullptr;
-  const AttnPacked<QCfg> md = {cu_q, cu_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
-  return bwd_launch(attn_bwd_packed_dq_kernel<QCfg>, dim3(unsigned((max_q + QCfg::BM - 1) / QCfg::BM), 1, unsigned(B * H)),
-                    QCfg::THREADS, dq_smem<QCfg>(), s, di, fn, q_tm, qa, md);
+  a.dst[0] = dQ;
+  a.dst[1] = nullptr;
+  return bwd_launch(attn_bwd_dq_kernel<QCfg, QMode>, q_grid, QCfg::THREADS, dq_smem<QCfg>(), s, di, fn, q_tm, a, qm);
 }
 
 }  // namespace b200k
@@ -776,27 +601,26 @@ extern "C" int b200k_fa2_bwd(const void* Q, const void* K, const void* V, const 
                              {workspace, "workspace", 16}, {dQ, "dQ", 4}, {dK, "dK", 4}, {dV, "dV", 4}, {lse, "lse", 4},
                              {seqlens_k, "seqlens_k", 4}})))
     return rc;
-  const int64_t rows = B * H * N;
-  const size_t need = 2 * bwd_section(rows);
-  if (workspace_bytes < need)
-    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, need, workspace_bytes);
+  const int64_t BH = B * H, rows = BH * N;
+  BwdArgs a;
+  if ((rc = bwd_args(fn, rows, D, scale, workspace, workspace_bytes, a))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  BwdArgs a;
-  a.delta = static_cast<const float*>(workspace);
-  a.lse2 = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + bwd_section(rows));
-  a.dst[0] = a.dst[1] = nullptr;
-  a.D = int(D);
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
-  a.scale = scale;
-  a.scale_log2 = scale * 1.4426950408889634f;
-  const bool narrow = D <= 64;
-  if (dtype == B200K_BF16)
-    return narrow ? run_bwd<1, 64>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di)
-                  : run_bwd<1, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
-  return narrow ? run_bwd<0, 64>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di)
-                : run_bwd<0, 128>(Q, K, V, O, lse, dO, dQ, dK, dV, B, H, N, D, seqlens_k, causal, a, s, di);
+  return run_bwd_cfg(dtype, D, [&](auto cfg) {
+    using KvCfg = decltype(cfg);
+    using QCfg = BwdQCfg<KvCfg>;
+    attn_bwd_prep_kernel<KvCfg::DT, false><<<bwd_prep_blocks(rows), 256, 0, s>>>(
+        static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
+        const_cast<float*>(a.lse2), rows, int(D), 0, {}, {}, {});
+    B200K_CHECK_CUDA(cudaGetLastError());
+    const AttnTensor kv_t[4] = {{K, BH, N, D, 1, 64}, {V, BH, N, D, 1, 64}, {Q, BH, N, D, 1, 64}, {dO, BH, N, D, 1, 64}};
+    const AttnTensor q_t[2] = {{Q, BH, N, D, 1, QCfg::BM}, {dO, BH, N, D, 1, QCfg::BM}};
+    const BwdKeysDense<KvCfg> km = {seqlens_k, int(N), int(H), causal ? 1 : 0};
+    const AttnDense<QCfg> qm = {seqlens_k, int(N), int(H), causal ? 1 : 0};
+    return bwd_main<KvCfg>(fn, kv_t, q_t, km, dim3(unsigned((N + 63) / 64), unsigned(BH)), qm,
+                           dim3(unsigned((N + QCfg::BM - 1) / QCfg::BM), 1, unsigned(BH)), a, dQ, dK, dV, s, di);
+  });
 }
 
 // The checks b200k_fa2_bwd_varlen shares with its workspace query.
@@ -829,6 +653,7 @@ extern "C" int b200k_fa2_bwd_varlen_workspace_bytes(int64_t total_q, int64_t H, 
   return B200K_OK;
 }
 
+// The packed layout: the maps over (D, heads, tokens), grids sized by the longest sequences.
 extern "C" int b200k_fa2_bwd_varlen(const void* Q, const void* K, const void* V, const void* O, const float* lse,
                                     const void* dO, void* dQ, void* dK, void* dV, const int* cu_seqlens_q,
                                     const int* cu_seqlens_k, int64_t B, int64_t max_seqlen_q, int64_t max_seqlen_k,
@@ -846,30 +671,27 @@ extern "C" int b200k_fa2_bwd_varlen(const void* Q, const void* K, const void* V,
                              {cu_seqlens_q, "cu_seqlens_q", 4}, {cu_seqlens_k, "cu_seqlens_k", 4}})))
     return rc;
   const int64_t rows = total_q * H;
-  const size_t need = 2 * bwd_section(rows);
-  if (workspace_bytes < need)
-    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, need, workspace_bytes);
+  BwdArgs a;
+  if ((rc = bwd_args(fn, rows, D, scale, workspace, workspace_bytes, a))) return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  BwdArgs a;
-  a.delta = static_cast<const float*>(workspace);
-  a.lse2 = reinterpret_cast<const float*>(static_cast<const uint8_t*>(workspace) + bwd_section(rows));
-  a.dst[0] = a.dst[1] = nullptr;
-  a.D = int(D);
-  if (scale <= 0.f) scale = 1.0f / sqrtf(float(D));
-  a.scale = scale;
-  a.scale_log2 = scale * 1.4426950408889634f;
-  auto run = [&](auto dt, auto dp) {
-    return run_bwd_varlen<decltype(dt)::value, decltype(dp)::value>(
-        Q, K, V, O, lse, dO, dQ, dK, dV, cu_seqlens_q, cu_seqlens_k, B, max_seqlen_q, max_seqlen_k, total_q, total_k, H,
-        H_kv, D, causal, a, s, di);
-  };
-  using F16 = std::integral_constant<int, 0>;
-  using BF16 = std::integral_constant<int, 1>;
-  using P64 = std::integral_constant<int, 64>;
-  using P128 = std::integral_constant<int, 128>;
-  const bool narrow = D <= 64;
-  if (dtype == B200K_BF16) return narrow ? run(BF16(), P64()) : run(BF16(), P128());
-  return narrow ? run(F16(), P64()) : run(F16(), P128());
+  return run_bwd_cfg(dtype, D, [&](auto cfg) {
+    using KvCfg = decltype(cfg);
+    using QCfg = BwdQCfg<KvCfg>;
+    const BwdPackedGrad gq = {dQ, cu_seqlens_q, total_q, H * D / 2}, gk = {dK, cu_seqlens_k, total_k, H_kv * D / 2},
+                        gv = {dV, cu_seqlens_k, total_k, H_kv * D / 2};
+    attn_bwd_prep_kernel<KvCfg::DT, true><<<bwd_prep_blocks(rows), 256, 0, s>>>(
+        static_cast<const uint16_t*>(O), static_cast<const uint16_t*>(dO), lse, const_cast<float*>(a.delta),
+        const_cast<float*>(a.lse2), rows, int(D), int(B), gq, gk, gv);
+    B200K_CHECK_CUDA(cudaGetLastError());
+    const AttnTensor kv_t[4] = {{K, total_k, H_kv, D, 64, 1}, {V, total_k, H_kv, D, 64, 1}, {Q, total_q, H, D, 64, 1},
+                                {dO, total_q, H, D, 64, 1}};
+    const AttnTensor q_t[2] = {{Q, total_q, H, D, QCfg::BM, 1}, {dO, total_q, H, D, QCfg::BM, 1}};
+    const BwdKeysPacked<KvCfg> km = {cu_seqlens_q, cu_seqlens_k, int(H), int(H_kv), int(H / H_kv), causal ? 1 : 0};
+    const AttnPacked<QCfg> qm = {cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
+    return bwd_main<KvCfg>(fn, kv_t, q_t, km, dim3(unsigned((max_seqlen_k + 63) / 64), unsigned(B * H_kv)), qm,
+                           dim3(unsigned((max_seqlen_q + QCfg::BM - 1) / QCfg::BM), 1, unsigned(B * H)), a, dQ, dK, dV,
+                           s, di);
+  });
 }

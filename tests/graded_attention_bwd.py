@@ -320,7 +320,7 @@ def emulate_bwd(q, k, v, o, lse, do, scale, causal, seqlens, mut=""):
     2^-126; dS = P (dP - Delta); P~, dS~ rounded to the dtype (pack_round); the sums, exact (closed_form asserts the
     window), then the stores: dQ, dK times fp32(scale), dV as is.  `mut` is one of MUTATIONS or "":
       ds_trunc, p_trunc        dS~ / P~ rounded toward zero
-      delta_swap, lse2_swap    Delta / lse2 of the thread's other row, r ^ 8 (load_row_stats' 0 / +inf past N)
+      delta_swap, lse2_swap    Delta / lse2 of the thread's other row, r ^ 8 (the row statistics' 0 / +inf past N)
       causal_diag, causal_next the causal mask key >= row, key > row + 1
       len_short, len_long      the length mask one key short, one key long
       scale_dv                 dV stored times scale;  dk_unscaled, dq_unscaled: dK / dQ stored without it

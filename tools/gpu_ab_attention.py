@@ -7,11 +7,13 @@ see the same arguments.
   1. Seeded random inputs through both builds; every output (and, for append, both caches) must have the same bits:
      dense f16 / bf16 at D 32 - 128 (causal, key padding, ragged N), V stored [B,H,D,N], FFPA at D 160 - 1024, packed
      GQA / MQA with empty sequences, decode on contiguous caches and pages of 16 / 64 / 256 at one split and at many
-     (G = 72 among them: two 64-row head tiles), and append with and without rotary.
+     (G = 72 among them: two 64-row head tiles), and append with and without rotary; the backward's dQ, dK and dV,
+     dense f16 / bf16 at D 64 and 128 (causal, key padding, ragged N) and packed GQA with empty sequences and Lq != Lk.
   2. Time per call of each build, alternating, one CUDA graph of `iters` calls per build per round: bench.py's
      attention shapes (dense (4, 48, 8192, 64) and (4, 64, 8192, 128), FFPA (1, 32, 4096, 512)), packed GQA (4 x 8192
-     tokens, H 64, H_kv 8, D 128, causal) and decode against an 8K cache at B 1 and 64.  Each line gives the median
-     and min - max of both builds and whether the new median lies inside the base's min - max.
+     tokens, H 64, H_kv 8, D 128, causal) and decode against an 8K cache at B 1 and 64; the backward at the dense
+     shapes and the packed GQA one, causal and not.  Each line gives the median and min - max of both builds and
+     whether the new median lies inside the base's min - max.
 
 The first line names the GPU, its power limit and its maximum SM clock, read in the same run.
 
@@ -179,6 +181,37 @@ def equal_cases(torch, ops):
                     ops.fa2_fwd_kvcache(q, kc, vc, o, lens, table, causal=True, k=kn, v=vn, **rot)
                     return [o, kc, vc]
                 cases.append(("append %s rotary=%s B=%d H_kv=%d" % (kind, rotary, B, H_kv), run))
+
+    # backward: o and lse from the in-tree forward, so both builds take the same inputs
+    for dt in (torch.float16, torch.bfloat16):
+        for D in (64, 128):
+            for causal in (False, True):
+                for pad in (False, True):
+                    torch.manual_seed(20 + D + 2 * causal + 4 * pad)
+                    B, H, N = 3, 4, 1000
+                    q, k, v, do = [rn(B, H, N, D, dt=dt) for _ in range(4)]
+                    sl = i32([1, 129, 700]) if pad else None
+                    o, lse = torch.empty_like(q), torch.empty(B, H, N, device=dev)
+                    ops.fa2_fwd(q, k, v, o, causal=causal, seqlens_k=sl, lse=lse)
+
+                    def run(q=q, k=k, v=v, o=o, lse=lse, do=do, sl=sl, causal=causal):
+                        g = [torch.full_like(t, float("nan")) for t in (q, k, v)]
+                        ops.fa2_bwd(q, k, v, o, lse, do, *g, causal=causal, seqlens_k=sl)
+                        return g
+                    cases.append(("bwd dense %s D=%d causal=%d pad=%d" % (str(dt)[6:], D, causal, pad), run))
+            for H_kv in (4, 1):
+                for causal in (False, True):
+                    torch.manual_seed(30 + D + H_kv + causal)
+                    q, do = rn(sum(lq), 16, D, dt=dt), rn(sum(lq), 16, D, dt=dt)
+                    k, v = rn(sum(lk), H_kv, D, dt=dt), rn(sum(lk), H_kv, D, dt=dt)
+                    o, lse = torch.empty_like(q), torch.empty(sum(lq), 16, device=dev)
+                    ops.fa2_fwd_varlen(q, k, v, o, cq, ck, max(lq), causal=causal, lse=lse)
+
+                    def run(q=q, k=k, v=v, o=o, lse=lse, do=do, causal=causal):
+                        g = [torch.full_like(t, float("nan")) for t in (q, k, v)]
+                        ops.fa2_bwd_varlen(q, k, v, o, lse, do, *g, cq, ck, max(lq), max(lk), causal=causal)
+                        return g
+                    cases.append(("bwd packed %s D=%d H=16 H_kv=%d causal=%d" % (str(dt)[6:], D, H_kv, causal), run))
     return cases
 
 
@@ -210,6 +243,28 @@ def timed_cases(torch, ops):
         lens = torch.full((B,), S, dtype=torch.int32, device=dev)
         cases.append(("decode B %d Lq 1 H 32 H_kv 8 D 128, 8K cache" % B, 4.0 * B * Lq * H * S * D,
                       lambda q=q, kc=kc, vc=vc, o=o, lens=lens: ops.fa2_fwd_kvcache(q, kc, vc, o, lens)))
+    # the backward's work counted as flash-attn does: 2.5 times the forward's (5 products), half of it when causal
+    for causal in (False, True):
+        for B, H, N, D in ((4, 48, 8192, 64), (4, 64, 8192, 128)):
+            q, k, v, do = [torch.randn(B, H, N, D, dtype=torch.half, device=dev) for _ in range(4)]
+            o, lse = torch.empty_like(q), torch.empty(B, H, N, device=dev)
+            ops.fa2_fwd(q, k, v, o, causal=causal, lse=lse)
+            g = [torch.empty_like(q) for _ in range(3)]
+            cases.append(("bwd dense (%d, %d, %d, %d)%s" % (B, H, N, D, " causal" if causal else ""),
+                          10.0 * B * H * N * N * D / (2 if causal else 1),
+                          lambda q=q, k=k, v=v, o=o, lse=lse, do=do, g=g, causal=causal:
+                          ops.fa2_bwd(q, k, v, o, lse, do, *g, causal=causal)))
+        B, N, H, H_kv, D = 4, 8192, 64, 8, 128
+        q, do = [torch.randn(B * N, H, D, dtype=torch.half, device=dev) for _ in range(2)]
+        k, v = [torch.randn(B * N, H_kv, D, dtype=torch.half, device=dev) for _ in range(2)]
+        o, lse = torch.empty_like(q), torch.empty(B * N, H, device=dev)
+        cu = torch.arange(0, (B + 1) * N, N, dtype=torch.int32, device=dev)
+        ops.fa2_fwd_varlen(q, k, v, o, cu, cu, N, causal=causal, lse=lse)
+        g = [torch.empty_like(t) for t in (q, k, v)]
+        cases.append(("bwd packed GQA 4 x 8192 H 64 H_kv 8 D 128%s" % (" causal" if causal else ""),
+                      10.0 * B * H * N * N * D / (2 if causal else 1),
+                      lambda q=q, k=k, v=v, o=o, lse=lse, do=do, g=g, cu=cu, causal=causal:
+                      ops.fa2_bwd_varlen(q, k, v, o, lse, do, *g, cu, cu, N, N, causal=causal)))
     return cases
 
 
