@@ -205,17 +205,29 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
 
 
 def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
-                   scale: Optional[float] = None, causal: bool = False, lse: Optional[torch.Tensor] = None) -> None:
+                   scale: Optional[float] = None, causal: bool = False, lse: Optional[torch.Tensor] = None, *,
+                   block_table: Optional[torch.Tensor] = None) -> None:
     """FA-2 forward on packed variable-length sequences (the forward of flash-attn's ``flash_attn_varlen_func``).
     q, o [total_q, H, D]; k, v [total_k, H_kv, D] with H % H_kv == 0 (query head h reads K/V head h // (H // H_kv));
     fp16 or bf16.  ``cu_seqlens_q`` / ``cu_seqlens_k``: int32 [B + 1] cumulative token offsets on the device.
     ``max_seqlen_q`` (a Python int, >= every query length) sizes the grid, so nothing is read back to the host.
     ``causal`` is aligned bottom-right (row r sees keys <= r + Lk - Lq); rows that see no key are 0.
     ``lse``: an fp32 [total_q, H] tensor that receives each row's softmax log-sum-exp (-inf for a row that sees no key);
-    tokens outside every sequence are left untouched, like o."""
+    tokens outside every sequence are left untouched, like o.
+
+    Paged K/V (prefill after a cached prefix, chunked prefill, prompts of mixed lengths): with an int32
+    ``block_table`` [B, pages_per_seq], k and v are caches [num_pages, page_size, H_kv, D] and key j of sequence b is
+    slot j % page_size of page block_table[b, j // page_size], as in flash-attn.  Sequence b then has
+    Lk = cu_seqlens_k[b + 1] - cu_seqlens_k[b] keys, clamped to [0, pages_per_seq * page_size]; page_size is 16, 32, 64
+    or a multiple of 128.  Cache slots past Lk and pages the table row does not list never affect o or lse, whatever
+    they hold.  o and lse have the bits of the call without a table on k / v gathered through it.  Each query tile is
+    128 rows, so for decode (one query token per sequence) :func:`fa2_fwd_kvcache` is the call to use."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     for t in (q, k, v, o):
         _check_dtype(t, dt)
+    if block_table is not None:
+        _fa2_fwd_varlen_paged(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse, block_table, dt)
+        return
     if q.dim() != 3 or k.dim() != 3:
         raise RuntimeError("Tensor size mismatch!")
     total_q, H, D = q.shape
@@ -245,6 +257,39 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
         L.check(_lib.b200k_fa2_fwd_varlen(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), cu_seqlens_q.data_ptr(),
                                           cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
                                           float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+
+
+def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
+                          block_table, dt) -> None:
+    """:func:`fa2_fwd_varlen` with ``block_table``: the shape checks of the paged layout, then the C call."""
+    if q.dim() != 3 or k_cache.dim() != 4:
+        raise RuntimeError("Tensor size mismatch!")
+    total_q, H, D = q.shape
+    num_pages, page_size, H_kv = k_cache.size(0), k_cache.size(1), k_cache.size(2)
+    if (tuple(k_cache.shape) != (num_pages, page_size, H_kv, D) or tuple(v_cache.shape) != tuple(k_cache.shape)
+            or tuple(o.shape) != tuple(q.shape)):
+        raise RuntimeError("Tensor size mismatch!")
+    if H_kv < 1 or H % H_kv:
+        raise RuntimeError("Tensor size mismatch!")
+    if D not in FA2_HEADDIMS:
+        raise RuntimeError("headdim not support!")
+    _check_dtype(cu_seqlens_q, torch.int32)
+    _check_dtype(cu_seqlens_k, torch.int32)
+    _check_dtype(block_table, torch.int32)
+    B = cu_seqlens_q.numel() - 1
+    if B < 1 or cu_seqlens_k.numel() != B + 1 or block_table.dim() != 2 or block_table.size(0) != B:
+        raise RuntimeError("Tensor size mismatch!")
+    if not block_table.is_contiguous():  # the kernel reads row b at b * pages_per_seq
+        raise RuntimeError("b200k: tensors must be contiguous")
+    if lse is not None:
+        _check_lse(lse, o)
+    _check_cuda_contig(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, block_table)
+    with _DeviceGuard(q):
+        L.check(_lib.b200k_fa2_varlen_paged(
+            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
+            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr(), B, int(max_seqlen_q), total_q, H,
+            H_kv, D, num_pages, page_size, block_table.size(1), float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
+            1 if causal else 0, _stream(q)))
 
 
 def fa2_fwd_kvcache_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int) -> int:

@@ -35,16 +35,84 @@ __device__ __forceinline__ float2 unpack2(uint32_t w) {
 // first row q0 (its rows are q0 .. q0 + BM - 1 in the numbering diag and store take), which setup fills (false: no rows
 // here; the CTA returns before any barrier exists); tiles, the KV tiles it visits; q_bytes and load_q, the bytes and the
 // box of 64-column chunk c of Q; kv_tile, where KV tile j is, for load_k (chunk c of K) and load_v (all of V); diag,
-// the causal diagonal (last key seen) of row r; zero_v_tail, which only decode fills in; out_row, whether row r is
-// stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.  The dense and packed modes, AttnDense
-// and AttnPacked, are in attn_common.cuh, which the backward shares.
+// the causal diagonal (last key seen) of row r; zero_v_tail, which only the paged modes fill in; out_row, whether row r
+// is stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.  The dense and packed modes,
+// AttnDense and AttnPacked, are in attn_common.cuh, which the backward shares.
 
-// KV-cache decode.  Q / O are [B, Lq, H, D]; the caches are [num_pages, page_size, H_kv, D], key j of sequence b at
-// slot j % page_size of page table[b * pages_per_seq + j / page_size] (table null: contiguous cache, sequence b at rows
-// [b * page_size, ...)).  CTA (x, y, z) = (split, token tile * nhb + head tile, b * H_kv + K/V head).  Its 64 rows are
-// T tokens x hb heads of one group (row r = token r / hb, head r % hb); row r of token t sees keys <= t + Lk - Lq under
-// the causal mask.  With more than one split (gridDim.x) the CTA writes O / l and the row's base-2 log-sum-exp to
-// `part` / `lse` ([split][row][D], [split][row], row = (b * Lq + t) * H + h) instead of O.
+// K / V read from caches [num_pages, page_size, H_kv, D] through a block table, for the modes that do (AttnDecode,
+// AttnPackedPaged).  Key j of sequence seq is at slot j % page_size of page table[seq * pages_per_seq + j / page_size]
+// (table null: contiguous cache, sequence seq at rows [seq * page_size, ...)).  A KV tile is BN / box_rows TMA boxes,
+// one per page when pages are smaller than a tile.  M is the mode, which holds table, page_size, pages_per_seq,
+// box_rows and oob (a row coordinate past the end of the cache maps: TMA zero-fills the box); kv_len is the sequence's
+// key count, already clamped to its capacity pages_per_seq * page_size.
+template <class Cfg>
+struct PagedKv {
+  // cache row of each box of a KV tile
+  struct Rows { int row[Cfg::BN / 16]; };
+  // A box past the sequence's last page reads outside the map, so the table is read only up to the length.
+  template <class M>
+  __device__ __forceinline__ static Rows tile(const M& m, int seq, int kv_len, int j) {
+    Rows t;
+#pragma unroll
+    for (int i = 0; i < Cfg::BN / 16; ++i) {
+      const int key = j * Cfg::BN + i * m.box_rows;
+      if (i * m.box_rows >= Cfg::BN) break;
+      if (!m.table) t.row[i] = seq * m.page_size + key;
+      else if (key >= kv_len) t.row[i] = m.oob;
+      else t.row[i] = __ldg(m.table + size_t(seq) * m.pages_per_seq + key / m.page_size) * m.page_size + key % m.page_size;
+    }
+    return t;
+  }
+  template <class M>
+  __device__ __forceinline__ static void load_k(const M& m, int kvh, const Rows& t, uint32_t dst, const CUtensorMap* tm,
+                                                uint32_t bar, int chunk) {
+#pragma unroll
+    for (int i = 0; i < Cfg::BN / 16; ++i) {
+      if (i * m.box_rows >= Cfg::BN) break;
+      tma_load_3d(dst + i * m.box_rows * 128, tm, bar, chunk * 64, kvh, t.row[i], kPolicyEvictNormal);
+    }
+  }
+  template <class M>
+  __device__ __forceinline__ static void load_v(const M& m, int kvh, const Rows& t, uint32_t dst, const CUtensorMap* tm,
+                                                uint32_t bar) {
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(m, kvh, t, dst + i * Cfg::BN * 128, tm, bar, i);
+  }
+  // The tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or Inf in
+  // V is NaN in the tensor core, so those V rows are zeroed (K needs nothing: its scores became -inf).  Every consumer
+  // warpgroup waits on the same V stage, so all 128 * NWG consumer threads share the stores and meet at one barrier
+  // before any of them issues its wgmma.  Each reaches it in the same iteration: the condition is the CTA's.
+  __device__ __forceinline__ static void zero_v_tail(int kv_len, int k0, uint32_t vb) {
+    constexpr int N = 128 * Cfg::NWG;
+    if (k0 + Cfg::BN <= kv_len) return;
+    const int r0 = kv_len - k0, words = (Cfg::BN - r0) * 8;  // 16-byte words per 64-column chunk
+    auto zero = [&](int i, int w) {
+      asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + i * Cfg::BN * 128 + r0 * 128 + w * 16), "r"(0)
+                   : "memory");
+    };
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) {
+      if constexpr (Cfg::NWG == 1) {
+        for (int w = threadIdx.x % N; w < words; w += N) zero(i, w);
+      } else {
+        // Two consumer warpgroups already hold 168 registers, the most a 384-thread CTA allows; a fixed count of
+        // predicated stores needs fewer live registers than the loop above, which would spill.
+        static_assert(Cfg::BN * 8 % N == 0, "zero_v_tail: every 16-byte word of a chunk needs a thread");
+#pragma unroll
+        for (int k = 0; k < Cfg::BN * 8 / N; ++k)
+          if (threadIdx.x % N + k * N < words) zero(i, threadIdx.x % N + k * N);
+      }
+    }
+    fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
+    named_bar_sync(1, N);
+  }
+};
+
+// KV-cache decode.  Q / O are [B, Lq, H, D]; the caches are paged as PagedKv describes.  CTA (x, y, z) = (split, token
+// tile * nhb + head tile, b * H_kv + K/V head).  Its 64 rows are T tokens x hb heads of one group (row r = token r / hb,
+// head r % hb); row r of token t sees keys <= t + Lk - Lq under the causal mask.  With more than one split (gridDim.x)
+// the CTA writes O / l and the row's base-2 log-sum-exp to `part` / `lse` ([split][row][D], [split][row], row =
+// (b * Lq + t) * H + h) instead of O.
 template <class Cfg>
 struct AttnDecode {
   static_assert(Cfg::NWG == 1 && !Cfg::V_DN, "decode: one consumer warpgroup, V [keys, heads, D]");
@@ -54,11 +122,10 @@ struct AttnDecode {
   int H = 1, causal = 0;
   int Lq = 1, group = 1, hb = 1, T = 1, nhb = 1;
   int page_size = 1, pages_per_seq = 1, box_rows = 1;
-  int oob = 0;  // a row coordinate past the end of the cache maps: TMA zero-fills the box
+  int oob = 0;
 
   struct Cta { int q0, seq, kvh, t0, h0, kv_len, shift; };  // q0 = 0; t0, h0: first token and head; shift: Lk - Lq
-  // cache row of each box of a KV tile: BN / box_rows boxes, one per page when pages are smaller than a tile
-  struct KvRows { int row[Cfg::BN / 16]; };
+  using KvRows = typename PagedKv<Cfg>::Rows;
   __device__ __forceinline__ bool setup(Cta& c) const {
     const int h_kv = H / group;
     c.q0 = 0;
@@ -85,45 +152,20 @@ struct AttnDecode {
   __device__ __forceinline__ void load_q(const Cta& c, uint32_t dst, const CUtensorMap* tm, uint32_t bar, int chunk) const {
     tma_load_3d(dst, tm, bar, chunk * 64, c.h0, c.seq * Lq + c.t0, kPolicyEvictFirst);
   }
-  // A box past the sequence's last page reads outside the map, so the table is read only up to the length.
   __device__ __forceinline__ KvRows kv_tile(const Cta& c, int j) const {
-    KvRows t;
-#pragma unroll
-    for (int i = 0; i < Cfg::BN / 16; ++i) {
-      const int key = j * Cfg::BN + i * box_rows;
-      if (i * box_rows >= Cfg::BN) break;
-      if (!table) t.row[i] = c.seq * page_size + key;
-      else if (key >= c.kv_len) t.row[i] = oob;
-      else t.row[i] = __ldg(table + size_t(c.seq) * pages_per_seq + key / page_size) * page_size + key % page_size;
-    }
-    return t;
+    return PagedKv<Cfg>::tile(*this, c.seq, c.kv_len, j);
   }
   __device__ __forceinline__ void load_k(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
                                          int chunk) const {
-#pragma unroll
-    for (int i = 0; i < Cfg::BN / 16; ++i) {
-      if (i * box_rows >= Cfg::BN) break;
-      tma_load_3d(dst + i * box_rows * 128, tm, bar, chunk * 64, c.kvh, t.row[i], kPolicyEvictNormal);
-    }
+    PagedKv<Cfg>::load_k(*this, c.kvh, t, dst, tm, bar, chunk);
   }
   __device__ __forceinline__ void load_v(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm,
                                          uint32_t bar) const {
-#pragma unroll
-    for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, t, dst + i * Cfg::BN * 128, tm, bar, i);
+    PagedKv<Cfg>::load_v(*this, c.kvh, t, dst, tm, bar);
   }
   __device__ __forceinline__ int diag(const Cta& c, int r) const { return c.t0 + r / hb + c.shift; }
-  // The tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or Inf in
-  // V is NaN in the tensor core, so those V rows are zeroed (K needs nothing: its scores became -inf).
   __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
-    if (k0 + Cfg::BN <= c.kv_len) return;
-    const int r0 = c.kv_len - k0, words = (Cfg::BN - r0) * 8;  // 16-byte words per 64-column chunk
-#pragma unroll
-    for (int i = 0; i < Cfg::DV / 64; ++i)
-      for (int w = threadIdx.x & 127; w < words; w += 128)
-        asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + i * Cfg::BN * 128 + r0 * 128 + w * 16), "r"(0)
-                     : "memory");
-    fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
-    named_bar_sync(1, 128);
+    PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
   }
   // rows past the box, the sequence or the group are not stored
   __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
@@ -147,6 +189,39 @@ struct AttnDecode {
       *reinterpret_cast<float2*>(dst + col) = make_float2(o[4 * i + 2 * h] * inv, o[4 * i + 2 * h + 1] * inv);
     }
     if ((lane & 3) == 0) lse[size_t(blockIdx.x) * size_t(rows) + row] = l > 0.f ? m + log2f(l) : -INFINITY;
+  }
+};
+
+// Packed queries over paged caches.  Q / O, the grid, the causal diagonals and the stores are AttnPacked's; K / V are
+// read through the block table as PagedKv describes.  Sequence b has Lk = cu_k[b + 1] - cu_k[b] keys, clamped to
+// [0, pages_per_seq * page_size] (cu_k gives lengths only, no cache position).
+template <class Cfg>
+struct AttnPackedPaged : AttnPacked<Cfg> {
+  const int* table;
+  int page_size, pages_per_seq, box_rows, oob;
+
+  using Cta = typename AttnPacked<Cfg>::Cta;
+  using KvRows = typename PagedKv<Cfg>::Rows;
+  __device__ __forceinline__ bool setup(Cta& c) const {
+    if (!AttnPacked<Cfg>::setup(c)) return false;
+    const int q_len = c.kv_len - c.shift;
+    c.kv_len = min(max(c.kv_len, 0), pages_per_seq * page_size);
+    c.shift = c.kv_len - q_len;
+    return true;
+  }
+  __device__ __forceinline__ KvRows kv_tile(const Cta& c, int j) const {
+    return PagedKv<Cfg>::tile(*this, blockIdx.z / this->H, c.kv_len, j);
+  }
+  __device__ __forceinline__ void load_k(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm, uint32_t bar,
+                                         int chunk) const {
+    PagedKv<Cfg>::load_k(*this, c.kv_head, t, dst, tm, bar, chunk);
+  }
+  __device__ __forceinline__ void load_v(const Cta& c, const KvRows& t, uint32_t dst, const CUtensorMap* tm,
+                                         uint32_t bar) const {
+    PagedKv<Cfg>::load_v(*this, c.kv_head, t, dst, tm, bar);
+  }
+  __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
+    PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
   }
 };
 
@@ -606,6 +681,24 @@ static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64
   return B200K_OK;
 }
 
+// Page counts of a cache read through a block table, or of a contiguous one: cache rows and a sequence's capacity
+// are int32.
+static int check_page_counts(const char* fn, int64_t num_pages, int64_t page_size, int64_t pages_per_seq) {
+  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
+    return set_error(B200K_ESHAPE, "%s: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)", fn,
+                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
+  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
+    return set_error(B200K_ESHAPE, "%s: num_pages * page_size and pages_per_seq * page_size must be <= 2^31 - 1", fn);
+  return B200K_OK;
+}
+
+// The pages a block table can name: a KV tile of 128 keys is one TMA box inside one page, or a whole number of pages.
+static int check_page_size(const char* fn, int64_t page_size) {
+  if (page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
+    return set_error(B200K_ESHAPE, "%s: page_size %lld (16, 32, 64 or a multiple of 128)", fn, (long long)page_size);
+  return B200K_OK;
+}
+
 // Argument checks of b200k_fa2_fwd_kvcache, which b200k_fa2_fwd_kvcache_append shares (before any CUDA call).
 static int kvcache_args(const char* fn, const void* Q, const void* K_cache, const void* V_cache, const void* O,
                         const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv,
@@ -614,15 +707,9 @@ static int kvcache_args(const char* fn, const void* Q, const void* K_cache, cons
   if (dtype != B200K_F16 && dtype != B200K_BF16)
     return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
   int rc = check_headdim(fn, D);
-  if (rc) return rc;
-  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
-    return set_error(B200K_ESHAPE, "%s: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)", fn,
-                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
-  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
-    return set_error(B200K_ESHAPE, "%s: num_pages * page_size and pages_per_seq * page_size must be <= 2^31 - 1", fn);
+  if (rc || (rc = check_page_counts(fn, num_pages, page_size, pages_per_seq))) return rc;
   if ((rc = kvcache_check(fn, B, Lq, H, H_kv, pages_per_seq * page_size))) return rc;
-  if (block_table && page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
-    return set_error(B200K_ESHAPE, "%s: page_size %lld (16, 32, 64 or a multiple of 128)", fn, (long long)page_size);
+  if (block_table && (rc = check_page_size(fn, page_size))) return rc;
   if (!block_table && (num_pages != B || pages_per_seq != 1))
     return set_error(B200K_ESHAPE, "%s: a contiguous cache (no block table) is num_pages = B pages of page_size = S keys, "
                      "pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)", fn, (long long)num_pages,
@@ -814,6 +901,51 @@ extern "C" int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void
     const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1}, {K, total_k, H_kv, D, Cfg::BN, 1}, {V, total_k, H_kv, D, Cfg::BN, 1}};
     const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
     const AttnPacked<Cfg> args = {cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0};
+    return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
+  });
+}
+
+extern "C" int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                                      const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
+                                      int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv,
+                                      int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                      float scale, int dtype, int causal, void* stream) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_varlen_paged";
+  if (!Q || !K_cache || !V_cache || !O || !cu_seqlens_q || !cu_seqlens_k || !block_table)
+    return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (dtype != B200K_F16 && dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
+  int rc = check_headdim(fn, D);
+  if (rc) return rc;
+  if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
+    return set_error(B200K_ESHAPE, "%s: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)", fn,
+                     (long long)B, (long long)H, (long long)H_kv);
+  if ((rc = check_page_counts(fn, num_pages, page_size, pages_per_seq)) || (rc = check_page_size(fn, page_size)))
+    return rc;
+  if (total_q < 1 || total_q > INT32_MAX || max_seqlen_q < 1 || max_seqlen_q > total_q)
+    return set_error(B200K_ESHAPE, "%s: need 1 <= total_q <= 2^31 - 1 and 1 <= max_seqlen_q <= total_q (got total_q=%lld "
+                     "max_seqlen_q=%lld)", fn, (long long)total_q, (long long)max_seqlen_q);
+  if (B > 65535 || H > 65535 || B * H > 65535)
+    return set_error(B200K_ESHAPE, "%s: B * H = %lld CTAs per query tile, the grid allows 65535", fn,
+                     (long long)B * (long long)H);
+  if ((rc = check_align(fn, {{Q, "Q", 16}, {K_cache, "K_cache", 16}, {V_cache, "V_cache", 16}, {O, "O", 4}, {lse, "lse", 4},
+                             {cu_seqlens_q, "cu_seqlens_q", 4}, {cu_seqlens_k, "cu_seqlens_k", 4},
+                             {block_table, "block_table", 4}})))
+    return rc;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  return run_attn_cfg<2, false>(dtype, D, [&](auto cfg) {
+    using Cfg = decltype(cfg);
+    const int box_rows = page_size < Cfg::BN ? int(page_size) : Cfg::BN;
+    const int64_t cache_rows = num_pages * page_size;
+    const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1},
+                               {K_cache, cache_rows, H_kv, D, box_rows, 1},
+                               {V_cache, cache_rows, H_kv, D, box_rows, 1}};
+    const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
+    const AttnPackedPaged<Cfg> args = {{cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0},
+                                       block_table, int(page_size), int(pages_per_seq), box_rows, int(cache_rows)};
     return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
   });
 }

@@ -255,6 +255,36 @@ int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, void* V_cache
                                      int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
                                      float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
                                      void* stream);
+/* b200k_fa2_varlen_paged — b200k_fa2_fwd_varlen with K / V read from paged caches through a block table (flash-attn's
+ * flash_attn_varlen_func with block_table): prefill of a prompt chunk after a cached prefix, chunked prefill, or a batch
+ * of prompts of different lengths, without gathering the cached keys into a contiguous buffer.  The same kernel as the
+ * packed call, 128 query rows per CTA, with the block-table addressing of b200k_fa2_fwd_kvcache:
+ *   Q, O, lse      as b200k_fa2_fwd_varlen_lse: Q, O [total_q, H, D], sequence b is query tokens
+ *                  [cu_seqlens_q[b], cu_seqlens_q[b+1]); lse NULL or fp32 [total_q, H].  Stores are clipped to tokens
+ *                  [0, total_q), and tokens outside every sequence are left untouched
+ *   K_cache, V_cache [num_pages, page_size, H_kv, D] contiguous, Q's dtype; H % H_kv == 0
+ *   block_table    int32 device array [B, pages_per_seq] (required): key j of sequence b is slot j % page_size of page
+ *                  block_table[b * pages_per_seq + j / page_size]; page_size is 16, 32, 64 or a multiple of 128.
+ *                  Entries past ceil(Lk_b / page_size) are never read
+ *   cu_seqlens_k   int32 device array [B + 1]: sequence b has Lk_b = cu_seqlens_k[b+1] - cu_seqlens_k[b] keys, clamped to
+ *                  [0, pages_per_seq * page_size].  Only the differences are used
+ *   causal         bottom-right as b200k_fa2_fwd_varlen: query row r sees key j iff j <= r + Lk_b - Lq_b
+ *   isolation      cache slots at or past Lk_b, and pages the sequence's table row does not list, never affect O or lse,
+ *                  whatever they hold (NaN and Inf included)
+ *   bits           O and lse have the bits b200k_fa2_fwd_varlen_lse gives on K / V gathered through the table
+ *   no sync        max_seqlen_q sizes the grid; nothing is read back to the host, so the call can be captured in a CUDA
+ *                  graph and replayed while cu_seqlens and block_table change.  A decode step (Lq = 1) still takes a CTA
+ *                  of 128 rows per query head: b200k_fa2_fwd_kvcache is the decode call
+ *   alignment      Q, K_cache, V_cache 16 bytes; O, lse, cu_seqlens_q, cu_seqlens_k, block_table 4 bytes
+ * Errors before any CUDA call: B200K_EARG for a null pointer (lse may be NULL), B200K_EDTYPE, B200K_EHEADDIM,
+ * B200K_ESHAPE unless B, H, H_kv >= 1, H % H_kv == 0, num_pages, page_size, pages_per_seq >= 1 with num_pages * page_size
+ * and pages_per_seq * page_size <= INT32_MAX, page_size as above, 1 <= max_seqlen_q <= total_q <= INT32_MAX and
+ * B * H <= 65535; then B200K_EALIGN. */
+int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                           const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table, int64_t B,
+                           int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D,
+                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype,
+                           int causal, void* stream);
 /* b200k_attn_merge — the attention over the union of S disjoint key sets from the attention over each (cascade /
  * shared-prefix decode, chunked prefill, keys sharded across devices):
  *   inputs      O_parts [S, rows, D] in dtype (B200K_F16 or B200K_BF16), lse_parts [S, rows] fp32 natural log, as the
