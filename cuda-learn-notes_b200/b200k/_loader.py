@@ -75,6 +75,11 @@ _SIGS = {
     "b200k_fa2_fwd_kvcache_append_lse": (c_int, [c_void_p] * 9 + [c_int64] + [c_void_p] * 2 + [c_int64] * 2 + [c_int]
                                          + [c_int64] * 8 + [c_float, c_int, c_int, c_void_p, c_size_t, c_void_p]),
     "b200k_fa2_varlen_paged": (c_int, [c_void_p] * 8 + [c_int64] * 9 + [c_float, c_int, c_int, c_void_p]),
+    "b200k_fa2_kvcache_fp8": (c_int, [c_void_p] * 9 + [c_int] + [c_void_p] * 2 + [c_int64] + [c_void_p] * 2
+                              + [c_int64] * 2 + [c_int] + [c_int64] * 8 + [c_float, c_int, c_int, c_void_p, c_size_t,
+                                                                         c_void_p]),
+    "b200k_fa2_kvcache_fp8_workspace_bytes": (c_int, [c_int64] * 6 + [c_int, c_int, ctypes.POINTER(c_size_t)]),
+    "b200k_fa2_varlen_paged_fp8": (c_int, [c_void_p] * 10 + [c_int] + [c_int64] * 9 + [c_float, c_int, c_int, c_void_p]),
     "b200k_attn_merge": (c_int, [c_void_p] * 4 + [c_int64] * 3 + [c_int, c_void_p]),
     "b200k_fa2_bwd": (c_int, [c_void_p] * 9 + [c_int64] * 4 + [c_float, c_int, c_int, c_void_p, c_void_p, c_size_t,
                                                                c_void_p]),

@@ -206,7 +206,8 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
 
 def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.Tensor, max_seqlen_q: int,
                    scale: Optional[float] = None, causal: bool = False, lse: Optional[torch.Tensor] = None, *,
-                   block_table: Optional[torch.Tensor] = None) -> None:
+                   block_table: Optional[torch.Tensor] = None, k_scale: Optional[torch.Tensor] = None,
+                   v_scale: Optional[torch.Tensor] = None) -> None:
     """FA-2 forward on packed variable-length sequences (the forward of flash-attn's ``flash_attn_varlen_func``).
     q, o [total_q, H, D]; k, v [total_k, H_kv, D] with H % H_kv == 0 (query head h reads K/V head h // (H // H_kv));
     fp16 or bf16.  ``cu_seqlens_q`` / ``cu_seqlens_k``: int32 [B + 1] cumulative token offsets on the device.
@@ -221,7 +222,17 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
     Lk = cu_seqlens_k[b + 1] - cu_seqlens_k[b] keys, clamped to [0, pages_per_seq * page_size]; page_size is 16, 32, 64
     or a multiple of 128.  Cache slots past Lk and pages the table row does not list never affect o or lse, whatever
     they hold.  o and lse have the bits of the call without a table on k / v gathered through it.  Each query tile is
-    128 rows, so for decode (one query token per sequence) :func:`fa2_fwd_kvcache` is the call to use."""
+    128 rows, so for decode (one query token per sequence) :func:`fa2_fwd_kvcache` is the call to use.
+
+    FP8 pages: with a ``block_table``, k and v may be ``torch.float8_e4m3fn`` or ``torch.float8_e5m2`` caches (one dtype
+    for both), dequantized as fp8 * ``k_scale`` / ``v_scale`` (fp32 [H_kv] device tensors, or None for 1.0); see
+    :func:`fa2_fwd_kvcache`.  o and lse then have the bits of the call on the gathered, dequantized K / V."""
+    if _fp8_kv(k, v, k_scale, v_scale):
+        if block_table is None:
+            raise RuntimeError("b200k: fp8 K / V are read from paged caches: pass block_table")
+        _fa2_fwd_varlen_paged_fp8(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse, block_table,
+                                  k_scale, v_scale)
+        return
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     for t in (q, k, v, o):
         _check_dtype(t, dt)
@@ -259,9 +270,9 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
                                           float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
 
 
-def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
-                          block_table, dt) -> None:
-    """:func:`fa2_fwd_varlen` with ``block_table``: the shape checks of the paged layout, then the C call."""
+def _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, lse, block_table):
+    """The shape checks of :func:`fa2_fwd_varlen` with ``block_table``, for caches of either dtype; returns
+    (B, total_q, H, H_kv, D, num_pages, page_size)."""
     if q.dim() != 3 or k_cache.dim() != 4:
         raise RuntimeError("Tensor size mismatch!")
     total_q, H, D = q.shape
@@ -284,12 +295,76 @@ def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, ma
     if lse is not None:
         _check_lse(lse, o)
     _check_cuda_contig(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, block_table)
+    return B, total_q, H, H_kv, D, num_pages, page_size
+
+
+def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
+                          block_table, dt) -> None:
+    """:func:`fa2_fwd_varlen` with ``block_table``: the shape checks of the paged layout, then the C call."""
+    B, total_q, H, H_kv, D, num_pages, page_size = _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k,
+                                                                 lse, block_table)
     with _DeviceGuard(q):
         L.check(_lib.b200k_fa2_varlen_paged(
             q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
             cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr(), B, int(max_seqlen_q), total_q, H,
             H_kv, D, num_pages, page_size, block_table.size(1), float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
             1 if causal else 0, _stream(q)))
+
+
+_FP8_KV = tuple(d for d in (getattr(torch, "float8_e4m3fn", None), getattr(torch, "float8_e5m2", None)) if d is not None)
+
+
+def _fp8_kv(k_cache, v_cache, k_scale, v_scale) -> bool:
+    """Whether a call reads fp8 caches.  Scales with 16-bit caches and caches of two different dtypes are refused."""
+    fp8 = k_cache.dtype in _FP8_KV or v_cache.dtype in _FP8_KV
+    if fp8 and k_cache.dtype != v_cache.dtype:
+        raise RuntimeError("b200k: k_cache and v_cache must hold the same fp8 dtype (got %s and %s)"
+                           % (k_cache.dtype, v_cache.dtype))
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise RuntimeError("b200k: k_scale / v_scale dequantize fp8 caches; the caches are %s" % k_cache.dtype)
+    return fp8
+
+
+def _fp8_scales(k_scale, v_scale, H_kv: int) -> list:
+    """The scale pointers (None for 1.0) after their checks: fp32 [H_kv], contiguous, on the device."""
+    ptrs = []
+    for t in (k_scale, v_scale):
+        if t is None:
+            ptrs.append(None)
+            continue
+        _check_dtype(t, torch.float32)
+        if t.numel() != H_kv:
+            raise RuntimeError("Tensor size mismatch!")
+        _check_cuda_contig(t)
+        ptrs.append(t.data_ptr())
+    return ptrs
+
+
+def _fa2_fwd_varlen_paged_fp8(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
+                              block_table, k_scale, v_scale) -> None:
+    """:func:`fa2_fwd_varlen` over fp8 pages: the checks of the 16-bit paged call, then b200k_fa2_varlen_paged_fp8."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    _check_dtype(q, dt)
+    _check_dtype(o, dt)
+    B, total_q, H, H_kv, D, num_pages, page_size = _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k,
+                                                                 lse, block_table)
+    ks, vs = _fp8_scales(k_scale, v_scale, H_kv)
+    with _DeviceGuard(q):
+        L.check(_lib.b200k_fa2_varlen_paged_fp8(
+            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
+            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr(), ks, vs, _DTYPE_ENUM[k_cache.dtype],
+            B, int(max_seqlen_q), total_q, H, H_kv, D, num_pages, page_size, block_table.size(1),
+            float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+
+
+def fa2_fwd_kvcache_fp8_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int,
+                                        append: bool = False, rotary: bool = False) -> int:
+    """Workspace bytes :func:`fa2_fwd_kvcache` needs over fp8 caches, with or without ``k`` / ``v``; queries the
+    device."""
+    n = ctypes.c_size_t(0)
+    L.check(_lib.b200k_fa2_kvcache_fp8_workspace_bytes(B, Lq, H, H_kv, D, max_seqlen_k, 1 if append else 0,
+                                                       1 if rotary else 0, ctypes.byref(n)))
+    return n.value
 
 
 def fa2_fwd_kvcache_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int) -> int:
@@ -308,32 +383,12 @@ def fa2_fwd_kvcache_append_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D
     return n.value
 
 
-def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_table: Optional[torch.Tensor] = None,
-                    scale: Optional[float] = None, causal: bool = False, *, k: Optional[torch.Tensor] = None,
-                    v: Optional[torch.Tensor] = None, rotary_cos: Optional[torch.Tensor] = None,
-                    rotary_sin: Optional[torch.Tensor] = None, rotary_interleaved: bool = True,
-                    lse: Optional[torch.Tensor] = None) -> None:
-    """Attention of the newest Lq query tokens of each sequence against its KV cache (flash-attn's
-    ``flash_attn_with_kvcache``).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
-    [B, S, H_kv, D] without ``block_table``, or [num_pages, page_size, H_kv, D] with an int32 ``block_table``
-    [B, pages_per_seq] (key j of sequence b is slot j % page_size of page block_table[b, j // page_size]).
-    ``cache_seqlens``: int32 [B] key counts on the device.  ``causal``: token t sees keys <= t + Lk - Lq.  H % H_kv == 0
-    (query head h reads K/V head h // (H // H_kv)).  Nothing is read back to the host, so the call can be captured in a
-    CUDA graph; the workspace is allocated per call on the current stream.
-
-    Append: ``k``, ``v`` [B, L_new, H_kv, D] are written into the caches in place at positions
-    cache_seqlens[b] + i (through the table when paged), and the attention runs over cache_seqlens[b] + L_new keys.
-    ``cache_seqlens`` itself is not updated; the caller adds L_new afterwards.  ``rotary_cos`` / ``rotary_sin``
-    [rotary_seqlen, rotary_dim / 2] in q's dtype (rotary_dim a multiple of 16, at most D; rotary_seqlen at least the
-    capacity) rotate the first rotary_dim columns of k and q: new key i at position cache_seqlens[b] + i, query token t
-    at cache_seqlens[b] + t when causal and at cache_seqlens[b] when not.  ``rotary_interleaved`` pairs columns
-    (2j, 2j + 1); otherwise (j, j + rotary_dim / 2), GPT-NeoX style.  q is not modified.
-
-    ``lse``: an fp32 [B, Lq, H] tensor that receives each row's softmax log-sum-exp over the keys it sees (-inf for
-    none), with or without ``k`` / ``v``."""
+def _kvcache_checks(q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin, cache_dt):
+    """The checks of :func:`fa2_fwd_kvcache` with caches of dtype cache_dt (q's, or an fp8 one); returns
+    (B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary)."""
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
-    for t in (q, k_cache, v_cache, o):
-        _check_dtype(t, dt)
+    for t, want in ((q, dt), (k_cache, cache_dt), (v_cache, cache_dt), (o, dt)):
+        _check_dtype(t, want)
     if q.dim() != 4 or k_cache.dim() != 4:
         raise RuntimeError("Tensor size mismatch!")
     B, Lq, H, D = q.shape
@@ -362,7 +417,8 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
     if lse is not None:
         _check_lse(lse, o)
     rotary = rotary_cos is not None or rotary_sin is not None
-    if k is not None or v is not None or rotary:
+    append = k is not None or v is not None or rotary
+    if append:
         if k is None or v is None:
             raise RuntimeError("b200k: append needs both k and v (rotary applies to appended keys)")
         if (rotary_cos is None) != (rotary_sin is None):
@@ -372,15 +428,57 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
         if k.dim() != 4 or k.size(0) != B or tuple(k.shape[2:]) != (H_kv, D) or tuple(v.shape) != tuple(k.shape):
             raise RuntimeError("Tensor size mismatch!")
         tensors += [k, v]
-        cos = sin = None
         if rotary:
             _check_dtype(rotary_cos, dt)
             _check_dtype(rotary_sin, dt)
             if rotary_cos.dim() != 2 or tuple(rotary_sin.shape) != tuple(rotary_cos.shape):
                 raise RuntimeError("Tensor size mismatch!")
-            cos, sin = rotary_cos, rotary_sin
-            tensors += [cos, sin]
-        _check_cuda_contig(*tensors)
+            tensors += [rotary_cos, rotary_sin]
+    _check_cuda_contig(*tensors)
+    return B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary
+
+
+def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_table: Optional[torch.Tensor] = None,
+                    scale: Optional[float] = None, causal: bool = False, *, k: Optional[torch.Tensor] = None,
+                    v: Optional[torch.Tensor] = None, rotary_cos: Optional[torch.Tensor] = None,
+                    rotary_sin: Optional[torch.Tensor] = None, rotary_interleaved: bool = True,
+                    lse: Optional[torch.Tensor] = None, k_scale: Optional[torch.Tensor] = None,
+                    v_scale: Optional[torch.Tensor] = None) -> None:
+    """Attention of the newest Lq query tokens of each sequence against its KV cache (flash-attn's
+    ``flash_attn_with_kvcache``).  q, o [B, Lq, H, D], fp16 or bf16.  Caches
+    [B, S, H_kv, D] without ``block_table``, or [num_pages, page_size, H_kv, D] with an int32 ``block_table``
+    [B, pages_per_seq] (key j of sequence b is slot j % page_size of page block_table[b, j // page_size]).
+    ``cache_seqlens``: int32 [B] key counts on the device.  ``causal``: token t sees keys <= t + Lk - Lq.  H % H_kv == 0
+    (query head h reads K/V head h // (H // H_kv)).  Nothing is read back to the host, so the call can be captured in a
+    CUDA graph; the workspace is allocated per call on the current stream.
+
+    Append: ``k``, ``v`` [B, L_new, H_kv, D] are written into the caches in place at positions
+    cache_seqlens[b] + i (through the table when paged), and the attention runs over cache_seqlens[b] + L_new keys.
+    ``cache_seqlens`` itself is not updated; the caller adds L_new afterwards.  ``rotary_cos`` / ``rotary_sin``
+    [rotary_seqlen, rotary_dim / 2] in q's dtype (rotary_dim a multiple of 16, at most D; rotary_seqlen at least the
+    capacity) rotate the first rotary_dim columns of k and q: new key i at position cache_seqlens[b] + i, query token t
+    at cache_seqlens[b] + t when causal and at cache_seqlens[b] when not.  ``rotary_interleaved`` pairs columns
+    (2j, 2j + 1); otherwise (j, j + rotary_dim / 2), GPT-NeoX style.  q is not modified.
+
+    ``lse``: an fp32 [B, Lq, H] tensor that receives each row's softmax log-sum-exp over the keys it sees (-inf for
+    none), with or without ``k`` / ``v``.
+
+    FP8 caches (vLLM's ``kv_cache_dtype="fp8"`` / ``"fp8_e5m2"``): k_cache and v_cache both ``torch.float8_e4m3fn``
+    or both ``torch.float8_e5m2``.  The key of K/V head h is fp8 * ``k_scale[h]`` and its value fp8 * ``v_scale[h]``
+    (fp32 [H_kv] device tensors, or None for 1.0; being tensors, they can change between replays of a captured graph).
+    q, o, ``k`` / ``v`` and cos / sin stay fp16 or bf16; appended rows are stored as
+    satfinite(float(x) / scale[h]) in the cache's format, after rotary.  With no scales, o and lse have the bits of the
+    16-bit call on the dequantized caches; with power-of-two scales too, as long as the dequantized values are normal
+    in q's dtype.  A scale with 16-bit caches, or caches of two dtypes, is a RuntimeError."""
+    if _fp8_kv(k_cache, v_cache, k_scale, v_scale):
+        _fa2_fwd_kvcache_fp8(q, k_cache, v_cache, o, cache_seqlens, block_table, scale, causal, k, v, rotary_cos,
+                             rotary_sin, rotary_interleaved, lse, k_scale, v_scale)
+        return
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary = _kvcache_checks(
+        q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin, dt)
+    if append:
+        cos, sin = rotary_cos, rotary_sin
         with _DeviceGuard(q):
             nbytes = fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, rotary)
             ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
@@ -397,7 +495,6 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
                 L.check(_lib.b200k_fa2_fwd_kvcache_append_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
                                                               o.data_ptr(), lse.data_ptr(), *args))
         return
-    _check_cuda_contig(*tensors)
     with _DeviceGuard(q):
         nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
@@ -409,6 +506,27 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
         else:
             L.check(_lib.b200k_fa2_fwd_kvcache_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
                                                    lse.data_ptr(), *args))
+
+
+def _fa2_fwd_kvcache_fp8(q, k_cache, v_cache, o, cache_seqlens, block_table, scale, causal, k, v, rotary_cos, rotary_sin,
+                         rotary_interleaved, lse, k_scale, v_scale) -> None:
+    """:func:`fa2_fwd_kvcache` over fp8 caches: the 16-bit call's checks, then b200k_fa2_kvcache_fp8."""
+    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
+    B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary = _kvcache_checks(
+        q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin, k_cache.dtype)
+    cos, sin = rotary_cos, rotary_sin
+    ks, vs = _fp8_scales(k_scale, v_scale, H_kv)
+    with _DeviceGuard(q):
+        nbytes = fa2_fwd_kvcache_fp8_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, append, rotary)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
+        L.check(_lib.b200k_fa2_kvcache_fp8(
+            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
+            cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None, ks, vs,
+            _DTYPE_ENUM[k_cache.dtype], k.data_ptr() if append else None, v.data_ptr() if append else None,
+            k.size(1) if append else 0, cos.data_ptr() if rotary else None, sin.data_ptr() if rotary else None,
+            cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0, 1 if rotary_interleaved else 0,
+            B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
+            1 if causal else 0, ws.data_ptr() if ws is not None else None, nbytes, _stream(q)))
 
 
 def attn_merge(o_parts: torch.Tensor, lse_parts: torch.Tensor, o: torch.Tensor,

@@ -85,7 +85,10 @@ int make_tmap(CUtensorMap* out, const void* base, int elem_bytes, int rank, cons
     return set_error(B200K_EALIGN, "TMA needs a 16-byte aligned base (%p) and strides (row stride %llu bytes)", base,
                      (unsigned long long)strides[0]);
   const cuuint32_t estr[3] = {1, 1, 1};
-  CUresult r = fn(out, elem_bytes == 4 ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, rank,
+  const CUtensorMapDataType type = elem_bytes == 4   ? CU_TENSOR_MAP_DATA_TYPE_FLOAT32
+                                   : elem_bytes == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT8
+                                                     : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUresult r = fn(out, type, rank,
                   const_cast<void*>(base), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
                   CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
   if (r != CUDA_SUCCESS)

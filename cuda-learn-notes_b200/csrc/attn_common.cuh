@@ -183,17 +183,20 @@ struct AttnPacked {
   }
 };
 
-// One contiguous 16-bit [d2, d1, d0] tensor read through boxes [box2, box1, 64]: each box row is one 128-byte swizzle row.
+// One contiguous [d2, d1, d0] tensor of `elem`-byte elements (2: f16 / bf16, 1: fp8) read through boxes
+// [box2, box1, 128 / elem]: each box row is one 128-byte swizzle row.
 struct AttnTensor {
   const void* p;
   int64_t d2, d1, d0;
   int box2, box1;
+  int elem = 2;
 };
 
 static int attn_tmap(CUtensorMap* m, const AttnTensor& t) {
-  const uint64_t dims[3] = {uint64_t(t.d0), uint64_t(t.d1), uint64_t(t.d2)}, strides[2] = {2 * dims[0], 2 * dims[0] * dims[1]};
-  const uint32_t box[3] = {64, uint32_t(t.box1), uint32_t(t.box2)};
-  return make_tmap(m, t.p, 2, 3, dims, strides, box);
+  const uint64_t e = uint64_t(t.elem);
+  const uint64_t dims[3] = {uint64_t(t.d0), uint64_t(t.d1), uint64_t(t.d2)}, strides[2] = {e * dims[0], e * dims[0] * dims[1]};
+  const uint32_t box[3] = {uint32_t(128 / t.elem), uint32_t(t.box1), uint32_t(t.box2)};
+  return make_tmap(m, t.p, t.elem, 3, dims, strides, box);
 }
 
 static int check_headdim(const char* fn, int64_t D) {

@@ -167,6 +167,8 @@ struct AttnDecode {
   __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
     PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
   }
+  // the CTA's K/V head, from the grid rather than from Cta, so that no register holds it through the main loop
+  __device__ __forceinline__ int kv_head() const { return blockIdx.z % (H / group); }
   // rows past the box, the sequence or the group are not stored
   __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
     const int tt = r / hb, hh = r % hb;
@@ -223,7 +225,142 @@ struct AttnPackedPaged : AttnPacked<Cfg> {
   __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
     PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
   }
+  __device__ __forceinline__ int kv_head() const { return blockIdx.z % this->H / this->group; }
 };
+
+// A paged mode (AttnDecode, AttnPackedPaged) over fp8 caches: KVF is B200K_FP8_E4M3 or B200K_FP8_E5M2, k_scale /
+// v_scale fp32 [H_kv] or null (1.0).  The producer warpgroup stages each KV tile's fp8 rows and converts them into the
+// 16-bit K / V rings (fp8_produce), so the consumers run the 16-bit main loop unchanged; the scales enter through two
+// hooks: k_scale[h] multiplies scale_log2, and v_scale[h] the epilogue's 1 / l.  V rows past the key count are written
+// as zeros by the producer, so zero_v_tail has nothing to do.
+template <class Mode, int KVF>
+struct Fp8Kv : Mode {
+  static constexpr int KV_FP8 = KVF;
+  const float *k_scale, *v_scale;
+
+  using Cta = typename Mode::Cta;
+  __device__ __forceinline__ float kv_scale_log2(float scale_log2) const {
+    return k_scale ? scale_log2 * __ldg(k_scale + Mode::kv_head()) : scale_log2;
+  }
+  __device__ __forceinline__ float kv_out_scale(float inv) const {
+    return v_scale ? inv * __ldg(v_scale + Mode::kv_head()) : inv;
+  }
+  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+};
+
+// The KV format of a mode: 0 for the 16-bit caches, else Fp8Kv's KVF (also through WithLse, which derives from it).
+template <class M, class = void>
+struct KvFormat {
+  static constexpr int value = 0;
+};
+template <class M>
+struct KvFormat<M, std::void_t<decltype(M::KV_FP8)>> {
+  static constexpr int value = M::KV_FP8;
+};
+
+// Shared memory a mode adds to Cfg::smem_bytes: an fp8 mode's staging ring of two slots, each one BN-row fp8 tile of K
+// and one of V (BN x 128 bytes each: columns past D are zero-filled by TMA), and the slots' two full barriers.
+template <class Cfg, class Mode>
+constexpr int kv_stage_bytes() {
+  return KvFormat<Mode>::value ? 2 * 2 * Cfg::BN * 128 + 16 : 0;
+}
+
+// Two fp8 values (x: the first in the low byte) -> two 16-bit values of DT (the first in the low half), exactly:
+// every e4m3 and e5m2 value is an f16 value, and every f16 value converts exactly to f32 and, from these formats,
+// to bf16.
+template <int DT, int KVF>
+__device__ __forceinline__ uint32_t fp8x2_to_16(uint16_t x) {
+  uint32_t h;
+  if constexpr (KVF == B200K_FP8_E4M3) asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h) : "h"(x));
+  else asm("cvt.rn.f16x2.e5m2x2 %0, %1;" : "=r"(h) : "h"(x));
+  if constexpr (DT == 0) {
+    return h;
+  } else {
+    const float2 f = __half22float2(*reinterpret_cast<const __half2*>(&h));
+    const __nv_bfloat162 b = __floats2bfloat162_rn(f.x, f.y);
+    return *reinterpret_cast<const uint32_t*>(&b);
+  }
+}
+
+// Columns [64 c, 64 c + 64) of row r of a staged fp8 tile (BN rows of 128 bytes, 128B-swizzled as TMA wrote them) into
+// row r of a 16-bit chunk (BN rows of 64 columns, the layout TMA writes for the 16-bit caches), or zeros.  Row r's
+// 16-byte unit u sits at unit u ^ (r % 8) of the row; eight threads with consecutive rows hit eight distinct units,
+// so neither the loads nor the stores conflict on banks.
+template <int DT, int KVF>
+__device__ __forceinline__ void fp8_row_chunk(uint32_t src, uint32_t dst, int r, int c, bool zero) {
+  const uint32_t sw = r & 7;
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    uint32_t w[4] = {0u, 0u, 0u, 0u}, y[8];
+    if (!zero)
+      asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
+                   : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3])
+                   : "r"(src + r * 128 + (((4 * c + u) ^ sw) << 4)));
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      y[2 * k] = fp8x2_to_16<DT, KVF>(uint16_t(w[k] & 0xFFFFu));
+      y[2 * k + 1] = fp8x2_to_16<DT, KVF>(uint16_t(w[k] >> 16));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+      asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};" ::"r"(dst + r * 128 + (((2 * u + h) ^ sw) << 4)),
+                   "r"(y[4 * h]), "r"(y[4 * h + 1]), "r"(y[4 * h + 2]), "r"(y[4 * h + 3])
+                   : "memory");
+  }
+}
+
+// The producer warpgroup of an fp8 mode.  Its thread 0 TMA-loads each KV tile's fp8 K and V rows (the mode's paged
+// boxes, 128 fp8 columns wide) into staging slot n % 2 and, for the first two tiles, before the loop.  Per tile all 128
+// threads wait for the slot, and thread t converts key row t: the nqc K chunks (each after its kempty), then
+// fence.proxy.async and a named barrier, after which thread 0 arrives once on each chunk's kfull; then the DV / 64 V
+// chunks (after vempty, zeros for keys at or past kv_len, whatever the cache holds there), the fence and the barrier,
+// after which thread 0 arrives on vfull and refills the slot with tile n + 2.  No thread ever waits on itself: the
+// slot's reads are done at the barrier.
+template <class Cfg, class Mode>
+__device__ __forceinline__ void fp8_produce(const Mode& md, const typename Mode::Cta& cta, KvTiles kv, int nqc, uint32_t sK,
+                                            uint32_t sV, uint32_t sS, uint32_t kfull, uint32_t kempty, uint32_t vfull,
+                                            uint32_t vempty, uint32_t sfull, const CUtensorMap* tmK,
+                                            const CUtensorMap* tmV) {
+  constexpr int KVF = KvFormat<Mode>::value, TILE = Cfg::BN * 128, KST = Cfg::KSTAGES, VST = Cfg::VSTAGES;
+  const int r = threadIdx.x;
+  auto stage = [&](int j) {
+    const int ss = (j - kv.first) % 2;
+    const auto rows = md.kv_tile(cta, j);
+    mbar_arrive_expect_tx(sfull + 8 * ss, 2 * TILE);
+    md.load_k(cta, rows, sS + ss * 2 * TILE, tmK, sfull + 8 * ss, 0);
+    md.load_k(cta, rows, sS + ss * 2 * TILE + TILE, tmV, sfull + 8 * ss, 0);
+  };
+  if (r == 0)
+    for (int j = kv.first; j < kv.end && j < kv.first + 2; ++j) stage(j);
+  int kc = 0;
+  for (int j = kv.first; j < kv.end; ++j) {
+    const int n = j - kv.first;
+    const uint32_t src = sS + (n % 2) * 2 * TILE;
+    mbar_wait_nocall(sfull + 8 * (n % 2), (n / 2) & 1);
+    for (int c = 0; c < nqc; ++c) {
+      const int s = (kc + c) % KST;
+      if (kc + c >= KST) mbar_wait_nocall(kempty + 8 * s, (((kc + c) / KST) - 1) & 1);
+      fp8_row_chunk<Cfg::DT, KVF>(src, sK + s * Cfg::K_BYTES, r, c, false);
+    }
+    fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
+    named_bar_sync(2, 128);
+    if (r == 0)
+      for (int c = 0; c < nqc; ++c) mbar_arrive(kfull + 8 * ((kc + c) % KST));
+    kc += nqc;
+    const int sv = n % VST;
+    if (n >= VST) mbar_wait_nocall(vempty + 8 * sv, ((n / VST) - 1) & 1);
+    const bool past = j * Cfg::BN + r >= cta.kv_len;
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i)
+      fp8_row_chunk<Cfg::DT, KVF>(src + TILE, sV + sv * Cfg::V_BYTES + i * Cfg::BN * 128, r, i, past);
+    fence_proxy_async_smem();
+    named_bar_sync(2, 128);
+    if (r == 0) {
+      mbar_arrive(vfull + 8 * sv);
+      if (j + 2 < kv.end) stage(j + 2);
+    }
+  }
+}
 
 // A mode that also writes each stored row's natural-log log-sum-exp to `lse` (fp32, indexed like the rows of O): m is
 // the row's final running max in base-2 units and l the sum of the rounded P that divides O, so O and lse describe
@@ -246,11 +383,15 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
                           const __grid_constant__ CUtensorMap tmV, void* O, int D, int nqc, float scale_log2,
                           const Mode md) {
   constexpr int BM = Cfg::BM, BN = Cfg::BN, DV = Cfg::DV, KST = Cfg::KSTAGES, VST = Cfg::VSTAGES;
+  constexpr bool FP8 = KvFormat<Mode>::value != 0;
+  static_assert(!FP8 || BN == 128, "fp8 caches: one producer thread per key of a tile");
   extern __shared__ uint8_t smem_raw[];
   const uint32_t sQ = (smem_u32(smem_raw) + 1023) & ~1023u;
   const uint32_t sK = sQ + nqc * BM * 128, sV = sK + KST * Cfg::K_BYTES;
-  const uint32_t qbar = sV + VST * Cfg::V_BYTES;
+  const uint32_t sS = sV + VST * Cfg::V_BYTES;  // fp8 staging ring (fp8 modes only)
+  const uint32_t qbar = sS + (FP8 ? 2 * 2 * BN * 128 : 0);
   const uint32_t kfull = qbar + 8, kempty = kfull + 8 * KST, vfull = kempty + 8 * KST, vempty = vfull + 8 * VST;
+  const uint32_t sfull = vempty + 8 * VST;  // fp8 staging slots' full barriers
 
   typename Mode::Cta cta;
   if (!md.setup(cta)) return;
@@ -267,11 +408,31 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
       mbar_init(vfull + 8 * s, 1);
       mbar_init(vempty + 8 * s, Cfg::NWG);
     }
+    if constexpr (FP8)
+      for (int s = 0; s < 2; ++s) mbar_init(sfull + 8 * s, 1);
     fence_mbar_init();
   }
   __syncthreads();
 
-  if (wg == 0) {
+  if constexpr (FP8) {
+    // Two consumer warpgroups hold 168 registers, the most a 384-thread CTA allows, and ptxas spills their row sums at
+    // that count once the converting producer shares the kernel.  The producer needs fewer: it runs on 80 and the
+    // consumers on 208, within the CTA's 384 x 168.  (The values computed before the split must fit the producer's
+    // count: at 56, ptxas spills them.)
+    constexpr int PRODUCER_REGS = 80, CONSUMER_REGS = 208;
+    static_assert(128 * PRODUCER_REGS + 256 * CONSUMER_REGS <= 384 * 168, "more registers than the CTA holds");
+    if (wg == 0) {
+      if constexpr (Cfg::NWG == 2) setmaxnreg_dec<PRODUCER_REGS>();
+      if (threadIdx.x == 0) {
+        mbar_arrive_expect_tx(qbar, nqc * md.q_bytes());
+        for (int c = 0; c < nqc; ++c) md.load_q(cta, sQ + c * BM * 128, &tmQ, qbar, c);
+      }
+      fp8_produce<Cfg>(md, cta, kv, nqc, sK, sV, sS, kfull, kempty, vfull, vempty, sfull, &tmK, &tmV);
+      return;
+    }
+    if constexpr (Cfg::NWG == 2) setmaxnreg_inc<CONSUMER_REGS>();
+    scale_log2 = md.kv_scale_log2(scale_log2);
+  } else if (wg == 0) {
     if (threadIdx.x == 0) {
       mbar_arrive_expect_tx(qbar, nqc * md.q_bytes());
       for (int c = 0; c < nqc; ++c) md.load_q(cta, sQ + c * BM * 128, &tmQ, qbar, c);
@@ -293,6 +454,12 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     return;
   }
 
+  // The fp8 modes wait without the timeout's printf: a kernel with a call in it keeps neither its setmaxnreg nor
+  // unserialised wgmmas.  The 16-bit modes keep the wait they have always compiled with.
+  auto wait = [](uint32_t bar, uint32_t parity) {
+    if constexpr (FP8) mbar_wait_nocall(bar, parity);
+    else mbar_wait(bar, parity);
+  };
   const int cw = wg - 1, lane = threadIdx.x & 31, warp = (threadIdx.x & 127) / 32;
   const bool leader = (threadIdx.x & 127) == 0;
   const int row0 = cta.q0 + cw * 64 + warp * 16 + lane / 4;  // this thread's rows: row0 and row0 + 8
@@ -300,7 +467,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
   for (int i = 0; i < DV / 2; ++i) o[i] = 0.f;
   float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f};
-  mbar_wait(qbar, 0);
+  wait(qbar, 0);
 
   int kc = 0;
   for (int j = kv.first; j < kv.end; ++j) {
@@ -311,7 +478,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     for (int i = 0; i < BN / 2; ++i) s_acc[i] = 0.f;
     for (int c = 0; c < nqc; ++c, ++kc) {
       const int s = kc % KST;
-      mbar_wait(kfull + 8 * s, (kc / KST) & 1);
+      wait(kfull + 8 * s, (kc / KST) & 1);
       fence_regs<BN / 2>(s_acc);
       wgmma_fence();
 #pragma unroll
@@ -380,7 +547,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 
     // ---- O += P V
     const int sv = n % VST;
-    mbar_wait(vfull + 8 * sv, (n / VST) & 1);
+    wait(vfull + 8 * sv, (n / VST) & 1);
     const uint32_t vb = sV + sv * Cfg::V_BYTES;
     md.zero_v_tail(cta, k0, vb);
     fence_regs<DV / 2>(o);
@@ -407,7 +574,8 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     float t = l[h];
     t += __shfl_xor_sync(0xffffffffu, t, 1);
     t += __shfl_xor_sync(0xffffffffu, t, 2);
-    md.store(cta, row0 + 8 * h, o, h, t > 0.f ? 1.f / t : 0.f, m[h], t, O, D);
+    if constexpr (FP8) md.store(cta, row0 + 8 * h, o, h, md.kv_out_scale(t > 0.f ? 1.f / t : 0.f), m[h], t, O, D);
+    else md.store(cta, row0 + 8 * h, o, h, t > 0.f ? 1.f / t : 0.f, m[h], t, O, D);
   }
 }
 
@@ -417,7 +585,7 @@ template <class Cfg, class Mode>
 static int launch_attn(const AttnTensor (&qkv)[3], dim3 grid, void* O, int64_t D, float scale, const Mode& args,
                        cudaStream_t s, const DeviceInfo& di) {
   const int nqc = int((D + 63) / 64);
-  const int smem = Cfg::smem_bytes(nqc);
+  const int smem = Cfg::smem_bytes(nqc) + kv_stage_bytes<Cfg, Mode>();
   if (smem > di.max_smem_optin)
     return set_error(B200K_ESHAPE, "attention: %d bytes of shared memory needed, device allows %d", smem, di.max_smem_optin);
   CUtensorMap tm[3];
@@ -537,7 +705,26 @@ struct KvAppend {
   long long kv_rows, q_rows;  // B * L_new * H_kv, B * Lq * H (rotary only, else 0)
   long long rotary_seqlen;
   int B, L_new, Lq, H, H_kv, D, page_size, pages_per_seq, rotary_dim, causal;
+  const float *k_scale = nullptr, *v_scale = nullptr;  // fp8 caches: fp32 [H_kv] or null (1.0)
 };
+
+// Eight 16-bit values of DT -> eight fp8 bytes of KVF (the first in the low byte): cvt.rn.satfinite of
+// float(x) / scale in IEEE fp32, so values past the format's largest finite value become it and NaN stays NaN.
+template <int DT, int KVF>
+__device__ __forceinline__ uint2 quantize8(uint4 x, float scale) {
+  const uint32_t* w = reinterpret_cast<const uint32_t*>(&x);
+  uint32_t out[2];
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    const float2 f = unpack2<DT>(w[k]);
+    const float lo = __fdiv_rn(f.x, scale), hi = __fdiv_rn(f.y, scale);
+    uint16_t q;
+    if constexpr (KVF == B200K_FP8_E4M3) asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(q) : "f"(hi), "f"(lo));
+    else asm("cvt.rn.satfinite.e5m2x2.f32 %0, %1, %2;" : "=h"(q) : "f"(hi), "f"(lo));
+    out[k / 2] = k & 1 ? out[k / 2] | (uint32_t(q) << 16) : uint32_t(q);
+  }
+  return make_uint2(out[0], out[1]);
+}
 
 // Pair (x0, x1) at position pos becomes (x0 c - x1 s, x0 s + x1 c) in fp32, rounded once.  The products are not left to
 // contraction, so Q and K rows go through the same operations wherever this is inlined.
@@ -584,8 +771,10 @@ __device__ __forceinline__ uint4 rotate_vec(uint4 x, const uint16_t* row, int v,
 }
 
 // One thread per 16-byte vector: K rows, then V rows, then (rotary) Q rows; the first B threads also write lens_out.
-// Cache slots are written only for positions below the capacity, and the block table is read only for those.
-template <int DT, bool ROTARY, bool INTERLEAVED>
+// Cache slots are written only for positions below the capacity, and the block table is read only for those.  KVF: 0
+// for 16-bit caches, or the fp8 format the vector is quantised to (quantize8, by the scale of its K/V head) after
+// rotary, into one 8-byte store.
+template <int DT, bool ROTARY, bool INTERLEAVED, int KVF>
 __global__ void __launch_bounds__(256) kvcache_append_kernel(const KvAppend a) {
   const int vecs = a.D / 8;
   const long long tid = blockIdx.x * (long long)blockDim.x + threadIdx.x;
@@ -610,8 +799,15 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const KvAppend a) {
       if constexpr (ROTARY)
         if (is_k && 8 * v < a.rotary_dim) x = rotate_vec<DT, INTERLEAVED>(x, src, v, p, a);
       const long long page = a.table ? (long long)__ldg(a.table + b * a.pages_per_seq + p / a.page_size) : b;
-      uint16_t* dst = (is_k ? a.k_cache : a.v_cache) + ((page * a.page_size + p % a.page_size) * a.H_kv + hk) * a.D;
-      reinterpret_cast<uint4*>(dst)[v] = x;
+      if constexpr (KVF == 0) {
+        uint16_t* dst = (is_k ? a.k_cache : a.v_cache) + ((page * a.page_size + p % a.page_size) * a.H_kv + hk) * a.D;
+        reinterpret_cast<uint4*>(dst)[v] = x;
+      } else {
+        const float* sc = is_k ? a.k_scale : a.v_scale;
+        uint8_t* dst = reinterpret_cast<uint8_t*>(is_k ? a.k_cache : a.v_cache) +
+                       ((page * a.page_size + p % a.page_size) * a.H_kv + hk) * a.D;
+        reinterpret_cast<uint2*>(dst)[v] = quantize8<DT, KVF>(x, sc ? __ldg(sc + hk) : 1.f);
+      }
     } else if constexpr (ROTARY) {
       row -= 2 * a.kv_rows;
       const long long b = row / ((long long)a.Lq * a.H);
@@ -720,11 +916,13 @@ static int kvcache_args(const char* fn, const void* Q, const void* K_cache, cons
 
 // Everything of a decode call after its workspace check: the decode kernel on `g`'s grid (Q read through a 3-D map,
 // lengths from `seqlens`), then the combine kernel when the call is split.  `part` is the split region of the workspace;
-// `lse` (null, or [B, Lq, H] fp32) is written by the decode kernel unsplit and by the combine kernel split.
+// `lse` (null, or [B, Lq, H] fp32) is written by the decode kernel unsplit and by the combine kernel split.  kv_dtype:
+// 0 for caches in dtype, or B200K_FP8_E4M3 / B200K_FP8_E5M2 with k_scale / v_scale (Fp8Kv).
 static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse, const int* seqlens,
                           const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
-                          const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di) {
+                          const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di, int kv_dtype = 0,
+                          const float* k_scale = nullptr, const float* v_scale = nullptr) {
   return run_attn_cfg<1, false>(dtype, D, [&](auto cfg) {
     using Cfg = decltype(cfg);
     AttnDecode<Cfg> d;
@@ -747,22 +945,35 @@ static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cach
       d.part = static_cast<float*>(part);
       d.lse = d.part + size_t(g.splits) * size_t(d.rows) * size_t(D);
     }
+    const int elem = kv_dtype ? 1 : 2;
     const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
-                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1},
-                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1}};
+                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1, elem},
+                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1, elem}};
     const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
-    if (g.splits == 1) return launch_mode<Cfg>(qkv, grid, O, D, scale, d, lse, s, di);
-    const int launched = launch_attn<Cfg>(qkv, grid, O, D, scale, d, s, di);
-    if (launched) return launched;
-    const long long work = d.rows * (D / 2);
-    const unsigned blocks = unsigned((work + 255) / 256);
-    if (lse)
-      attn_combine_kernel<Cfg::DT, float, true><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits, lse);
-    else
-      attn_combine_kernel<Cfg::DT><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
-    B200K_CHECK_CUDA(cudaGetLastError());
-    return B200K_OK;
+    auto run = [&](const auto& mode) {
+      if (g.splits == 1) return launch_mode<Cfg>(qkv, grid, O, D, scale, mode, lse, s, di);
+      const int launched = launch_attn<Cfg>(qkv, grid, O, D, scale, mode, s, di);
+      if (launched) return launched;
+      const long long work = d.rows * (D / 2);
+      const unsigned blocks = unsigned((work + 255) / 256);
+      if (lse)
+        attn_combine_kernel<Cfg::DT, float, true><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits, lse);
+      else
+        attn_combine_kernel<Cfg::DT><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
+      B200K_CHECK_CUDA(cudaGetLastError());
+      return B200K_OK;
+    };
+    if (kv_dtype == B200K_FP8_E4M3) return run(Fp8Kv<AttnDecode<Cfg>, B200K_FP8_E4M3>{d, k_scale, v_scale});
+    if (kv_dtype == B200K_FP8_E5M2) return run(Fp8Kv<AttnDecode<Cfg>, B200K_FP8_E5M2>{d, k_scale, v_scale});
+    return run(d);
   });
+}
+
+// The checks the fp8 entry points add (before any CUDA call): the cache format, and the scales' alignment.
+static int fp8_args(const char* fn, int kv_dtype, const float* k_scale, const float* v_scale) {
+  if (kv_dtype != B200K_FP8_E4M3 && kv_dtype != B200K_FP8_E5M2)
+    return set_error(B200K_EDTYPE, "%s: kv_dtype %d not supported (fp8 e4m3, fp8 e5m2)", fn, kv_dtype);
+  return check_align(fn, {{k_scale, "k_scale", 4}, {v_scale, "v_scale", 4}});
 }
 
 // Workspace of b200k_fa2_fwd_kvcache_append, each section on a 256-byte boundary: int32 lengths [B], the rotated Q
@@ -814,6 +1025,83 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
 
 // The one check an lse output adds to an attention call (null: no lse).
 static int check_lse(const char* fn, const float* lse) { return check_align(fn, {{lse, "lse", 4}}); }
+
+// The append kernel of cache format KVF (0: dtype) for dtype and the rotary options, on `grid`.
+template <int KVF>
+static int launch_append(const KvAppend& a, int dtype, bool rotary, int rotary_interleaved, dim3 grid, cudaStream_t s) {
+  auto append = [&](auto kern) {
+    kern<<<grid, 256, 0, s>>>(a);
+    B200K_CHECK_CUDA(cudaGetLastError());
+    return B200K_OK;
+  };
+  if (dtype == B200K_BF16)
+    return !rotary ? append(kvcache_append_kernel<1, false, false, KVF>)
+                   : rotary_interleaved ? append(kvcache_append_kernel<1, true, true, KVF>)
+                                        : append(kvcache_append_kernel<1, true, false, KVF>);
+  return !rotary ? append(kvcache_append_kernel<0, false, false, KVF>)
+                 : rotary_interleaved ? append(kvcache_append_kernel<0, true, true, KVF>)
+                                      : append(kvcache_append_kernel<0, true, false, KVF>);
+}
+
+// Everything of an append call after its argument checks: the workspace check, the append kernel, then the decode.
+static int kvcache_append_launch(const char* fn, const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
+                                 const int* cache_seqlens, const int* block_table, const void* K_new, const void* V_new,
+                                 int64_t L_new, const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
+                                 int64_t rotary_dim, int rotary_interleaved, int64_t B, int64_t Lq, int64_t H,
+                                 int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                 float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
+                                 void* stream, int kv_dtype, const float* k_scale, const float* v_scale) {
+  int rc;
+  const int64_t capacity = pages_per_seq * page_size;
+  const bool rotary = rotary_cos != nullptr;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, capacity, di.sm_count);
+  const AppendLayout lay = append_layout(B, Lq, H, D, rotary, g);
+  if (!workspace || workspace_bytes < lay.bytes)
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, lay.bytes,
+                     workspace ? workspace_bytes : size_t(0));
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  uint8_t* ws = static_cast<uint8_t*>(workspace);
+  KvAppend a;
+  a.q = static_cast<const uint16_t*>(Q);
+  a.k_new = static_cast<const uint16_t*>(K_new);
+  a.v_new = static_cast<const uint16_t*>(V_new);
+  a.cos = static_cast<const uint16_t*>(rotary_cos);
+  a.sin = static_cast<const uint16_t*>(rotary_sin);
+  a.q_out = rotary ? reinterpret_cast<uint16_t*>(ws + lay.q) : nullptr;
+  a.k_cache = static_cast<uint16_t*>(K_cache);
+  a.v_cache = static_cast<uint16_t*>(V_cache);
+  a.seqlens = cache_seqlens;
+  a.table = block_table;
+  a.lens_out = reinterpret_cast<int*>(ws);
+  a.kv_rows = B * L_new * H_kv;
+  a.q_rows = rotary ? B * Lq * H : 0;
+  a.rotary_seqlen = rotary_seqlen;
+  a.B = int(B);
+  a.L_new = int(L_new);
+  a.Lq = int(Lq);
+  a.H = int(H);
+  a.H_kv = int(H_kv);
+  a.D = int(D);
+  a.page_size = int(page_size);
+  a.pages_per_seq = int(pages_per_seq);
+  a.rotary_dim = rotary ? int(rotary_dim) : 0;
+  a.causal = causal ? 1 : 0;
+  a.k_scale = k_scale;
+  a.v_scale = v_scale;
+  const long long items = (2 * a.kv_rows + a.q_rows) * (D / 8);
+  const long long blocks = ((items > B ? items : B) + 255) / 256;
+  const dim3 grid(unsigned(blocks < 65535 ? blocks : 65535));
+  rc = kv_dtype == B200K_FP8_E4M3   ? launch_append<B200K_FP8_E4M3>(a, dtype, rotary, rotary_interleaved, grid, s)
+       : kv_dtype == B200K_FP8_E5M2 ? launch_append<B200K_FP8_E5M2>(a, dtype, rotary, rotary_interleaved, grid, s)
+                                    : launch_append<0>(a, dtype, rotary, rotary_interleaved, grid, s);
+  if (rc) return rc;
+  // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
+  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, lse, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
+                        page_size, pages_per_seq, scale, dtype, causal, g, ws + lay.part, s, di, kv_dtype, k_scale, v_scale);
+}
+
 
 }  // namespace b200k
 
@@ -905,19 +1193,20 @@ extern "C" int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void
   });
 }
 
-extern "C" int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
-                                      const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
-                                      int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv,
-                                      int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
-                                      float scale, int dtype, int causal, void* stream) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_varlen_paged";
+namespace b200k {
+
+// b200k_fa2_varlen_paged, and with kv_dtype = B200K_FP8_E4M3 / B200K_FP8_E5M2 and its scales, the fp8 call.
+static int varlen_paged(const char* fn, const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                        const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table, int64_t B,
+                        int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D, int64_t num_pages,
+                        int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal, void* stream,
+                        int kv_dtype, const float* k_scale, const float* v_scale) {
   if (!Q || !K_cache || !V_cache || !O || !cu_seqlens_q || !cu_seqlens_k || !block_table)
     return set_error(B200K_EARG, "%s: null pointer", fn);
   if (dtype != B200K_F16 && dtype != B200K_BF16)
     return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
-  int rc = check_headdim(fn, D);
-  if (rc) return rc;
+  int rc = kv_dtype ? fp8_args(fn, kv_dtype, k_scale, v_scale) : B200K_OK;
+  if (rc || (rc = check_headdim(fn, D))) return rc;
   if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
     return set_error(B200K_ESHAPE, "%s: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)", fn,
                      (long long)B, (long long)H, (long long)H_kv);
@@ -940,14 +1229,44 @@ extern "C" int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const 
     using Cfg = decltype(cfg);
     const int box_rows = page_size < Cfg::BN ? int(page_size) : Cfg::BN;
     const int64_t cache_rows = num_pages * page_size;
+    const int elem = kv_dtype ? 1 : 2;
     const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1},
-                               {K_cache, cache_rows, H_kv, D, box_rows, 1},
-                               {V_cache, cache_rows, H_kv, D, box_rows, 1}};
+                               {K_cache, cache_rows, H_kv, D, box_rows, 1, elem},
+                               {V_cache, cache_rows, H_kv, D, box_rows, 1, elem}};
     const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
     const AttnPackedPaged<Cfg> args = {{cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0},
                                        block_table, int(page_size), int(pages_per_seq), box_rows, int(cache_rows)};
+    if (kv_dtype == B200K_FP8_E4M3)
+      return launch_mode<Cfg>(qkv, grid, O, D, scale, Fp8Kv<AttnPackedPaged<Cfg>, B200K_FP8_E4M3>{args, k_scale, v_scale},
+                              lse, s, di);
+    if (kv_dtype == B200K_FP8_E5M2)
+      return launch_mode<Cfg>(qkv, grid, O, D, scale, Fp8Kv<AttnPackedPaged<Cfg>, B200K_FP8_E5M2>{args, k_scale, v_scale},
+                              lse, s, di);
     return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
   });
+}
+
+}  // namespace b200k
+
+extern "C" int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                                      const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
+                                      int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv,
+                                      int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                      float scale, int dtype, int causal, void* stream) {
+  return b200k::varlen_paged("b200k_fa2_varlen_paged", Q, K_cache, V_cache, O, lse, cu_seqlens_q, cu_seqlens_k,
+                             block_table, B, max_seqlen_q, total_q, H, H_kv, D, num_pages, page_size, pages_per_seq,
+                             scale, dtype, causal, stream, 0, nullptr, nullptr);
+}
+
+extern "C" int b200k_fa2_varlen_paged_fp8(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                                          const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
+                                          const float* k_scale, const float* v_scale, int kv_dtype, int64_t B,
+                                          int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D,
+                                          int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale,
+                                          int dtype, int causal, void* stream) {
+  return b200k::varlen_paged("b200k_fa2_varlen_paged_fp8", Q, K_cache, V_cache, O, lse, cu_seqlens_q, cu_seqlens_k,
+                             block_table, B, max_seqlen_q, total_q, H, H_kv, D, num_pages, page_size, pages_per_seq,
+                             scale, dtype, causal, stream, kv_dtype, k_scale, v_scale);
 }
 
 extern "C" int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
@@ -1038,59 +1357,10 @@ extern "C" int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, vo
                         workspace)) ||
       (rc = check_lse("b200k_fa2_fwd_kvcache_append_lse", lse)))
     return rc;
-  const bool rotary = rotary_cos != nullptr;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, capacity, di.sm_count);
-  const AppendLayout lay = append_layout(B, Lq, H, D, rotary, g);
-  if (!workspace || workspace_bytes < lay.bytes)
-    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, lay.bytes,
-                     workspace ? workspace_bytes : size_t(0));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  KvAppend a;
-  a.q = static_cast<const uint16_t*>(Q);
-  a.k_new = static_cast<const uint16_t*>(K_new);
-  a.v_new = static_cast<const uint16_t*>(V_new);
-  a.cos = static_cast<const uint16_t*>(rotary_cos);
-  a.sin = static_cast<const uint16_t*>(rotary_sin);
-  a.q_out = rotary ? reinterpret_cast<uint16_t*>(ws + lay.q) : nullptr;
-  a.k_cache = static_cast<uint16_t*>(K_cache);
-  a.v_cache = static_cast<uint16_t*>(V_cache);
-  a.seqlens = cache_seqlens;
-  a.table = block_table;
-  a.lens_out = reinterpret_cast<int*>(ws);
-  a.kv_rows = B * L_new * H_kv;
-  a.q_rows = rotary ? B * Lq * H : 0;
-  a.rotary_seqlen = rotary_seqlen;
-  a.B = int(B);
-  a.L_new = int(L_new);
-  a.Lq = int(Lq);
-  a.H = int(H);
-  a.H_kv = int(H_kv);
-  a.D = int(D);
-  a.page_size = int(page_size);
-  a.pages_per_seq = int(pages_per_seq);
-  a.rotary_dim = rotary ? int(rotary_dim) : 0;
-  a.causal = causal ? 1 : 0;
-  const long long items = (2 * a.kv_rows + a.q_rows) * (D / 8);
-  const long long blocks = ((items > B ? items : B) + 255) / 256;
-  const dim3 grid(unsigned(blocks < 65535 ? blocks : 65535));
-  auto append = [&](auto kern) {
-    kern<<<grid, 256, 0, s>>>(a);
-    B200K_CHECK_CUDA(cudaGetLastError());
-    return B200K_OK;
-  };
-  if (dtype == B200K_BF16)
-    rc = !rotary ? append(kvcache_append_kernel<1, false, false>)
-                 : rotary_interleaved ? append(kvcache_append_kernel<1, true, true>) : append(kvcache_append_kernel<1, true, false>);
-  else
-    rc = !rotary ? append(kvcache_append_kernel<0, false, false>)
-                 : rotary_interleaved ? append(kvcache_append_kernel<0, true, true>) : append(kvcache_append_kernel<0, true, false>);
-  if (rc) return rc;
-  // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
-  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, lse, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
-                        page_size, pages_per_seq, scale, dtype, causal, g, ws + lay.part, s, di);
+  return kvcache_append_launch(fn, Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, K_new, V_new, L_new,
+                               rotary_cos, rotary_sin, rotary_seqlen, rotary_dim, rotary_interleaved, B, Lq, H, H_kv, D,
+                               num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace, workspace_bytes,
+                               stream, 0, nullptr, nullptr);
 }
 
 extern "C" int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows,
@@ -1136,4 +1406,54 @@ extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, v
   const int nqc = int((D + 63) / 64), slices = (nqc + 3) / 4, chunks = (nqc + slices - 1) / slices;
   return chunks == 3 ? launch_ffpa<192>(Q, K, V, O, B, H, N, D, scale, s, di)
                      : launch_ffpa<256>(Q, K, V, O, B, H, N, D, scale, s, di);
+}
+
+extern "C" int b200k_fa2_kvcache_fp8_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                                     int64_t max_seqlen_k, int append, int rotary, size_t* bytes) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_kvcache_fp8_workspace_bytes";
+  if (!bytes) return set_error(B200K_EARG, "%s: null pointer", fn);
+  int rc = check_headdim(fn, D);
+  if (rc || (rc = kvcache_check(fn, B, Lq, H, H_kv, max_seqlen_k))) return rc;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count);
+  *bytes = append ? append_layout(B, Lq, H, D, rotary != 0, g).bytes : g.workspace;
+  return B200K_OK;
+}
+
+extern "C" int b200k_fa2_kvcache_fp8(const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
+                                     const int* cache_seqlens, const int* block_table, const float* k_scale,
+                                     const float* v_scale, int kv_dtype, const void* K_new, const void* V_new,
+                                     int64_t L_new, const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
+                                     int64_t rotary_dim, int rotary_interleaved, int64_t B, int64_t Lq, int64_t H,
+                                     int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
+                                     float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  using namespace b200k;
+  const char* fn = "b200k_fa2_kvcache_fp8";
+  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+                        pages_per_seq, dtype);
+  if (rc || (rc = fp8_args(fn, kv_dtype, k_scale, v_scale)) || (rc = check_lse(fn, lse))) return rc;
+  if (K_new || V_new) {
+    if ((rc = append_args(fn, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, pages_per_seq * page_size, rotary_seqlen,
+                          rotary_dim, workspace)))
+      return rc;
+    return kvcache_append_launch(fn, Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, K_new, V_new, L_new,
+                                 rotary_cos, rotary_sin, rotary_seqlen, rotary_dim, rotary_interleaved, B, Lq, H, H_kv,
+                                 D, num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace,
+                                 workspace_bytes, stream, kv_dtype, k_scale, v_scale);
+  }
+  if (rotary_cos || rotary_sin)
+    return set_error(B200K_EARG, "%s: rotary_cos / rotary_sin rotate appended keys and need K_new / V_new", fn);
+  if ((rc = check_align(fn, {{workspace, "workspace", 16}}))) return rc;
+  DeviceInfo di;
+  if ((rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
+  if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, g.workspace,
+                     workspace ? workspace_bytes : size_t(0));
+  return kvcache_launch(Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
+                        pages_per_seq, scale, dtype, causal, g, workspace, static_cast<cudaStream_t>(stream), di, kv_dtype,
+                        k_scale, v_scale);
 }

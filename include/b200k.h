@@ -285,6 +285,53 @@ int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cac
                            int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D,
                            int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype,
                            int causal, void* stream);
+/* ------------------------------------------------------------------------------------------------ fp8 KV caches
+ * Decode (with or without append) and paged prefill over caches that hold K and V in 8-bit floats: twice the tokens in
+ * the same memory, and half the bytes a decode step reads (vLLM's kv_cache_dtype "fp8" / "fp8_e5m2" with k_scale /
+ * v_scale, flash-attn 3's descale_k / descale_v).  Everything not stated here is the 16-bit call's:
+ *   kv_dtype     B200K_FP8_E4M3 (torch float8_e4m3fn) or B200K_FP8_E5M2 (torch float8_e5m2).  K_cache, V_cache are
+ *                [num_pages, page_size, H_kv, D] (or contiguous [B, S, H_kv, D]) of 1-byte elements; Q, O, K_new, V_new,
+ *                rotary_cos / rotary_sin stay in dtype (B200K_F16 or B200K_BF16); D in {32, 64, 96, 128}.  Page sizes,
+ *                block table, lengths, causal rule, split rule, isolation, lse and "no sync" are the 16-bit calls'
+ *   scales       k_scale, v_scale: NULL (1.0) or fp32 device arrays [H_kv]; the key of K/V head h is fp8 * k_scale[h]
+ *                (vLLM's convention).  Device arrays, so a captured graph stays valid when the scales change
+ *   arithmetic   every fp8 value converts exactly to dtype.  k_scale folds into the softmax exponent: the kernel's
+ *                scale_log2 = (scale * log2 e) is multiplied once more, by k_scale[h], in fp32.  v_scale folds into
+ *                the epilogue: O = dtype(o * ((1 / l) * v_scale[h])), and split partials carry the same factor.  lse
+ *                is the log-sum-exp of the scaled scores
+ *   bits         with NULL scales, O and lse have the bits of the 16-bit call on caches holding dtype(K8), dtype(V8);
+ *                with power-of-two scales, on caches holding dtype(K8) * k_scale[h] and dtype(V8) * v_scale[h]
+ *                (while those products are normal dtype values), since every step above is then an exact rescaling
+ *   append       the byte stored for new element x is cvt.rn.satfinite(float(x16) / scale[h]) in the cache's format:
+ *                x16 the 16-bit value b200k_fa2_fwd_kvcache_append would store (rotary included), the division IEEE
+ *                fp32; values past the largest finite value become +-448 (e4m3) or +-57344 (e5m2), NaN stays NaN
+ *   alignment    the 16-bit call's, and k_scale, v_scale 4 bytes
+ * Errors before any CUDA call: those of the 16-bit call, B200K_EDTYPE for a kv_dtype other than the two above, and
+ * B200K_EALIGN naming k_scale or v_scale. */
+/* b200k_fa2_kvcache_fp8 — b200k_fa2_fwd_kvcache_lse over fp8 caches, and with K_new, V_new (both non-NULL)
+ * b200k_fa2_fwd_kvcache_append_lse: L_new, rotary_* and the workspace then mean what they mean there.  K_new == V_new
+ * == NULL is decode alone (L_new and the rotary sizes are ignored; rotary_cos / rotary_sin must be NULL, else
+ * B200K_EARG).  lse may be NULL.  workspace: at least what b200k_fa2_kvcache_fp8_workspace_bytes reports. */
+int b200k_fa2_kvcache_fp8(const void* Q, void* K_cache, void* V_cache, void* O, float* lse, const int* cache_seqlens,
+                          const int* block_table, const float* k_scale, const float* v_scale, int kv_dtype,
+                          const void* K_new, const void* V_new, int64_t L_new, const void* rotary_cos,
+                          const void* rotary_sin, int64_t rotary_seqlen, int64_t rotary_dim, int rotary_interleaved,
+                          int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D, int64_t num_pages,
+                          int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
+                          void* workspace, size_t workspace_bytes, void* stream);
+/* Workspace b200k_fa2_kvcache_fp8 needs: append == 0, decode's (b200k_fa2_fwd_kvcache_workspace_bytes); otherwise
+ * append's layout (b200k_fa2_fwd_kvcache_append_workspace_bytes with rotary).  Depends on the device's SM count. */
+int b200k_fa2_kvcache_fp8_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
+                                          int64_t max_seqlen_k, int append, int rotary, size_t* bytes);
+/* b200k_fa2_varlen_paged_fp8 — b200k_fa2_varlen_paged over fp8 pages, with k_scale, v_scale and kv_dtype as above.
+ * O and lse have the bits b200k_fa2_fwd_varlen_lse gives on K / V gathered through the table and dequantized (with
+ * NULL or power-of-two scales). */
+int b200k_fa2_varlen_paged_fp8(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
+                               const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
+                               const float* k_scale, const float* v_scale, int kv_dtype, int64_t B,
+                               int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D,
+                               int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype,
+                               int causal, void* stream);
 /* b200k_attn_merge — the attention over the union of S disjoint key sets from the attention over each (cascade /
  * shared-prefix decode, chunked prefill, keys sharded across devices):
  *   inputs      O_parts [S, rows, D] in dtype (B200K_F16 or B200K_BF16), lse_parts [S, rows] fp32 natural log, as the
