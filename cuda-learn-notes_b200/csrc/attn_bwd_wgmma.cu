@@ -139,6 +139,7 @@ struct BwdKeysDense {
     tma_load_3d(dst, tm, bar, chunk * 64, i * 64, c.bh, kPolicyEvictNormal);
   }
   __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
+  __device__ __forceinline__ void zero_q_tail(const Cta&, int, uint32_t) const {}
   __device__ __forceinline__ void row_stats(const BwdArgs& a, const Cta& c, int, int r, float& l2, float& dl) const {
     const size_t base = size_t(c.bh) * N;
     l2 = r < N ? __ldg(a.lse2 + base + r) : INFINITY;
@@ -153,7 +154,8 @@ struct BwdKeysDense {
 
 // Packed (AttnPacked's layout): y = b * H_kv + K/V head; the CTA visits the query tiles of each query head
 // h = K/V head * group + g of its group in turn, g ascending.  A key tile past Lk returns.  A query tile that runs past
-// Lq reads the next sequence's rows: their lse2 is +inf, so their P and dS are 0.  Keys past Lk are masked and not
+// Lq reads the next sequence's rows: their lse2 is +inf, so their P and dS are 0, and zero_q_tail zeroes their Q and
+// dO, which P^T and dS^T multiply.  Keys past Lk are masked and not
 // stored.  Row r sees keys <= r + Lk - Lq under the causal mask.  The store reloads cu_k rather than keep it through the
 // main loop.
 template <class Cfg>
@@ -186,6 +188,11 @@ struct BwdKeysPacked {
     tma_load_3d(dst, tm, bar, chunk * 64, c.kvh * group + g, c.q_tok + i * 64, kPolicyEvictNormal);
   }
   __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
+  // the Q and dO rows of query tile q0 past Lq, which S^T / dP^T hold as P^T = 0 columns that still multiply them
+  __device__ __forceinline__ void zero_q_tail(const Cta& c, int q0, uint32_t sq) const {
+    zero_tile_tail<Cfg>(c.q_len, q0, sq);
+    zero_tile_tail<Cfg>(c.q_len, q0, sq + 64 * Cfg::DV * 2);
+  }
   __device__ __forceinline__ void row_stats(const BwdArgs& a, const Cta& c, int g, int r, float& l2, float& dl) const {
     const size_t row = size_t(c.q_tok + r) * H + c.kvh * group + g;
     l2 = r < c.q_len ? __ldg(a.lse2 + row) : INFINITY;
@@ -265,6 +272,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
       for (int e = 0; e < 32; ++e) st[e] = dpt[e] = 0.f;
       mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
+      md.zero_q_tail(c, q0, sq);
       fence_regs<32>(st);
       fence_regs<32>(dpt);
       wgmma_fence();
@@ -420,6 +428,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
 #pragma unroll
     for (int e = 0; e < BN / 2; ++e) sa[e] = dp[e] = 0.f;
     mbar_wait_nocall(full + 8 * s, (n / ST) & 1);
+    md.zero_kv_tail(cta, k0, sk);  // dQ += dS~ K_j multiplies the masked dS of 0 by the K rows past the length
     fence_regs<BN / 2>(sa);
     fence_regs<BN / 2>(dp);
     wgmma_fence();

@@ -66,6 +66,56 @@ __device__ __forceinline__ void store_o(void* O, size_t row, int dv0, int D, con
 // KV tiles [first, end) of a CTA: tile j holds keys [j * BN, (j + 1) * BN) of its sequence.
 struct KvTiles { int first, end; };
 
+// Zeroes the rows at and past `len` of the BN-row tile of rows [k0, k0 + BN) at `tile`, laid out as Cfg's V: DV / 64
+// chunks of BN rows of 128 bytes (V [keys, D], a K tile, or the backward's Q and dO tiles), or with V_DN those keys'
+// columns of BN / 64 sub-tiles of DV rows of 64 keys, 128B-swizzled (unit u of row d at unit u ^ (d % 8)).  Rows a call
+// does not own may hold anything, and a masked P or dS of 0 times a NaN or Inf is NaN in the tensor core, so each mode
+// zeroes the operand rows it multiplies by a masked 0.  All 128 * NWG consumer threads share the stores and meet at one
+// barrier before any of them issues its wgmma; each reaches it in the same iteration, since the condition is the CTA's.
+template <class Cfg>
+__device__ __forceinline__ void zero_tile_tail(int len, int k0, uint32_t tile) {
+  constexpr int N = 128 * Cfg::NWG;
+  if (k0 + Cfg::BN <= len) return;
+  const int r0 = len - k0;  // first row to zero, within the tile
+  if constexpr (Cfg::V_DN) {
+    constexpr int UNITS = Cfg::BN / 64 * Cfg::DV * 8;  // 16-byte units of the tile
+    static_assert(UNITS % N == 0, "zero_tile_tail: every unit needs a thread");
+#pragma unroll
+    for (int k = 0; k < UNITS / N; ++k) {
+      const int w = threadIdx.x % N + k * N, d = w / 8 % Cfg::DV, u = w % 8, key = w / (8 * Cfg::DV) * 64 + 8 * u;
+      const uint32_t a = tile + w / (8 * Cfg::DV) * Cfg::DV * 128 + d * 128 + ((u ^ (d & 7)) << 4);
+      if (key >= r0) {
+        asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(a), "r"(0) : "memory");
+      } else if (key + 8 > r0) {
+#pragma unroll
+        for (int e = 0; e < 8; ++e)
+          if (key + e >= r0) asm volatile("st.shared.u16 [%0], %1;" ::"r"(a + 2 * e), "h"((unsigned short)0) : "memory");
+      }
+    }
+  } else {
+    const int words = (Cfg::BN - r0) * 8;  // 16-byte words per 64-column chunk
+    auto zero = [&](int i, int w) {
+      asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(tile + i * Cfg::BN * 128 + r0 * 128 + w * 16), "r"(0)
+                   : "memory");
+    };
+#pragma unroll
+    for (int i = 0; i < Cfg::DV / 64; ++i) {
+      if constexpr (Cfg::NWG == 1) {
+        for (int w = threadIdx.x % N; w < words; w += N) zero(i, w);
+      } else {
+        // Two consumer warpgroups already hold 168 registers, the most a 384-thread CTA allows; a fixed count of
+        // predicated stores needs fewer live registers than the loop above, which would spill.
+        static_assert(Cfg::BN * 8 % N == 0, "zero_tile_tail: every 16-byte word of a chunk needs a thread");
+#pragma unroll
+        for (int k = 0; k < Cfg::BN * 8 / N; ++k)
+          if (threadIdx.x % N + k * N < words) zero(i, threadIdx.x % N + k * N);
+      }
+    }
+  }
+  fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
+  named_bar_sync(1, N);
+}
+
 // [B, H, N, D], one 3-D map per tensor over (D, N, B * H); V stored [B, H, D, N] over (N, D, B * H).  CTA (x, y, z) =
 // (query tile, O column slice, batch * H + head).  Rows are numbered within the head, so row r sees keys <= r under the
 // causal mask.  The modes of the forward are described in attn_fwd_wgmma.cu; the backward's dQ kernel takes this one
@@ -109,7 +159,11 @@ struct AttnDense {
     }
   }
   __device__ __forceinline__ int diag(const Cta&, int r) const { return r; }
-  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  // keys past seqlens_k are the caller's padding; past N, TMA has zero-filled the tile, so a call without seqlens_k
+  // (kv_len = N) does no extra work
+  __device__ __forceinline__ void zero_kv_tail(const Cta& c, int k0, uint32_t tile) const {
+    if (c.kv_len < N) zero_tile_tail<Cfg>(c.kv_len, k0, tile);
+  }
   __device__ __forceinline__ bool out_row(const Cta& c, int r, size_t& row) const {
     if (r >= N) return false;
     row = size_t(c.bh) * N + r;
@@ -167,7 +221,10 @@ struct AttnPacked {
     for (int i = 0; i < Cfg::DV / 64; ++i) load_k(c, tok, dst + i * Cfg::BN * 128, tm, bar, i);
   }
   __device__ __forceinline__ int diag(const Cta& c, int r) const { return r + c.shift; }
-  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  // keys past Lk are the next sequence's tokens, or whatever lies past cu_k[B]
+  __device__ __forceinline__ void zero_kv_tail(const Cta& c, int k0, uint32_t tile) const {
+    zero_tile_tail<Cfg>(c.kv_len, k0, tile);
+  }
   __device__ __forceinline__ bool out_row(const Cta&, int r, size_t& row) const {
     const int b = blockIdx.z / H, q_tok = __ldg(cu_q + b);
     if (r >= __ldg(cu_q + b + 1) - q_tok) return false;

@@ -35,7 +35,8 @@ __device__ __forceinline__ float2 unpack2(uint32_t w) {
 // first row q0 (its rows are q0 .. q0 + BM - 1 in the numbering diag and store take), which setup fills (false: no rows
 // here; the CTA returns before any barrier exists); tiles, the KV tiles it visits; q_bytes and load_q, the bytes and the
 // box of 64-column chunk c of Q; kv_tile, where KV tile j is, for load_k (chunk c of K) and load_v (all of V); diag,
-// the causal diagonal (last key seen) of row r; zero_v_tail, which only the paged modes fill in; out_row, whether row r
+// the causal diagonal (last key seen) of row r; zero_kv_tail, which zeroes the V rows of a tile past the CTA's key
+// count (zero_tile_tail, attn_common.cuh; what the tile holds there is not the call's); out_row, whether row r
 // is stored and to which row of O (viewed as [rows, D]); store, the epilogue of row r.  The dense and packed modes,
 // AttnDense and AttnPacked, are in attn_common.cuh, which the backward shares.
 
@@ -77,34 +78,6 @@ struct PagedKv {
                                                 uint32_t bar) {
 #pragma unroll
     for (int i = 0; i < Cfg::DV / 64; ++i) load_k(m, kvh, t, dst + i * Cfg::BN * 128, tm, bar, i);
-  }
-  // The tile that straddles the length: cache rows past it may hold anything, and a masked P of 0 times a NaN or Inf in
-  // V is NaN in the tensor core, so those V rows are zeroed (K needs nothing: its scores became -inf).  Every consumer
-  // warpgroup waits on the same V stage, so all 128 * NWG consumer threads share the stores and meet at one barrier
-  // before any of them issues its wgmma.  Each reaches it in the same iteration: the condition is the CTA's.
-  __device__ __forceinline__ static void zero_v_tail(int kv_len, int k0, uint32_t vb) {
-    constexpr int N = 128 * Cfg::NWG;
-    if (k0 + Cfg::BN <= kv_len) return;
-    const int r0 = kv_len - k0, words = (Cfg::BN - r0) * 8;  // 16-byte words per 64-column chunk
-    auto zero = [&](int i, int w) {
-      asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(vb + i * Cfg::BN * 128 + r0 * 128 + w * 16), "r"(0)
-                   : "memory");
-    };
-#pragma unroll
-    for (int i = 0; i < Cfg::DV / 64; ++i) {
-      if constexpr (Cfg::NWG == 1) {
-        for (int w = threadIdx.x % N; w < words; w += N) zero(i, w);
-      } else {
-        // Two consumer warpgroups already hold 168 registers, the most a 384-thread CTA allows; a fixed count of
-        // predicated stores needs fewer live registers than the loop above, which would spill.
-        static_assert(Cfg::BN * 8 % N == 0, "zero_v_tail: every 16-byte word of a chunk needs a thread");
-#pragma unroll
-        for (int k = 0; k < Cfg::BN * 8 / N; ++k)
-          if (threadIdx.x % N + k * N < words) zero(i, threadIdx.x % N + k * N);
-      }
-    }
-    fence_proxy_async_smem();  // generic-proxy stores -> the wgmma's operand reads
-    named_bar_sync(1, N);
   }
 };
 
@@ -164,8 +137,8 @@ struct AttnDecode {
     PagedKv<Cfg>::load_v(*this, c.kvh, t, dst, tm, bar);
   }
   __device__ __forceinline__ int diag(const Cta& c, int r) const { return c.t0 + r / hb + c.shift; }
-  __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
-    PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
+  __device__ __forceinline__ void zero_kv_tail(const Cta& c, int k0, uint32_t tile) const {
+    zero_tile_tail<Cfg>(c.kv_len, k0, tile);
   }
   // the CTA's K/V head, from the grid rather than from Cta, so that no register holds it through the main loop
   __device__ __forceinline__ int kv_head() const { return blockIdx.z % (H / group); }
@@ -222,9 +195,6 @@ struct AttnPackedPaged : AttnPacked<Cfg> {
                                          uint32_t bar) const {
     PagedKv<Cfg>::load_v(*this, c.kv_head, t, dst, tm, bar);
   }
-  __device__ __forceinline__ void zero_v_tail(const Cta& c, int k0, uint32_t vb) const {
-    PagedKv<Cfg>::zero_v_tail(c.kv_len, k0, vb);
-  }
   __device__ __forceinline__ int kv_head() const { return blockIdx.z % this->H / this->group; }
 };
 
@@ -232,7 +202,7 @@ struct AttnPackedPaged : AttnPacked<Cfg> {
 // v_scale fp32 [H_kv] or null (1.0).  The producer warpgroup stages each KV tile's fp8 rows and converts them into the
 // 16-bit K / V rings (fp8_produce), so the consumers run the 16-bit main loop unchanged; the scales enter through two
 // hooks: k_scale[h] multiplies scale_log2, and v_scale[h] the epilogue's 1 / l.  V rows past the key count are written
-// as zeros by the producer, so zero_v_tail has nothing to do.
+// as zeros by the producer, so zero_kv_tail has nothing to do.
 template <class Mode, int KVF>
 struct Fp8Kv : Mode {
   static constexpr int KV_FP8 = KVF;
@@ -245,7 +215,7 @@ struct Fp8Kv : Mode {
   __device__ __forceinline__ float kv_out_scale(float inv) const {
     return v_scale ? inv * __ldg(v_scale + Mode::kv_head()) : inv;
   }
-  __device__ __forceinline__ void zero_v_tail(const Cta&, int, uint32_t) const {}
+  __device__ __forceinline__ void zero_kv_tail(const Cta&, int, uint32_t) const {}
 };
 
 // The KV format of a mode: 0 for the 16-bit caches, else Fp8Kv's KVF (also through WithLse, which derives from it).
@@ -549,7 +519,7 @@ __global__ void __launch_bounds__(Cfg::THREADS, 1)
     const int sv = n % VST;
     wait(vfull + 8 * sv, (n / VST) & 1);
     const uint32_t vb = sV + sv * Cfg::V_BYTES;
-    md.zero_v_tail(cta, k0, vb);
+    md.zero_kv_tail(cta, k0, vb);
     fence_regs<DV / 2>(o);
     wgmma_fence();
 #pragma unroll
