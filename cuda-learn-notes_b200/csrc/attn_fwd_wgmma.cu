@@ -980,17 +980,14 @@ static int append_args(const char* fn, const void* K_new, const void* V_new, con
 }
 
 // Large head dims: O in column slices of DV = 192 or 256 (as few slices as possible, each a whole number of 64-column
-// chunks).  DV = 192 runs two consumer warpgroups when Q (128 rows) fits in shared memory next to the K and V rings;
-// DV = 256 needs more registers than a 384-thread block can give each thread (168), so it runs one.
+// chunks).  DV = 192 runs two consumer warpgroups: it serves at most 9 Q chunks (D <= 576), whose 128 Q rows fit in
+// shared memory next to the K and V rings on every sm_90 part (230 504 of 232 448 bytes at 9 chunks).  DV = 256 needs
+// more registers than a 384-thread block can give each thread (168), so it runs one.
 template <int DV>
 static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int64_t B, int64_t H, int64_t N, int64_t D,
                        float scale, cudaStream_t s, const DeviceInfo& di) {
-  if constexpr (DV == 192) {
-    using Two = AttnCfg<0, DV, 2, 64, false>;
-    if (Two::smem_bytes(int((D + 63) / 64)) <= di.max_smem_optin)
-      return launch_dense<Two>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, nullptr, s, di);
-  }
-  return launch_dense<AttnCfg<0, DV, 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, nullptr, s, di);
+  return launch_dense<AttnCfg<0, DV, DV == 192 ? 2 : 1, 64, false>>(Q, K, V, O, B, H, N, D, scale, nullptr, 0, nullptr, s,
+                                                                     di);
 }
 
 // The one check an lse output adds to an attention call (null: no lse).

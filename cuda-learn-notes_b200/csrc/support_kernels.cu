@@ -255,7 +255,9 @@ static int launch_reduce(const void* x, void* out, int64_t n, int acc_f16, void*
                          const DeviceInfo& di) {
   const int grid = reduce_grid(n / Loader<DT>::N, di.sm_count);
   const bool vec_ok = aligned16(x);
-  if (acc_f16 && !EXP) reduce_sum_kernel<DT, true, false><<<grid, kThreads, 0, s>>>(x, out, n, ws, vec_ok);
+  // fp16 accumulation exists for the 16-bit and fp8 inputs only: no f32, int8 or exp-sum kernel is built with it
+  constexpr bool kAcc16 = !EXP && DT != B200K_F32 && DT != B200K_I8;
+  if (kAcc16 && acc_f16) reduce_sum_kernel<DT, kAcc16, false><<<grid, kThreads, 0, s>>>(x, out, n, ws, vec_ok);
   else reduce_sum_kernel<DT, false, EXP><<<grid, kThreads, 0, s>>>(x, out, n, ws, vec_ok);
   B200K_CHECK_CUDA(cudaGetLastError());
   return B200K_OK;
