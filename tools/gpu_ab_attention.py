@@ -21,42 +21,11 @@ The first line names the GPU, its power limit and its maximum SM clock, read in 
     python tools/gpu_ab_attention.py [--base-lib PATH] [--rounds 9]
 """
 import argparse
-import contextlib
-import ctypes
 import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-from gpu_perf_hgemm import BASE_LIB, build_base, gpu_info  # noqa: E402
-
-
-def load(path):
-    from b200k import _loader
-
-    lib = ctypes.CDLL(os.path.abspath(path))
-    for name, (res, argtypes) in _loader._SIGS.items():
-        if not hasattr(lib, name):  # an entry point the other build predates; no case here calls it
-            continue
-        fn = getattr(lib, name)
-        fn.restype = res
-        fn.argtypes = argtypes
-    return lib
-
-
-@contextlib.contextmanager
-def using(lib):
-    """b200k.ops calls `lib` inside the block."""
-    from b200k import ops
-
-    saved = ops._lib
-    ops._lib = lib
-    try:
-        yield
-    finally:
-        ops._lib = saved
+from gpu_timing import BASE_LIB, ROOT, build_base, compare_and_time, gpu_info, load_lib
 
 
 def equal_cases(torch, ops):
@@ -268,84 +237,6 @@ def timed_cases(torch, ops):
     return cases
 
 
-def same_bits(a, b):
-    """Same dtype, shape and bytes: a NaN or a -0 counts like any other value."""
-    import torch
-
-    raw = [t.contiguous().reshape(-1).view(torch.uint8) for t in (a, b)]
-    return a.dtype == b.dtype and a.shape == b.shape and torch.equal(*raw)
-
-
-def compare_and_time(torch, libs, cases, timed, rounds, unit=("tflops", 1e-12)):
-    """Runs each (name, run) of `cases` through libs["base"] and libs["new"] and prints the ones whose outputs differ
-    in any bit, then times each (name, work, fn) of `timed` (a rate in `unit` = (name, scale) is work / time * scale).
-    Returns (differing cases, timed cases whose new median lies above the base's maximum)."""
-    bad = 0
-    for name, run in cases:
-        outs = {}
-        for key, lib in libs.items():
-            with using(lib):
-                outs[key] = run()
-        same = len(outs["base"]) == len(outs["new"]) and all(same_bits(a, b) for a, b in zip(outs["base"], outs["new"]))
-        bad += not same
-        if not same:
-            print(json.dumps({"case": name, "bit_equal": False}), flush=True)
-    if cases:
-        print(json.dumps({"equal_cases": len(cases), "differing": bad}), flush=True)
-
-    slow = 0
-    for name, work, fn in timed:
-        graphs, iters = {}, None
-        for key, lib in libs.items():
-            with using(lib):
-                fn()
-                torch.cuda.synchronize()
-                if iters is None:  # about 100 ms of work per build per round
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    for _ in range(3):
-                        fn()
-                    e1.record()
-                    torch.cuda.synchronize()
-                    iters = max(3, min(2000, int(100.0 / (e0.elapsed_time(e1) / 3))))
-                s = torch.cuda.Stream()
-                s.wait_stream(torch.cuda.current_stream())
-                with torch.cuda.stream(s):
-                    fn()  # warm-up on the capture stream
-                torch.cuda.current_stream().wait_stream(s)
-                g = torch.cuda.CUDAGraph()
-                with torch.cuda.graph(g):
-                    for _ in range(iters):
-                        fn()
-                graphs[key] = g
-        for g in graphs.values():
-            g.replay()
-        torch.cuda.synchronize()
-        times = {k: [] for k in graphs}
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        for r in range(rounds):
-            for key in (("base", "new") if r % 2 == 0 else ("new", "base")):
-                e0.record()
-                graphs[key].replay()
-                e1.record()
-                torch.cuda.synchronize()
-                times[key].append(e0.elapsed_time(e1) * 1e3 / iters)
-        med = {k: sorted(v)[len(v) // 2] for k, v in times.items()}
-        inside = min(times["base"]) <= med["new"] <= max(times["base"])
-        slow += med["new"] > max(times["base"])
-        line = {"case": name, "iters_per_round": iters}
-        for k, v in times.items():
-            line[k + "_us"] = round(med[k], 2)
-            line[k + "_min_max_us"] = [round(min(v), 2), round(max(v), 2)]
-            line[k + "_" + unit[0]] = round(work / (med[k] * 1e-6) * unit[1], 1)
-        line["new_over_base"] = round(med["new"] / med["base"], 4)
-        line["new_median_inside_base_range"] = inside
-        print(json.dumps(line), flush=True)
-        del graphs
-        torch.cuda.empty_cache()
-    return bad, slow
-
-
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--build-base", metavar="REV", help="build REV's library into build_ab/base and exit")
@@ -358,12 +249,10 @@ def main():
 
     import torch
 
-    if not torch.cuda.is_available():
-        sys.exit("gpu_ab_attention.py needs a CUDA device")
+    info = gpu_info(torch)
     from b200k import _loader, ops
 
-    libs = {"base": load(args.base_lib), "new": _loader.lib}
-    info = gpu_info(torch)
+    libs = {"base": load_lib(args.base_lib), "new": _loader.lib}
     print(json.dumps(dict(info, base_lib=os.path.relpath(os.path.abspath(args.base_lib), ROOT), rounds=args.rounds)),
           flush=True)
 

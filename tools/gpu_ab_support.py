@@ -1,8 +1,8 @@
 """A/B of the bandwidth kernels against an earlier build of the library, in one process: same bits, then time.
 
-Built like tools/gpu_ab_attention.py and sharing its loader and its compare-and-time loop: the base build's
-libb200k.so is loaded through ctypes next to the one in the tree, and every call goes through b200k.ops, pointed at
-one library or the other.
+Built like tools/gpu_ab_attention.py, on the loader and the compare-and-time loop of tools/gpu_timing.py: the base
+build's libb200k.so is loaded through ctypes next to the one in the tree, and every call goes through b200k.ops, pointed
+at one library or the other.
 
   1. Seeded inputs through both builds; the raw bits of every output must be equal (NaN and -0 count):
      softmax modes 0-3, RMS norm in every acc_f16 / eps_inside_k combination and layer norm with both eps forms, f32
@@ -25,11 +25,7 @@ import json
 import os
 import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-from gpu_ab_attention import compare_and_time, load  # noqa: E402
-from gpu_perf_hgemm import BASE_LIB, build_base, gpu_info  # noqa: E402
+from gpu_timing import BASE_LIB, ROOT, build_base, compare_and_time, gpu_info, load_lib
 
 
 def equal_cases(torch, ops):
@@ -220,12 +216,10 @@ def main():
 
     import torch
 
-    if not torch.cuda.is_available():
-        sys.exit("gpu_ab_support.py needs a CUDA device")
+    info = gpu_info(torch)
     from b200k import _loader, ops
 
-    libs = {"base": load(args.base_lib), "new": _loader.lib}
-    info = gpu_info(torch)
+    libs = {"base": load_lib(args.base_lib), "new": _loader.lib}
     print(json.dumps(dict(info, base_lib=os.path.relpath(os.path.abspath(args.base_lib), ROOT), rounds=args.rounds)),
           flush=True)
     bad, slow = compare_and_time(torch, libs, equal_cases(torch, ops), timed_cases(torch, ops), args.rounds,

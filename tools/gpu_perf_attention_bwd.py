@@ -14,14 +14,8 @@ Prints one JSON object per line.
 """
 import argparse
 import json
-import os
-import statistics
-import sys
 
-ROOT = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(os.path.dirname(ROOT), "cuda-learn-notes_b200"))
-from gpu_perf_hgemm import gpu_info  # noqa: E402
+from gpu_timing import gpu_info, stats, time_rounds
 
 SHAPES = [(4, 48, 8192, 64), (4, 64, 8192, 128), (8, 16, 2048, 128)]
 
@@ -37,7 +31,6 @@ def main():
 
     from b200k import ops
 
-    assert torch.cuda.is_available(), "needs a GPU"
     print(json.dumps(gpu_info(torch)), flush=True)
     for B, H, N, D in SHAPES:
         for causal in (False, True):
@@ -69,37 +62,28 @@ def main():
                         "sdpa_flash_bwd": sdpa_bwd_of(SDPBackend.FLASH_ATTENTION),
                         "sdpa_flash_fwd_bwd": sdpa_fb_of(SDPBackend.FLASH_ATTENTION),
                         "math_fwd_bwd": sdpa_fb_of(SDPBackend.MATH)}
-            times = {name: [] for name in variants}
-            for name, fn in list(variants.items()):  # warm-up; a variant that does not fit is dropped
+            names = list(variants)
+            for name in names:  # a variant that does not fit is dropped
                 try:
-                    fn()
+                    variants[name]()
                     torch.cuda.synchronize()
                 except torch.OutOfMemoryError:
                     del variants[name]
-                    times[name] = None
                     torch.cuda.empty_cache()
-            for _ in range(args.rounds):
-                for name, fn in variants.items():
-                    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-                    e0.record()
-                    for _ in range(args.iters):
-                        fn()
-                    e1.record()
-                    e1.synchronize()
-                    times[name].append(e0.elapsed_time(e1) / args.iters)
+            times = time_rounds(variants, args.iters, args.rounds)
             fwd_flops = 4.0 * B * H * N * N * D / (2 if causal else 1)
             row = {"shape": [B, H, N, D], "causal": causal, "dtype": "f16"}
-            for name, t in times.items():
-                if t is None:
+            for name in names:
+                if name not in times:
                     row[name] = "out of memory"
                     continue
-                med = statistics.median(t)
+                med, lo, hi = (s * 1e3 for s in stats(times[name]))
                 flops = fwd_flops * (2.5 if name.endswith("_bwd") and "fwd" not in name else 3.5)
-                row[name] = {"ms_median": round(med, 3), "ms_min": round(min(t), 3), "ms_max": round(max(t), 3),
+                row[name] = {"ms_median": round(med, 3), "ms_min": round(lo, 3), "ms_max": round(hi, 3),
                              "tflops": round(flops / med / 1e9, 1)}
-            if times["sdpa_flash_bwd"]:
-                row["bwd_ratio_ours_over_flash"] = round(statistics.median(times["ours_bwd"]) /
-                                                         statistics.median(times["sdpa_flash_bwd"]), 2)
+            if "sdpa_flash_bwd" in times:
+                row["bwd_ratio_ours_over_flash"] = round(stats(times["ours_bwd"])[0] /
+                                                         stats(times["sdpa_flash_bwd"])[0], 2)
             print(json.dumps(row), flush=True)
             del q, k, v, do, o, lse, dq, dk, dv, qa, ka, va, variants
             torch.cuda.empty_cache()

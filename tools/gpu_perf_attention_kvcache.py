@@ -16,54 +16,15 @@ split call), not a kernel's share of peak.
 """
 import argparse
 import json
-import os
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.nn.functional as F  # noqa: E402
-from b200k import ops  # noqa: E402
-from gpu_perf_attention_varlen import gpu_info  # noqa: E402
+import numpy as np
+import torch
+import torch.nn.functional as F
+from gpu_timing import gpu_info, stats, time_rounds
+from b200k import ops
 
 PEAK_BYTES_PER_S = 3.35e12
 D = 128
-
-
-def graphed(fn, iters):
-    """A function that replays `iters` captured calls of fn."""
-    fn()   # warm-up outside the capture: tensor maps, shared-memory attribute, backend choice
-    torch.cuda.synchronize()
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(iters):
-            fn()
-    return g.replay
-
-
-def time_alternating(fns, iters, rounds):
-    """Per-call seconds of each function over the rounds; the graphs take turns."""
-    replays = {name: graphed(fn, iters) for name, fn in fns.items()}
-    for r in replays.values():
-        r()
-    torch.cuda.synchronize()
-    times = {name: [] for name in fns}
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(rounds):
-        for name, r in replays.items():
-            e0.record()
-            r()
-            e1.record()
-            torch.cuda.synchronize()
-            times[name].append(e0.elapsed_time(e1) * 1e-3 / iters)
-    return times
 
 
 def splits_of(B, Lq, H, H_kv, cap):
@@ -116,24 +77,25 @@ def run_case(info, args, name, B, Lq, H, H_kv, lens, cap, causal=False, page_siz
     else:
         sdpa_note = "not run: lengths differ from the capacity" if not causal else "not run: causal (SDPA aligns top-left)"
     try:
-        t = time_alternating(fns, args.iters, args.rounds)
+        t = time_rounds(fns, args.iters, args.rounds, graph=True)
     except Exception as e:   # e.g. a comparator that cannot be captured: reported, the case still runs without it
         sdpa_note = "dropped: " + str(e).splitlines()[0][:200]
         fns.pop("sdpa_enable_gqa", None)
-        t = time_alternating(fns, args.iters, args.rounds)
+        t = time_rounds(fns, args.iters, args.rounds, graph=True)
     nbytes = sum(lens) * H_kv * D * 2 * 2 + 2 * B * Lq * H * D * 2
     line = dict(case=name, B=B, Lq=Lq, H=H, H_kv=H_kv, D=D, causal=causal, capacity=cap,
                 lens=lens if len(set(lens)) > 1 and len(lens) <= 16 else None,
                 total_keys=int(sum(lens)), splits=int(splits_of(B, Lq, H, H_kv, cap)), bytes=int(nbytes))
+    med = {}
     for k, ts in t.items():
-        med = float(np.median(ts))
-        line[k + "_us"] = round(med * 1e6, 2)
-        line[k + "_us_min_max"] = [round(min(ts) * 1e6, 2), round(max(ts) * 1e6, 2)]
-        line[k + "_GBps"] = round(nbytes / med * 1e-9, 1)
-        line[k + "_frac_3350GBps"] = round(nbytes / med / PEAK_BYTES_PER_S, 3)
-    line["speed_vs_varlen"] = round(float(np.median(t["varlen"])) / float(np.median(t["kvcache"])), 3)
+        med[k], lo, hi = stats(ts)
+        line[k + "_us"] = round(med[k] * 1e6, 2)
+        line[k + "_us_min_max"] = [round(lo * 1e6, 2), round(hi * 1e6, 2)]
+        line[k + "_GBps"] = round(nbytes / med[k] * 1e-9, 1)
+        line[k + "_frac_3350GBps"] = round(nbytes / med[k] / PEAK_BYTES_PER_S, 3)
+    line["speed_vs_varlen"] = round(med["varlen"] / med["kvcache"], 3)
     if "sdpa_enable_gqa" in t:
-        line["speed_vs_sdpa"] = round(float(np.median(t["sdpa_enable_gqa"])) / float(np.median(t["kvcache"])), 3)
+        line["speed_vs_sdpa"] = round(med["sdpa_enable_gqa"] / med["kvcache"], 3)
     if sdpa_note:
         line["sdpa_note"] = sdpa_note
     # the compared calls compute the same rows (paged: the same bits as contiguous)
@@ -153,9 +115,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=7)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("gpu_perf_attention_kvcache.py needs a CUDA device")
-    info = gpu_info()
+    info = gpu_info(torch)
     for B in (1, 8, 64):
         for L in (1024, 8192, 32768):
             run_case(info, args, "1_decode_gqa4", B, 1, 32, 8, [L] * B, L, seed=B + L)

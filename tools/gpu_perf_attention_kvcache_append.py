@@ -1,7 +1,7 @@
 """KV-cache decode with append and rotary (ops.fa2_fwd_kvcache with k / v / rotary) against what a caller runs without
 it, one JSON line per case.  D = 128, fp16, H = 32, H_kv = 8, L_new = Lq = 1, NeoX rotary over all 128 columns unless
-stated.  Three calls, each captured `--iters` times into one CUDA graph (graphed / time_alternating of
-gpu_perf_attention_kvcache.py), alternate in this process for `--rounds` rounds:
+stated.  Three calls, each captured `--iters` times into one CUDA graph (time_rounds of gpu_timing.py), alternate
+in this process for `--rounds` rounds:
 
     append  the new call: rows appended and rotated, then the decode
     floor   fa2_fwd_kvcache alone on a cache that already holds the new tokens
@@ -16,17 +16,10 @@ check, not timed), and the GPU's name and power limit read in the same run.
 """
 import argparse
 import json
-import os
-import sys
 
-ROOT = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, os.path.join(os.path.dirname(ROOT), "cuda-learn-notes_b200"))
-sys.path.insert(0, ROOT)
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-from b200k import ops  # noqa: E402
-from gpu_perf_attention_kvcache import time_alternating  # noqa: E402
-from gpu_perf_attention_varlen import gpu_info  # noqa: E402
+import torch
+from gpu_timing import gpu_info, stats, time_rounds
+from b200k import ops
 
 D, H, H_KV = 128, 32, 8
 
@@ -89,14 +82,14 @@ def run_case(info, args, name, B, cap, Lq=1, causal=False, ps=None, seed=0):
         vt[pg, slot] = vn
         ops.fa2_fwd_kvcache(qr, kt, vt, o, lens + L_new, table, causal=causal)
 
-    t = time_alternating({"append": append, "floor": floor, "today": today}, args.iters, args.rounds)
+    t = time_rounds({"append": append, "floor": floor, "today": today}, args.iters, args.rounds, graph=True)
     line = dict(case=name, B=B, Lq=Lq, L_new=L_new, H=H, H_kv=H_KV, D=D, causal=causal, capacity=cap,
                 page_size=ps, rotary="neox 128")
     med = {}
     for k, ts in t.items():
-        med[k] = float(np.median(ts))
+        med[k], lo, hi = stats(ts)
         line[k + "_us"] = round(med[k] * 1e6, 2)
-        line[k + "_us_min_max"] = [round(min(ts) * 1e6, 2), round(max(ts) * 1e6, 2)]
+        line[k + "_us_min_max"] = [round(lo * 1e6, 2), round(hi * 1e6, 2)]
     line["append_minus_floor_us"] = round((med["append"] - med["floor"]) * 1e6, 2)
     line["speed_vs_today"] = round(med["today"] / med["append"], 3)
     # without rotary: append and the torch scatter + decode give the same bits
@@ -117,9 +110,7 @@ def main():
     ap.add_argument("--iters", type=int, default=20)
     ap.add_argument("--rounds", type=int, default=7)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("gpu_perf_attention_kvcache_append.py needs a CUDA device")
-    info = gpu_info()
+    info = gpu_info(torch)
     for B in (1, 8, 64):
         for cap in (1024, 8192, 32768):
             run_case(info, args, "decode", B, cap, seed=B + cap)

@@ -16,17 +16,11 @@ Q and O.  `speedup` is the 16-bit median over the fp8 median; the bound from hal
 """
 import argparse
 import json
-import os
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-from b200k import ops  # noqa: E402
-from gpu_perf_attention_kvcache import time_alternating  # noqa: E402
-from gpu_perf_attention_varlen import gpu_info  # noqa: E402
+import numpy as np
+import torch
+from gpu_timing import gpu_info, stats, time_rounds
+from b200k import ops
 
 D, H, H_KV = 128, 32, 8
 FMTS = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
@@ -34,12 +28,13 @@ FMTS = {"e4m3": torch.float8_e4m3fn, "e5m2": torch.float8_e5m2}
 
 def report(info, args, name, t, bytes16, bytes8, extra):
     line = dict(case=name, fmt=args.fmt, **extra)
-    for k, ts, nb in (("fp8", t["fp8"], bytes8), ("f16", t["f16"], bytes16)):
-        med = float(np.median(ts))
-        line[k + "_us"] = round(med * 1e6, 2)
-        line[k + "_us_min_max"] = [round(min(ts) * 1e6, 2), round(max(ts) * 1e6, 2)]
-        line[k + "_GBps"] = round(nb / med * 1e-9, 1)
-    line["speedup"] = round(float(np.median(t["f16"])) / float(np.median(t["fp8"])), 3)
+    med = {}
+    for k, nb in (("fp8", bytes8), ("f16", bytes16)):
+        med[k], lo, hi = stats(t[k])
+        line[k + "_us"] = round(med[k] * 1e6, 2)
+        line[k + "_us_min_max"] = [round(lo * 1e6, 2), round(hi * 1e6, 2)]
+        line[k + "_GBps"] = round(nb / med[k] * 1e-9, 1)
+    line["speedup"] = round(med["f16"] / med["fp8"], 3)
     line.update(info)
     print(json.dumps(line), flush=True)
 
@@ -82,7 +77,7 @@ def decode_case(info, args, name, B, lens, cap, page_size=None, append=False):
     fns = {"fp8": lambda: ops.fa2_fwd_kvcache(q, k8, v8, o8, sl, table if page_size else None, k_scale=ks, v_scale=vs,
                                               **kw),
            "f16": lambda: ops.fa2_fwd_kvcache(q, k16, v16, o16, sl, table if page_size else None, **kw)}
-    t = time_alternating(fns, args.iters, args.rounds)
+    t = time_rounds(fns, args.iters, args.rounds, graph=True)
     keys = int(sum(lens))
     qo = 2 * B * H * D * 2
     report(info, args, name, t, keys * H_KV * D * 2 * 2 + qo, keys * H_KV * D * 2 + qo,
@@ -107,7 +102,7 @@ def prefill_case(info, args, name, Lq, Lk, ps=256):
     o8, o16 = torch.empty_like(q), torch.empty_like(q)
     fns = {"fp8": lambda: ops.fa2_fwd_varlen(q, k8, v8, o8, cu_q, cu_k, max(Lq), causal=True, block_table=table),
            "f16": lambda: ops.fa2_fwd_varlen(q, k16, v16, o16, cu_q, cu_k, max(Lq), causal=True, block_table=table)}
-    t = time_alternating(fns, args.iters, args.rounds)
+    t = time_rounds(fns, args.iters, args.rounds, graph=True)
     keys = int(sum(Lk))
     qo = 2 * sum(Lq) * H * D * 2
     report(info, args, name, t, keys * H_KV * D * 2 * 2 + qo, keys * H_KV * D * 2 + qo,
@@ -121,8 +116,7 @@ def main():
     ap.add_argument("--fmt", choices=sorted(FMTS), default="e4m3")
     ap.add_argument("--only", default="", help="comma list of case names to run (default: all)")
     args = ap.parse_args()
-    assert torch.cuda.is_available(), "this tool measures the GPU; there is no CPU figure to give"
-    info = gpu_info()
+    info = gpu_info(torch)
     for B in (1, 8, 64):
         for keys in (1024, 8192, 32768):
             decode_case(info, args, "decode_B%d_%dk" % (B, keys // 1024), B, [keys] * B, keys)

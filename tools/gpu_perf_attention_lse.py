@@ -17,49 +17,13 @@ maximum SM clock, read in the same run.  Prints one JSON object per line.
 """
 import argparse
 import json
-import os
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-from gpu_perf_hgemm import gpu_info  # noqa: E402
+from gpu_timing import gpu_info, stats, time_rounds
 
 
-def graph_of(torch, fn, iters):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        for _ in range(iters):
-            fn()
-    return g
-
-
-def compare(torch, variants, rounds, iters):
-    """{name: [us per call per round]} with the variants alternating inside each round."""
-    graphs = {name: graph_of(torch, fn, iters) for name, fn in variants.items()}
-    for g in graphs.values():
-        g.replay()
-    torch.cuda.synchronize()
-    times = {name: [] for name in variants}
-    for _ in range(rounds):
-        for name, g in graphs.items():
-            a, b = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            a.record()
-            g.replay()
-            b.record()
-            b.synchronize()
-            times[name].append(a.elapsed_time(b) * 1000.0 / iters)
-    return times
-
-
-def stats(xs):
-    xs = sorted(xs)
-    return {"median_us": round(xs[len(xs) // 2], 2), "min_us": round(xs[0], 2), "max_us": round(xs[-1], 2)}
+def us(samples):
+    med, lo, hi = stats(samples)
+    return {"median_us": round(med * 1e6, 2), "min_us": round(lo * 1e6, 2), "max_us": round(hi * 1e6, 2)}
 
 
 def main():
@@ -80,7 +44,7 @@ def main():
 
     def report(section, name, times, **extra):
         line = {"section": section, "case": name}
-        line.update({k: stats(v) for k, v in times.items()})
+        line.update({k: us(v) for k, v in times.items()})
         line.update(extra)
         print(json.dumps(line), flush=True)
 
@@ -88,17 +52,17 @@ def main():
     for B, H, N, D in ((4, 48, 8192, 64), (4, 64, 8192, 128)):
         q, k, v = [rn(B, H, N, D) for _ in range(3)]
         o, lse = torch.empty_like(q), torch.empty(B, H, N, device=dev)
-        t = compare(torch, {"without": lambda: ops.fa2_fwd(q, k, v, o), "with": lambda: ops.fa2_fwd(q, k, v, o, lse=lse)},
-                    args.rounds, max(1, args.iters // 4))
+        t = time_rounds({"without": lambda: ops.fa2_fwd(q, k, v, o), "with": lambda: ops.fa2_fwd(q, k, v, o, lse=lse)},
+                        max(1, args.iters // 4), args.rounds, graph=True)
         report("a", "dense B%d H%d N%d D%d" % (B, H, N, D), t)
         del q, k, v, o, lse
     T, H, H_kv, D = 4 * 8192, 64, 8, 128
     cu = torch.arange(5, dtype=torch.int32, device=dev) * 8192
     q, k, v = rn(T, H, D), rn(T, H_kv, D), rn(T, H_kv, D)
     o, lse = torch.empty_like(q), torch.empty(T, H, device=dev)
-    t = compare(torch, {"without": lambda: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, 8192, causal=True),
-                        "with": lambda: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, 8192, causal=True, lse=lse)},
-                args.rounds, max(1, args.iters // 4))
+    t = time_rounds({"without": lambda: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, 8192, causal=True),
+                     "with": lambda: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, 8192, causal=True, lse=lse)},
+                    max(1, args.iters // 4), args.rounds, graph=True)
     report("a", "packed GQA 4x8192 H64 Hkv8 D128 causal", t)
     del q, k, v, o, lse
     for B in (1, 64):
@@ -107,8 +71,9 @@ def main():
         kc, vc = rn(B, S, H_kv, D), rn(B, S, H_kv, D)
         lens = torch.full((B,), S, dtype=torch.int32, device=dev)
         o, lse = torch.empty_like(q), torch.empty(B, 1, H, device=dev)
-        t = compare(torch, {"without": lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens),
-                            "with": lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens, lse=lse)}, args.rounds, args.iters)
+        t = time_rounds({"without": lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens),
+                         "with": lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens, lse=lse)}, args.iters, args.rounds,
+                        graph=True)
         report("a", "decode B%d 8K cache H32 Hkv8 D128 (%s)" % (B, "split" if ops.fa2_fwd_kvcache_workspace_bytes(
             B, 1, H, H_kv, D, S) else "unsplit"), t)
         del q, kc, vc, o, lse
@@ -128,10 +93,10 @@ def main():
                 o.copy_(x.half())
                 lse.copy_(m + torch.log(w.sum(0)))
 
-            t = compare(torch, {"attn_merge": lambda: ops.attn_merge(parts, lps, o, lse), "torch": composed},
-                        args.rounds, args.iters)
+            t = time_rounds({"attn_merge": lambda: ops.attn_merge(parts, lps, o, lse), "torch": composed},
+                            args.iters, args.rounds, graph=True)
             nbytes = (S + 1) * rows * D * 2 + (S + 1) * rows * 4
-            gbs = {name: round(nbytes / (stats(v)["median_us"] * 1e3), 1) for name, v in t.items()}
+            gbs = {name: round(nbytes / (us(v)["median_us"] * 1e3), 1) for name, v in t.items()}
             report("b", "merge S%d rows%d D%d" % (S, rows, D), t, bytes=nbytes, gb_per_s=gbs,
                    share_of_3350_gbs=round(gbs["attn_merge"] / 3350.0, 3))
             del parts, lps, o, lse
@@ -156,8 +121,8 @@ def main():
     fv = torch.cat([vp.expand(B, P, H_kv, D), vs], 1).contiguous()
     flens = lens + P
     of = torch.empty_like(q)
-    t = compare(torch, {"cascade": cascade, "full_copies": lambda: ops.fa2_fwd_kvcache(q, fk, fv, of, flens)},
-                args.rounds, args.iters)
+    t = time_rounds({"cascade": cascade, "full_copies": lambda: ops.fa2_fwd_kvcache(q, fk, fv, of, flens)},
+                    args.iters, args.rounds, graph=True)
     cascade()
     ops.fa2_fwd_kvcache(q, fk, fv, of, flens)
     torch.cuda.synchronize()

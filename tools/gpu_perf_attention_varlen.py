@@ -12,56 +12,12 @@ the rounds).  Every line carries the GPU's name and power limit, read in the sam
 """
 import argparse
 import json
-import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-import torch.nn.functional as F  # noqa: E402
-from b200k import ops  # noqa: E402
-
-
-def gpu_info():
-    """Name and power limit of cuda:0 (read-only nvidia-smi query)."""
-    info = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": None}
-    try:
-        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits", "-i",
-                              str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout
-        name, power = [s.strip() for s in out.strip().splitlines()[0].split(",")]
-        info.update(gpu=name, power_limit_w=float(power))
-    except Exception as e:  # the name from torch stays; the missing power limit is reported as such
-        info["power_limit_error"] = str(e)[:200]
-    return info
-
-
-def visible_pairs(lq, lk, causal):
-    """(query row, key) pairs the attention computes: Lq * Lk, or with the bottom-right causal mask
-    sum over rows r of clamp(r + Lk - Lq + 1, 0, Lk)."""
-    if not causal:
-        return int(lq) * int(lk)
-    r = np.arange(int(lq), dtype=np.int64)
-    return int(np.clip(r + int(lk) - int(lq) + 1, 0, int(lk)).sum())
-
-
-def time_alternating(fns, iters, rounds):
-    """Median seconds per call of each function; the functions take turns, `iters` calls per turn."""
-    for fn in fns.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {name: [] for name in fns}
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(rounds):
-        for name, fn in fns.items():
-            e0.record()
-            for _ in range(iters):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            times[name].append(e0.elapsed_time(e1) * 1e-3 / iters)
-    return {name: float(np.median(t)) for name, t in times.items()}
+import numpy as np
+import torch
+import torch.nn.functional as F
+from gpu_timing import gpu_info, stats, time_rounds, visible_pairs
+from b200k import ops
 
 
 def emit(info, **kw):
@@ -76,10 +32,10 @@ def case_equal_lengths(info, args):
         o, po = torch.empty_like(q), torch.empty_like(pq)
         cu = torch.arange(0, (B + 1) * N, N, dtype=torch.int32, device="cuda")
         for causal in (False, True):
-            t = time_alternating({
+            t = {name: stats(ts)[0] for name, ts in time_rounds({
                 "dense": lambda: ops.fa2_fwd(q, k, v, o, causal=causal),
                 "varlen": lambda: ops.fa2_fwd_varlen(pq, pk, pv, po, cu, cu, N, causal=causal),
-            }, args.iters, args.rounds)
+            }, args.iters, args.rounds).items()}
             flop = 4 * H * D * B * visible_pairs(N, N, causal)
             same = torch.equal(po.view(B, N, H, D).transpose(1, 2), o)
             emit(info, case="1_equal_lengths_mha", shape=[B, H, N, D], causal=causal, dense_ms=round(t["dense"] * 1e3, 3),
@@ -117,7 +73,7 @@ def case_gqa(info, args):
             fns["sdpa_enable_gqa"] = sdpa
         except Exception as e:  # no fused backend takes this call: reported, never replaced by the math backend
             sdpa_error = str(e).splitlines()[0][:200]
-        t = time_alternating(fns, args.iters, args.rounds)
+        t = {name: stats(ts)[0] for name, ts in time_rounds(fns, args.iters, args.rounds).items()}
         flop = 4 * H * D * B * visible_pairs(N, N, causal)
         line = dict(case="2_gqa", B=B, N=N, H=H, H_kv=H_kv, D=D, causal=causal,
                     same_bits_as_repeated_kv=bool(torch.equal(o, o_rep)))
@@ -153,10 +109,10 @@ def case_mixed_lengths(info, args):
     op = torch.empty_like(pad[0])
     sl = torch.tensor(lens, dtype=torch.int32, device="cuda")
     for causal in (False, True):
-        t = time_alternating({
+        t = {name: stats(ts)[0] for name, ts in time_rounds({
             "padded_dense": lambda: ops.fa2_fwd(pad[0], pad[1], pad[2], op, causal=causal, seqlens_k=sl),
             "varlen": lambda: ops.fa2_fwd_varlen(q, k, v, o, cu, cu, N, causal=causal),
-        }, args.iters, args.rounds)
+        }, args.iters, args.rounds).items()}
         useful = 4 * H * D * sum(visible_pairs(L, L, causal) for L in lens)
         emit(info, case="3_mixed_lengths", nseq=nseq, H=H, D=D, total_tokens=total, max_len=N, causal=causal,
              padded_dense_ms=round(t["padded_dense"] * 1e3, 3), varlen_ms=round(t["varlen"] * 1e3, 3),
@@ -170,9 +126,7 @@ def main():
     ap.add_argument("--iters", type=int, default=10)
     ap.add_argument("--rounds", type=int, default=3)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("gpu_perf_attention_varlen.py needs a CUDA device")
-    info = gpu_info()
+    info = gpu_info(torch)
     case_equal_lengths(info, args)
     case_gqa(info, args)
     case_mixed_lengths(info, args)

@@ -18,31 +18,8 @@ the same run.  Prints one JSON object per line.
 """
 import argparse
 import json
-import os
-import statistics
-import sys
 
-ROOT = os.path.dirname(os.path.abspath(__file__))
-sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(os.path.dirname(ROOT), "cuda-learn-notes_b200"))
-from gpu_perf_hgemm import gpu_info  # noqa: E402
-
-
-def _time(torch, variants, rounds, iters):
-    for fn in variants.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {n: [] for n in variants}
-    for _ in range(rounds):
-        for n, fn in variants.items():
-            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-            e0.record()
-            for _ in range(iters):
-                fn()
-            e1.record()
-            e1.synchronize()
-            times[n].append(e0.elapsed_time(e1) / iters)
-    return times
+from gpu_timing import gpu_info, stats, time_rounds
 
 
 def main():
@@ -55,7 +32,6 @@ def main():
 
     from b200k import ops
 
-    assert torch.cuda.is_available(), "needs a GPU"
     print(json.dumps(gpu_info(torch)), flush=True)
     dev, h = "cuda", torch.half
 
@@ -81,8 +57,8 @@ def main():
         row = {"case": case, "causal": causal, "dtype": "f16"}
         useful = flops(lens, H, D, causal)
         for n, t in times.items():
-            med = statistics.median(t)
-            row[n] = {"ms_median": round(med, 3), "ms_min": round(min(t), 3), "ms_max": round(max(t), 3),
+            med, lo, hi = (s * 1e3 for s in stats(t))
+            row[n] = {"ms_median": round(med, 3), "ms_min": round(lo, 3), "ms_max": round(hi, 3),
                       "useful_tflops": round(useful / med / 1e9, 1)}
         row.update(extra or {})
         print(json.dumps(row), flush=True)
@@ -96,7 +72,7 @@ def main():
             lsed = lse.view(B, N, H).transpose(1, 2).contiguous()
             dd = [torch.empty_like(qd) for _ in range(3)]
             dense = lambda: ops.fa2_bwd(qd, kd, vd, od, lsed, dod, *dd, causal=causal)  # noqa: E731
-            times = _time(torch, {"packed": ours, "dense": dense}, args.rounds, args.iters)
+            times = time_rounds({"packed": ours, "dense": dense}, args.iters, args.rounds)
             same = all(torch.equal(a.view(torch.int16), dn(b).view(torch.int16)) for a, b in zip(dd, outs))
             report("mha %dx%dx%dx%d" % (B, H, N, D), [N] * B, H, D, causal, times, {"same_bits_as_dense": same})
             del q, k, v, o, lse, do, outs, qd, kd, vd, od, dod, lsed, dd
@@ -118,8 +94,8 @@ def main():
         out = F.scaled_dot_product_attention(qa, ka, va, is_causal=causal, enable_gqa=True)
         backend = out.grad_fn.name()
         sd = lambda: torch.autograd.grad(out, (qa, ka, va), dod, retain_graph=True)  # noqa: E731
-        times = _time(torch, {"packed": ours, "repeat_interleave_fa2_bwd_sum": expand, "sdpa_gqa": sd},
-                      args.rounds, args.iters)
+        times = time_rounds({"packed": ours, "repeat_interleave_fa2_bwd_sum": expand, "sdpa_gqa": sd},
+                            args.iters, args.rounds)
         report("gqa %dx%dx%d H_kv=%d" % (B, H, N, H_kv), [N] * B, H, D, causal, times, {"sdpa_backend": backend})
         del q, k, v, o, lse, do, outs, qd, od, dod, lsed, dd, qa, ka, va, out
         torch.cuda.empty_cache()
@@ -136,13 +112,13 @@ def main():
         ops.fa2_fwd(qp, kp, vp, op, causal=causal, seqlens_k=sl, lse=lsep)
         dp = [torch.empty_like(qp) for _ in range(3)]
         padded = lambda: ops.fa2_bwd(qp, kp, vp, op, lsep, dop, *dp, causal=causal, seqlens_k=sl)  # noqa: E731
-        times = _time(torch, {"packed": ours, "padded_fa2_bwd": padded}, args.rounds, args.iters)
+        times = time_rounds({"packed": ours, "padded_fa2_bwd": padded}, args.iters, args.rounds)
         report("mixed 64 seqs [128, 8192] H=32 D=128", lens, H, D, causal, times, {"tokens": sum(lens), "padded_to": Nmax})
         del q, k, v, o, lse, do, outs, qp, kp, vp, dop, op, lsep, dp
         torch.cuda.empty_cache()
         # 4. MQA, low parallelism
         (q, k, v, o, lse, do, cu), outs, ours = packed([4096], 32, 1, 128, causal)
-        times = _time(torch, {"packed": ours}, args.rounds, args.iters)
+        times = time_rounds({"packed": ours}, args.iters, args.rounds)
         report("mqa 1x32x4096 H_kv=1", [4096], 32, 128, causal, times, {"dkdv_ctas": 4096 // 64})
         del q, k, v, o, lse, do, outs
         torch.cuda.empty_cache()

@@ -14,37 +14,15 @@ work, 4 * H * D per visible (query row, key) pair, as gpu_perf_attention_varlen.
     python tools/gpu_perf_attention_varlen_paged.py [--iters 5] [--rounds 7]
 """
 import argparse
-import os
-import sys
+import json
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "tools"))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-from b200k import ops  # noqa: E402
-from gpu_perf_attention_varlen import emit, gpu_info, visible_pairs  # noqa: E402
+import numpy as np
+import torch
+from gpu_timing import gpu_info, stats, time_rounds, visible_pairs
+from b200k import ops
 
 H, H_KV, D = 32, 8, 128
 PAGE_SIZES = (16, 64, 256)
-
-
-def time_alternating(fns, iters, rounds):
-    """(median, min, max) seconds per call of each function; the functions take turns, `iters` calls per turn."""
-    for fn in fns.values():
-        fn()
-    torch.cuda.synchronize()
-    times = {name: [] for name in fns}
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    for _ in range(rounds):
-        for name, fn in fns.items():
-            e0.record()
-            for _ in range(iters):
-                fn()
-            e1.record()
-            torch.cuda.synchronize()
-            times[name].append(e0.elapsed_time(e1) * 1e-3 / iters)
-    return {name: (float(np.median(t)), float(min(t)), float(max(t))) for name, t in times.items()}
 
 
 def paged_cache(k, v, lens, page_size, seed):
@@ -80,7 +58,7 @@ def line(info, case, t, useful, **kw):
     for name in t:
         if name != "paged":
             out["paged_speed_vs_" + name] = round(t[name][0] / t["paged"][0], 3)
-    emit(info, **out)
+    print(json.dumps(dict(out, **info)), flush=True)
 
 
 def run_case(info, args, case, lq, lk, seed, with_kvcache=False):
@@ -111,7 +89,7 @@ def run_case(info, args, case, lq, lk, seed, with_kvcache=False):
             q4, o4 = q.view(B, Lq, H, D), torch.empty(B, Lq, H, D, dtype=torch.half, device="cuda")
             lens = torch.tensor(lk, dtype=torch.int32, device="cuda")
             fns["kvcache"] = lambda: ops.fa2_fwd_kvcache(q4, kc, vc, o4, lens, table, causal=True)
-        t = time_alternating(fns, args.iters, args.rounds)
+        t = {name: stats(ts) for name, ts in time_rounds(fns, args.iters, args.rounds).items()}
         ops.fa2_fwd_varlen(q, k, v, o_ref, cq, ck, max_q, causal=True)
         ops.fa2_fwd_varlen(q, kc, vc, o, cq, ck, max_q, causal=True, block_table=table)
         line(info, case, t, useful, page_size=ps, B=len(lq), total_q=int(sum(lq)), total_k=int(sum(lk)), H=H,
@@ -125,9 +103,7 @@ def main():
     ap.add_argument("--iters", type=int, default=5)
     ap.add_argument("--rounds", type=int, default=7)
     args = ap.parse_args()
-    if not torch.cuda.is_available():
-        sys.exit("gpu_perf_attention_varlen_paged.py needs a CUDA device")
-    info = gpu_info()
+    info = gpu_info(torch)
     lens = np.random.RandomState(2024).randint(128, 8192 + 1, size=64)
     run_case(info, args, "1_mixed_prompts", lens, lens, seed=1)
     for cached in (8192, 32768):

@@ -1,36 +1,23 @@
-"""Achieved HBM bandwidth of the support kernels (algorithmic bytes / CUDA-event time), one JSON line per kernel.
-Inputs are larger than the 50 MB L2 or rotated over several buffers, so every launch streams from HBM.
+"""Achieved HBM bandwidth of the support kernels (algorithmic bytes / CUDA-event time), one JSON line per kernel after
+a first line that names the GPU, its power limit and its maximum SM clock, read in the same run.  Inputs are larger
+than the 50 MB L2 or rotated over several buffers, so every launch streams from HBM.
 
     python tools/gpu_perf_support.py [--iters 20]
 """
 import argparse
 import json
 import os
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "cuda-learn-notes_b200"))
-import torch  # noqa: E402
-from b200k import ops  # noqa: E402
-
-
-def timeit(fn, iters):
-    for _ in range(3):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(iters):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / iters * 1e-3
+import torch
+from gpu_timing import ROOT, gpu_info, time_rounds
+from b200k import ops
 
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--iters", type=int, default=20)
     args = ap.parse_args()
+    print(json.dumps(gpu_info(torch)), flush=True)
     peak = None
     try:
         peak = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))).get("hbm_gbs")
@@ -89,7 +76,7 @@ def main():
         ("hgemv_32768x8192", lambda: ops.gemv(x16, gx16, gy16), x16.numel() * 2),
     ]
     for name, fn, nbytes in cases:
-        t = timeit(fn, args.iters)
+        t = time_rounds({name: fn}, args.iters, 1)[name][0]
         out = {"kernel": name, "us": round(t * 1e6, 1), "algorithmic_bytes": nbytes, "gbps": round(nbytes / t * 1e-9, 1)}
         if peak:
             out["frac_of_measured_hbm_peak"] = round(out["gbps"] / peak, 3)
