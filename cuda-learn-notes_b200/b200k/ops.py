@@ -188,18 +188,9 @@ def fa2_fwd(q, k, v, o, scale: Optional[float] = None, v_is_dn: bool = False, va
         if seqlens_k.numel() != B:
             raise RuntimeError("Tensor size mismatch!")
         sl = seqlens_k.data_ptr()
-    if lse is not None:
-        with _DeviceGuard(q):
-            L.check(_lib.b200k_fa2_fwd_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), B, H,
-                                           N, D, float(scale) if scale else 0.0, 1 if v_is_dn else 0, _DTYPE_ENUM[dt],
-                                           1 if causal else 0, sl, variant, _stream(q)))
-        return
     with _DeviceGuard(q):
-        if dt == torch.float16 and not causal and seqlens_k is None:
-            L.check(_lib.b200k_fa2_fwd_f16(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, H, N, D,
-                                           float(scale) if scale else 0.0, 1 if v_is_dn else 0, variant, _stream(q)))
-        else:
-            L.check(_lib.b200k_fa2_fwd(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), B, H, N, D,
+        L.check(_lib.b200k_fa2_fwd_lse(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(),
+                                       lse.data_ptr() if lse is not None else None, B, H, N, D,
                                        float(scale) if scale else 0.0, 1 if v_is_dn else 0, _DTYPE_ENUM[dt],
                                        1 if causal else 0, sl, variant, _stream(q)))
 
@@ -227,17 +218,15 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
     FP8 pages: with a ``block_table``, k and v may be ``torch.float8_e4m3fn`` or ``torch.float8_e5m2`` caches (one dtype
     for both), dequantized as fp8 * ``k_scale`` / ``v_scale`` (fp32 [H_kv] device tensors, or None for 1.0); see
     :func:`fa2_fwd_kvcache`.  o and lse then have the bits of the call on the gathered, dequantized K / V."""
-    if _fp8_kv(k, v, k_scale, v_scale):
-        if block_table is None:
-            raise RuntimeError("b200k: fp8 K / V are read from paged caches: pass block_table")
-        _fa2_fwd_varlen_paged_fp8(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse, block_table,
-                                  k_scale, v_scale)
-        return
+    fp8 = _fp8_kv(k, v, k_scale, v_scale)
+    if fp8 and block_table is None:
+        raise RuntimeError("b200k: fp8 K / V are read from paged caches: pass block_table")
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
-    for t in (q, k, v, o):
+    for t in (q, o) if fp8 else (q, k, v, o):
         _check_dtype(t, dt)
     if block_table is not None:
-        _fa2_fwd_varlen_paged(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse, block_table, dt)
+        _fa2_fwd_varlen_paged(q, k, v, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse, block_table, dt,
+                              fp8, k_scale, v_scale)
         return
     if q.dim() != 3 or k.dim() != 3:
         raise RuntimeError("Tensor size mismatch!")
@@ -257,22 +246,17 @@ def fa2_fwd_varlen(q, k, v, o, cu_seqlens_q: torch.Tensor, cu_seqlens_k: torch.T
     if lse is not None:
         _check_lse(lse, o)
     _check_cuda_contig(q, k, v, o, cu_seqlens_q, cu_seqlens_k)
-    if lse is not None:
-        with _DeviceGuard(q):
-            L.check(_lib.b200k_fa2_fwd_varlen_lse(
-                q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr(), cu_seqlens_q.data_ptr(),
-                cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
-                float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
-        return
     with _DeviceGuard(q):
-        L.check(_lib.b200k_fa2_fwd_varlen(q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), cu_seqlens_q.data_ptr(),
-                                          cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
-                                          float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
+        L.check(_lib.b200k_fa2_fwd_varlen_lse(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
+            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), B, int(max_seqlen_q), total_q, total_k, H, H_kv, D,
+            float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
 
 
-def _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, lse, block_table):
-    """The shape checks of :func:`fa2_fwd_varlen` with ``block_table``, for caches of either dtype; returns
-    (B, total_q, H, H_kv, D, num_pages, page_size)."""
+def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
+                          block_table, dt, fp8, k_scale, v_scale) -> None:
+    """:func:`fa2_fwd_varlen` with ``block_table``: the shape checks of the paged layout, for caches of either dtype,
+    then b200k_fa2_varlen_paged, or b200k_fa2_varlen_paged_fp8 over fp8 pages."""
     if q.dim() != 3 or k_cache.dim() != 4:
         raise RuntimeError("Tensor size mismatch!")
     total_q, H, D = q.shape
@@ -295,20 +279,16 @@ def _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, lse, block
     if lse is not None:
         _check_lse(lse, o)
     _check_cuda_contig(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, block_table)
-    return B, total_q, H, H_kv, D, num_pages, page_size
-
-
-def _fa2_fwd_varlen_paged(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
-                          block_table, dt) -> None:
-    """:func:`fa2_fwd_varlen` with ``block_table``: the shape checks of the paged layout, then the C call."""
-    B, total_q, H, H_kv, D, num_pages, page_size = _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k,
-                                                                 lse, block_table)
+    ks, vs = _fp8_scales(k_scale, v_scale, H_kv) if fp8 else (None, None)
+    ptrs = (q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
+            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr())
+    shapes = (B, int(max_seqlen_q), total_q, H, H_kv, D, num_pages, page_size, block_table.size(1),
+              float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q))
     with _DeviceGuard(q):
-        L.check(_lib.b200k_fa2_varlen_paged(
-            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
-            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr(), B, int(max_seqlen_q), total_q, H,
-            H_kv, D, num_pages, page_size, block_table.size(1), float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
-            1 if causal else 0, _stream(q)))
+        if fp8:
+            L.check(_lib.b200k_fa2_varlen_paged_fp8(*ptrs, ks, vs, _DTYPE_ENUM[k_cache.dtype], *shapes))
+        else:
+            L.check(_lib.b200k_fa2_varlen_paged(*ptrs, *shapes))
 
 
 _FP8_KV = tuple(d for d in (getattr(torch, "float8_e4m3fn", None), getattr(torch, "float8_e5m2", None)) if d is not None)
@@ -338,23 +318,6 @@ def _fp8_scales(k_scale, v_scale, H_kv: int) -> list:
         _check_cuda_contig(t)
         ptrs.append(t.data_ptr())
     return ptrs
-
-
-def _fa2_fwd_varlen_paged_fp8(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k, max_seqlen_q, scale, causal, lse,
-                              block_table, k_scale, v_scale) -> None:
-    """:func:`fa2_fwd_varlen` over fp8 pages: the checks of the 16-bit paged call, then b200k_fa2_varlen_paged_fp8."""
-    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
-    _check_dtype(q, dt)
-    _check_dtype(o, dt)
-    B, total_q, H, H_kv, D, num_pages, page_size = _paged_checks(q, k_cache, v_cache, o, cu_seqlens_q, cu_seqlens_k,
-                                                                 lse, block_table)
-    ks, vs = _fp8_scales(k_scale, v_scale, H_kv)
-    with _DeviceGuard(q):
-        L.check(_lib.b200k_fa2_varlen_paged_fp8(
-            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
-            cu_seqlens_q.data_ptr(), cu_seqlens_k.data_ptr(), block_table.data_ptr(), ks, vs, _DTYPE_ENUM[k_cache.dtype],
-            B, int(max_seqlen_q), total_q, H, H_kv, D, num_pages, page_size, block_table.size(1),
-            float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, _stream(q)))
 
 
 def fa2_fwd_kvcache_fp8_workspace_bytes(B: int, Lq: int, H: int, H_kv: int, D: int, max_seqlen_k: int,
@@ -470,63 +433,36 @@ def fa2_fwd_kvcache(q, k_cache, v_cache, o, cache_seqlens: torch.Tensor, block_t
     satfinite(float(x) / scale[h]) in the cache's format, after rotary.  With no scales, o and lse have the bits of the
     16-bit call on the dequantized caches; with power-of-two scales too, as long as the dequantized values are normal
     in q's dtype.  A scale with 16-bit caches, or caches of two dtypes, is a RuntimeError."""
-    if _fp8_kv(k_cache, v_cache, k_scale, v_scale):
-        _fa2_fwd_kvcache_fp8(q, k_cache, v_cache, o, cache_seqlens, block_table, scale, causal, k, v, rotary_cos,
-                             rotary_sin, rotary_interleaved, lse, k_scale, v_scale)
-        return
+    fp8 = _fp8_kv(k_cache, v_cache, k_scale, v_scale)
     dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
     B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary = _kvcache_checks(
-        q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin, dt)
-    if append:
-        cos, sin = rotary_cos, rotary_sin
-        with _DeviceGuard(q):
-            nbytes = fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, rotary)
-            ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device)
-            args = (cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None,
-                    k.data_ptr(), v.data_ptr(), k.size(1), cos.data_ptr() if rotary else None,
-                    sin.data_ptr() if rotary else None, cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0,
-                    1 if rotary_interleaved else 0, B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq,
-                    float(scale) if scale else 0.0, _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr(), nbytes,
-                    _stream(q))
-            if lse is None:
-                L.check(_lib.b200k_fa2_fwd_kvcache_append(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                          o.data_ptr(), *args))
-            else:
-                L.check(_lib.b200k_fa2_fwd_kvcache_append_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(),
-                                                              o.data_ptr(), lse.data_ptr(), *args))
-        return
-    with _DeviceGuard(q):
-        nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size)
-        ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
-        args = (cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None,
-                B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0,
-                _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr() if ws is not None else None, nbytes, _stream(q))
-        if lse is None:
-            L.check(_lib.b200k_fa2_fwd_kvcache(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), *args))
-        else:
-            L.check(_lib.b200k_fa2_fwd_kvcache_lse(q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
-                                                   lse.data_ptr(), *args))
-
-
-def _fa2_fwd_kvcache_fp8(q, k_cache, v_cache, o, cache_seqlens, block_table, scale, causal, k, v, rotary_cos, rotary_sin,
-                         rotary_interleaved, lse, k_scale, v_scale) -> None:
-    """:func:`fa2_fwd_kvcache` over fp8 caches: the 16-bit call's checks, then b200k_fa2_kvcache_fp8."""
-    dt = q.dtype if q.dtype == torch.bfloat16 else torch.float16
-    B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, append, rotary = _kvcache_checks(
-        q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin, k_cache.dtype)
+        q, k_cache, v_cache, o, cache_seqlens, block_table, lse, k, v, rotary_cos, rotary_sin,
+        k_cache.dtype if fp8 else dt)
     cos, sin = rotary_cos, rotary_sin
-    ks, vs = _fp8_scales(k_scale, v_scale, H_kv)
+    ks, vs = _fp8_scales(k_scale, v_scale, H_kv) if fp8 else (None, None)
+    capacity = pages_per_seq * page_size
     with _DeviceGuard(q):
-        nbytes = fa2_fwd_kvcache_fp8_workspace_bytes(B, Lq, H, H_kv, D, pages_per_seq * page_size, append, rotary)
+        if fp8:
+            nbytes = fa2_fwd_kvcache_fp8_workspace_bytes(B, Lq, H, H_kv, D, capacity, append, rotary)
+        elif append:
+            nbytes = fa2_fwd_kvcache_append_workspace_bytes(B, Lq, H, H_kv, D, capacity, rotary)
+        else:
+            nbytes = fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, capacity)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=q.device) if nbytes else None
-        L.check(_lib.b200k_fa2_kvcache_fp8(
-            q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(), lse.data_ptr() if lse is not None else None,
-            cache_seqlens.data_ptr(), block_table.data_ptr() if block_table is not None else None, ks, vs,
-            _DTYPE_ENUM[k_cache.dtype], k.data_ptr() if append else None, v.data_ptr() if append else None,
-            k.size(1) if append else 0, cos.data_ptr() if rotary else None, sin.data_ptr() if rotary else None,
-            cos.size(0) if rotary else 0, 2 * cos.size(1) if rotary else 0, 1 if rotary_interleaved else 0,
-            B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0, _DTYPE_ENUM[dt],
-            1 if causal else 0, ws.data_ptr() if ws is not None else None, nbytes, _stream(q)))
+        ptrs = (q.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), o.data_ptr(),
+                lse.data_ptr() if lse is not None else None, cache_seqlens.data_ptr(),
+                block_table.data_ptr() if block_table is not None else None)
+        new = (k.data_ptr() if append else None, v.data_ptr() if append else None, k.size(1) if append else 0,
+               cos.data_ptr() if rotary else None, sin.data_ptr() if rotary else None, cos.size(0) if rotary else 0,
+               2 * cos.size(1) if rotary else 0, 1 if rotary_interleaved else 0)
+        shapes = (B, Lq, H, H_kv, D, num_pages, page_size, pages_per_seq, float(scale) if scale else 0.0,
+                  _DTYPE_ENUM[dt], 1 if causal else 0, ws.data_ptr() if ws is not None else None, nbytes, _stream(q))
+        if fp8:
+            L.check(_lib.b200k_fa2_kvcache_fp8(*ptrs, ks, vs, _DTYPE_ENUM[k_cache.dtype], *new, *shapes))
+        elif append:
+            L.check(_lib.b200k_fa2_fwd_kvcache_append_lse(*ptrs, *new, *shapes))
+        else:
+            L.check(_lib.b200k_fa2_fwd_kvcache_lse(*ptrs, *shapes))
 
 
 def attn_merge(o_parts: torch.Tensor, lse_parts: torch.Tensor, o: torch.Tensor,

@@ -791,12 +791,65 @@ __global__ void __launch_bounds__(256) kvcache_append_kernel(const KvAppend a) {
   }
 }
 
-// Launch geometry of KV-cache decode, shared by b200k_fa2_fwd_kvcache and its workspace query.  The 64 rows of a CTA
-// are T tokens x hb query heads of one K/V head's group of G; a group wider than 64 takes nhb head tiles.
+// One call of the KV-cache family as its entry point received it: decode (b200k_fa2_fwd_kvcache), append
+// (b200k_fa2_fwd_kvcache_append), fp8 caches (b200k_fa2_kvcache_fp8), packed prefill over paged caches
+// (b200k_fa2_varlen_paged, _fp8), or the shapes of a workspace query.  The fields follow the entry points' parameter
+// order.  A cache holds num_pages pages of page_size keys; a sequence's capacity is pages_per_seq pages (a contiguous
+// cache: B pages of S keys, one per sequence; a workspace query: one page of max_seqlen_k keys).
+struct KvCall {
+  const char* fn;               // the entry point, in messages
+  const char* lse_fn = nullptr;  // the name lse's alignment message uses (decode, append, fp8)
+  bool fp8 = false;     // b200k_fa2_kvcache_fp8: kv_dtype, the scales and lse are checked before the append part
+  bool append = false;  // new K / V rows go into the caches before the decode
+  bool rotary = false;  // ... rotated by cos / sin
+  const void *Q = nullptr, *K_cache = nullptr, *V_cache = nullptr;
+  void* O = nullptr;
+  float* lse = nullptr;
+  const int* cu_seqlens_q = nullptr;  // paged prefill
+  const int* seqlens = nullptr;       // cache_seqlens [B], or cu_seqlens_k [B + 1] in paged prefill
+  const int* table = nullptr;         // block table [B, pages_per_seq], or null
+  const float *k_scale = nullptr, *v_scale = nullptr;
+  int kv_dtype = 0;  // 0: caches in dtype; B200K_FP8_E4M3 / B200K_FP8_E5M2 (Fp8Kv)
+  const void *K_new = nullptr, *V_new = nullptr;
+  int64_t L_new = 0;
+  const void *cos = nullptr, *sin = nullptr;
+  int64_t rotary_seqlen = 0, rotary_dim = 0;
+  int interleaved = 0;
+  int64_t B = 0, Lq = 0, total_q = 0, H = 0, H_kv = 0, D = 0;  // paged prefill: Lq is max_seqlen_q
+  int64_t num_pages = 0, page_size = 0, pages_per_seq = 0;
+  float scale = 0.f;
+  int dtype = 0, causal = 0;
+  void* workspace = nullptr;
+  size_t workspace_bytes = 0;
+  void* stream = nullptr;
+
+  int64_t capacity() const { return pages_per_seq * page_size; }
+};
+
+// Calls f with the cache format of kv_dtype as a std::integral_constant: B200K_FP8_E4M3, B200K_FP8_E5M2, or 0 for
+// caches in the call's dtype.
+template <class F>
+static int with_kv_format(int kv_dtype, F&& f) {
+  if (kv_dtype == B200K_FP8_E4M3) return f(std::integral_constant<int, B200K_FP8_E4M3>());
+  if (kv_dtype == B200K_FP8_E5M2) return f(std::integral_constant<int, B200K_FP8_E5M2>());
+  return f(std::integral_constant<int, 0>());
+}
+
+// Mode `m` over caches of format KVF: as it is for 0, else through Fp8Kv with the call's scales.
+template <int KVF, class Mode>
+static auto kv_mode(const Mode& m, const KvCall& c) {
+  if constexpr (KVF == 0) return m;
+  else return Fp8Kv<Mode, KVF>{m, c.k_scale, c.v_scale};
+}
+
+// Launch geometry and workspace of a decode call, with or without new rows.  The 64 rows of a CTA are T tokens x hb
+// query heads of one K/V head's group of G; a group wider than 64 takes nhb head tiles.  The workspace, each section on
+// a 256-byte boundary: with new rows, int32 lengths [B] at 0 and the rotated Q [B, Lq, H, D] (rotary only) at q; from
+// part, the fp32 partials of a split call.
 struct KvcacheGrid {
   int hb = 1, T = 1, nhb = 1, splits = 1;
   int64_t qtiles = 1;
-  size_t workspace = 0;
+  size_t q = 0, part = 0, bytes = 0;
 };
 
 // The split rule.  ctas = B * H_kv * q tiles * head tiles CTAs each stream one K/V head of one sequence.  When they fill
@@ -819,21 +872,29 @@ static int kvcache_splits(int64_t ctas, int64_t max_seqlen_k, int sm_count) {
   return 1;
 }
 
-static KvcacheGrid kvcache_grid(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D, int64_t max_seqlen_k,
-                                int sm_count) {
+// The one workspace rule: the calls and the three workspace queries all size it here.
+static KvcacheGrid kvcache_grid(const KvCall& c, int sm_count) {
+  auto up = [](size_t n) { return (n + 255) & ~size_t(255); };
   KvcacheGrid g;
-  const int64_t G = H / H_kv;
+  const int64_t G = c.H / c.H_kv;
   g.hb = int(G < 64 ? G : 64);
   g.T = 64 / g.hb;
   g.nhb = int((G + g.hb - 1) / g.hb);
-  g.qtiles = (Lq + g.T - 1) / g.T;
-  g.splits = kvcache_splits(B * H_kv * g.qtiles * g.nhb, max_seqlen_k, sm_count);
-  if (g.splits > 1) g.workspace = size_t(g.splits) * size_t(B * Lq * H) * size_t(D + 1) * sizeof(float);
+  g.qtiles = (c.Lq + g.T - 1) / g.T;
+  g.splits = kvcache_splits(c.B * c.H_kv * g.qtiles * g.nhb, c.capacity(), sm_count);
+  if (c.append) {
+    g.q = up(size_t(c.B) * sizeof(int));
+    g.part = g.q + (c.rotary ? up(size_t(c.B * c.Lq * c.H) * size_t(c.D) * 2) : 0);
+  }
+  g.bytes = g.part;
+  if (g.splits > 1) g.bytes += size_t(g.splits) * size_t(c.B * c.Lq * c.H) * size_t(c.D + 1) * sizeof(float);
   return g;
 }
 
-// Shape checks shared by both decode entry points (before any CUDA call).
-static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t max_seqlen_k) {
+// Shape checks of the decode calls and their workspace queries (before any CUDA call).
+static int kvcache_check(const KvCall& c) {
+  const char* fn = c.fn;
+  const int64_t B = c.B, Lq = c.Lq, H = c.H, H_kv = c.H_kv, max_seqlen_k = c.capacity();
   if (B < 1 || Lq < 1 || H < 1 || H_kv < 1 || max_seqlen_k < 1 || H % H_kv != 0 || H > INT32_MAX)
     return set_error(B200K_ESHAPE, "%s: need B, Lq, H, H_kv, key capacity >= 1 and H %% H_kv == 0 (got B=%lld Lq=%lld "
                      "H=%lld H_kv=%lld capacity=%lld)", fn, (long long)B, (long long)Lq, (long long)H, (long long)H_kv,
@@ -849,134 +910,27 @@ static int kvcache_check(const char* fn, int64_t B, int64_t Lq, int64_t H, int64
 
 // Page counts of a cache read through a block table, or of a contiguous one: cache rows and a sequence's capacity
 // are int32.
-static int check_page_counts(const char* fn, int64_t num_pages, int64_t page_size, int64_t pages_per_seq) {
-  if (num_pages < 1 || page_size < 1 || pages_per_seq < 1)
-    return set_error(B200K_ESHAPE, "%s: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)", fn,
-                     (long long)num_pages, (long long)page_size, (long long)pages_per_seq);
-  if (num_pages > INT32_MAX / page_size || pages_per_seq > INT32_MAX / page_size)
-    return set_error(B200K_ESHAPE, "%s: num_pages * page_size and pages_per_seq * page_size must be <= 2^31 - 1", fn);
+static int check_page_counts(const KvCall& c) {
+  if (c.num_pages < 1 || c.page_size < 1 || c.pages_per_seq < 1)
+    return set_error(B200K_ESHAPE, "%s: need num_pages, page_size, pages_per_seq >= 1 (got %lld %lld %lld)", c.fn,
+                     (long long)c.num_pages, (long long)c.page_size, (long long)c.pages_per_seq);
+  if (c.num_pages > INT32_MAX / c.page_size || c.pages_per_seq > INT32_MAX / c.page_size)
+    return set_error(B200K_ESHAPE, "%s: num_pages * page_size and pages_per_seq * page_size must be <= 2^31 - 1", c.fn);
   return B200K_OK;
 }
 
 // The pages a block table can name: a KV tile of 128 keys is one TMA box inside one page, or a whole number of pages.
-static int check_page_size(const char* fn, int64_t page_size) {
-  if (page_size != 16 && page_size != 32 && page_size != 64 && page_size % 128 != 0)
-    return set_error(B200K_ESHAPE, "%s: page_size %lld (16, 32, 64 or a multiple of 128)", fn, (long long)page_size);
+static int check_page_size(const KvCall& c) {
+  if (c.page_size != 16 && c.page_size != 32 && c.page_size != 64 && c.page_size % 128 != 0)
+    return set_error(B200K_ESHAPE, "%s: page_size %lld (16, 32, 64 or a multiple of 128)", c.fn, (long long)c.page_size);
   return B200K_OK;
 }
 
-// Argument checks of b200k_fa2_fwd_kvcache, which b200k_fa2_fwd_kvcache_append shares (before any CUDA call).
-static int kvcache_args(const char* fn, const void* Q, const void* K_cache, const void* V_cache, const void* O,
-                        const int* cache_seqlens, const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv,
-                        int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq, int dtype) {
-  if (!Q || !K_cache || !V_cache || !O || !cache_seqlens) return set_error(B200K_EARG, "%s: null pointer", fn);
-  if (dtype != B200K_F16 && dtype != B200K_BF16)
-    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
-  int rc = check_headdim(fn, D);
-  if (rc || (rc = check_page_counts(fn, num_pages, page_size, pages_per_seq))) return rc;
-  if ((rc = kvcache_check(fn, B, Lq, H, H_kv, pages_per_seq * page_size))) return rc;
-  if (block_table && (rc = check_page_size(fn, page_size))) return rc;
-  if (!block_table && (num_pages != B || pages_per_seq != 1))
-    return set_error(B200K_ESHAPE, "%s: a contiguous cache (no block table) is num_pages = B pages of page_size = S keys, "
-                     "pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)", fn, (long long)num_pages,
-                     (long long)pages_per_seq);
-  return check_align(fn, {{Q, "Q", 16}, {K_cache, "K_cache", 16}, {V_cache, "V_cache", 16}, {O, "O", 4},
-                          {cache_seqlens, "cache_seqlens", 4}, {block_table, "block_table", 4}});
-}
-
-// Everything of a decode call after its workspace check: the decode kernel on `g`'s grid (Q read through a 3-D map,
-// lengths from `seqlens`), then the combine kernel when the call is split.  `part` is the split region of the workspace;
-// `lse` (null, or [B, Lq, H] fp32) is written by the decode kernel unsplit and by the combine kernel split.  kv_dtype:
-// 0 for caches in dtype, or B200K_FP8_E4M3 / B200K_FP8_E5M2 with k_scale / v_scale (Fp8Kv).
-static int kvcache_launch(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse, const int* seqlens,
-                          const int* block_table, int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
-                          int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal,
-                          const KvcacheGrid& g, void* part, cudaStream_t s, const DeviceInfo& di, int kv_dtype = 0,
-                          const float* k_scale = nullptr, const float* v_scale = nullptr) {
-  return run_attn_cfg<1, false>(dtype, D, [&](auto cfg) {
-    using Cfg = decltype(cfg);
-    AttnDecode<Cfg> d;
-    d.seqlens = seqlens;
-    d.table = block_table;
-    d.rows = B * Lq * H;
-    d.H = int(H);
-    d.causal = causal ? 1 : 0;
-    d.Lq = int(Lq);
-    d.group = int(H / H_kv);
-    d.hb = g.hb;
-    d.T = g.T;
-    d.nhb = g.nhb;
-    d.page_size = int(page_size);
-    d.pages_per_seq = int(pages_per_seq);
-    // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
-    d.box_rows = block_table && page_size < Cfg::BN ? int(page_size) : Cfg::BN;
-    d.oob = int(num_pages * page_size);
-    if (g.splits > 1) {
-      d.part = static_cast<float*>(part);
-      d.lse = d.part + size_t(g.splits) * size_t(d.rows) * size_t(D);
-    }
-    const int elem = kv_dtype ? 1 : 2;
-    const AttnTensor qkv[3] = {{Q, B * Lq, H, D, g.T, g.hb},
-                               {K_cache, num_pages * page_size, H_kv, D, d.box_rows, 1, elem},
-                               {V_cache, num_pages * page_size, H_kv, D, d.box_rows, 1, elem}};
-    const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(B * H_kv));
-    auto run = [&](const auto& mode) {
-      if (g.splits == 1) return launch_mode<Cfg>(qkv, grid, O, D, scale, mode, lse, s, di);
-      const int launched = launch_attn<Cfg>(qkv, grid, O, D, scale, mode, s, di);
-      if (launched) return launched;
-      const long long work = d.rows * (D / 2);
-      const unsigned blocks = unsigned((work + 255) / 256);
-      if (lse)
-        attn_combine_kernel<Cfg::DT, float, true><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits, lse);
-      else
-        attn_combine_kernel<Cfg::DT><<<blocks, 256, 0, s>>>(d.part, d.lse, O, d.rows, int(D), g.splits);
-      B200K_CHECK_CUDA(cudaGetLastError());
-      return B200K_OK;
-    };
-    if (kv_dtype == B200K_FP8_E4M3) return run(Fp8Kv<AttnDecode<Cfg>, B200K_FP8_E4M3>{d, k_scale, v_scale});
-    if (kv_dtype == B200K_FP8_E5M2) return run(Fp8Kv<AttnDecode<Cfg>, B200K_FP8_E5M2>{d, k_scale, v_scale});
-    return run(d);
-  });
-}
-
-// The checks the fp8 entry points add (before any CUDA call): the cache format, and the scales' alignment.
-static int fp8_args(const char* fn, int kv_dtype, const float* k_scale, const float* v_scale) {
-  if (kv_dtype != B200K_FP8_E4M3 && kv_dtype != B200K_FP8_E5M2)
-    return set_error(B200K_EDTYPE, "%s: kv_dtype %d not supported (fp8 e4m3, fp8 e5m2)", fn, kv_dtype);
-  return check_align(fn, {{k_scale, "k_scale", 4}, {v_scale, "v_scale", 4}});
-}
-
-// Workspace of b200k_fa2_fwd_kvcache_append, each section on a 256-byte boundary: int32 lengths [B], the rotated Q
-// [B, Lq, H, D] (rotary only), then the split region of kvcache_grid.
-struct AppendLayout {
-  size_t q = 0, part = 0, bytes = 0;
-};
-
-static AppendLayout append_layout(int64_t B, int64_t Lq, int64_t H, int64_t D, bool rotary, const KvcacheGrid& g) {
-  auto up = [](size_t n) { return (n + 255) & ~size_t(255); };
-  AppendLayout l;
-  l.q = up(size_t(B) * sizeof(int));
-  l.part = l.q + (rotary ? up(size_t(B * Lq * H) * size_t(D) * 2) : 0);
-  l.bytes = l.part + g.workspace;
-  return l;
-}
-
-// Checks of the append entry point beyond the decode call's (before any CUDA call).
-static int append_args(const char* fn, const void* K_new, const void* V_new, const void* cos, const void* sin, int64_t B,
-                       int64_t L_new, int64_t D, int64_t capacity, int64_t rotary_seqlen, int64_t rotary_dim,
-                       const void* workspace) {
-  if (!K_new || !V_new) return set_error(B200K_EARG, "%s: null K_new / V_new", fn);
-  if (!cos != !sin) return set_error(B200K_EARG, "%s: rotary needs both rotary_cos and rotary_sin", fn);
-  if (L_new < 1 || L_new > INT32_MAX || B > INT32_MAX / L_new)
-    return set_error(B200K_ESHAPE, "%s: need L_new >= 1 and B * L_new <= 2^31 - 1 (got L_new=%lld)", fn, (long long)L_new);
-  if (cos && (rotary_dim < 16 || rotary_dim > D || rotary_dim % 16 != 0))
-    return set_error(B200K_ESHAPE, "%s: rotary_dim %lld (a multiple of 16 in [16, D = %lld])", fn, (long long)rotary_dim,
-                     (long long)D);
-  if (cos && rotary_seqlen < capacity)
-    return set_error(B200K_ESHAPE, "%s: rotary_seqlen %lld is below the cache capacity %lld", fn, (long long)rotary_seqlen,
-                     (long long)capacity);
-  return check_align(fn, {{K_new, "K_new", 16}, {V_new, "V_new", 16}, {cos, "rotary_cos", 16}, {sin, "rotary_sin", 16},
-                          {workspace, "workspace", 16}});
+// The checks fp8 caches add: the cache format, and the scales' alignment.
+static int fp8_args(const KvCall& c) {
+  if (c.kv_dtype != B200K_FP8_E4M3 && c.kv_dtype != B200K_FP8_E5M2)
+    return set_error(B200K_EDTYPE, "%s: kv_dtype %d not supported (fp8 e4m3, fp8 e5m2)", c.fn, c.kv_dtype);
+  return check_align(c.fn, {{c.k_scale, "k_scale", 4}, {c.v_scale, "v_scale", 4}});
 }
 
 // Large head dims: O in column slices of DV = 192 or 256 (as few slices as possible, each a whole number of 64-column
@@ -993,82 +947,191 @@ static int launch_ffpa(const void* Q, const void* K, const void* V, void* O, int
 // The one check an lse output adds to an attention call (null: no lse).
 static int check_lse(const char* fn, const float* lse) { return check_align(fn, {{lse, "lse", 4}}); }
 
-// The append kernel of cache format KVF (0: dtype) for dtype and the rotary options, on `grid`.
+// The checks of a decode, append or fp8 call, before any CUDA call.  The fp8 entry point checks its cache format and
+// lse before the append part; the 16-bit ones check lse last.
+static int kvcache_args(const KvCall& c) {
+  const char* fn = c.fn;
+  if (!c.Q || !c.K_cache || !c.V_cache || !c.O || !c.seqlens) return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (c.dtype != B200K_F16 && c.dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, c.dtype);
+  int rc = check_headdim(fn, c.D);
+  if (rc || (rc = check_page_counts(c)) || (rc = kvcache_check(c))) return rc;
+  if (c.table && (rc = check_page_size(c))) return rc;
+  if (!c.table && (c.num_pages != c.B || c.pages_per_seq != 1))
+    return set_error(B200K_ESHAPE, "%s: a contiguous cache (no block table) is num_pages = B pages of page_size = S keys, "
+                     "pages_per_seq = 1 (got num_pages=%lld pages_per_seq=%lld)", fn, (long long)c.num_pages,
+                     (long long)c.pages_per_seq);
+  if ((rc = check_align(fn, {{c.Q, "Q", 16}, {c.K_cache, "K_cache", 16}, {c.V_cache, "V_cache", 16}, {c.O, "O", 4},
+                             {c.seqlens, "cache_seqlens", 4}, {c.table, "block_table", 4}})))
+    return rc;
+  if (c.fp8 && ((rc = fp8_args(c)) || (rc = check_lse(c.lse_fn, c.lse)))) return rc;
+  if (c.append) {
+    if (!c.K_new || !c.V_new) return set_error(B200K_EARG, "%s: null K_new / V_new", fn);
+    if (!c.cos != !c.sin) return set_error(B200K_EARG, "%s: rotary needs both rotary_cos and rotary_sin", fn);
+    if (c.L_new < 1 || c.L_new > INT32_MAX || c.B > INT32_MAX / c.L_new)
+      return set_error(B200K_ESHAPE, "%s: need L_new >= 1 and B * L_new <= 2^31 - 1 (got L_new=%lld)", fn,
+                       (long long)c.L_new);
+    if (c.cos && (c.rotary_dim < 16 || c.rotary_dim > c.D || c.rotary_dim % 16 != 0))
+      return set_error(B200K_ESHAPE, "%s: rotary_dim %lld (a multiple of 16 in [16, D = %lld])", fn,
+                       (long long)c.rotary_dim, (long long)c.D);
+    if (c.cos && c.rotary_seqlen < c.capacity())
+      return set_error(B200K_ESHAPE, "%s: rotary_seqlen %lld is below the cache capacity %lld", fn,
+                       (long long)c.rotary_seqlen, (long long)c.capacity());
+    rc = check_align(fn, {{c.K_new, "K_new", 16}, {c.V_new, "V_new", 16}, {c.cos, "rotary_cos", 16},
+                          {c.sin, "rotary_sin", 16}, {c.workspace, "workspace", 16}});
+  } else if (c.cos || c.sin) {
+    return set_error(B200K_EARG, "%s: rotary_cos / rotary_sin rotate appended keys and need K_new / V_new", fn);
+  } else {
+    rc = check_align(fn, {{c.workspace, "workspace", 16}});
+  }
+  if (rc || c.fp8) return rc;
+  return check_lse(c.lse_fn, c.lse);
+}
+
+// The append kernel of cache format KVF for the call's dtype and rotary options: one thread per 16-byte vector, at most
+// 65535 blocks.
 template <int KVF>
-static int launch_append(const KvAppend& a, int dtype, bool rotary, int rotary_interleaved, dim3 grid, cudaStream_t s) {
+static int launch_append(const KvAppend& a, const KvCall& c, cudaStream_t s) {
+  const long long items = (2 * a.kv_rows + a.q_rows) * (c.D / 8);
+  const long long blocks = ((items > c.B ? items : c.B) + 255) / 256;
+  const dim3 grid(unsigned(blocks < 65535 ? blocks : 65535));
   auto append = [&](auto kern) {
     kern<<<grid, 256, 0, s>>>(a);
     B200K_CHECK_CUDA(cudaGetLastError());
     return B200K_OK;
   };
-  if (dtype == B200K_BF16)
-    return !rotary ? append(kvcache_append_kernel<1, false, false, KVF>)
-                   : rotary_interleaved ? append(kvcache_append_kernel<1, true, true, KVF>)
-                                        : append(kvcache_append_kernel<1, true, false, KVF>);
-  return !rotary ? append(kvcache_append_kernel<0, false, false, KVF>)
-                 : rotary_interleaved ? append(kvcache_append_kernel<0, true, true, KVF>)
-                                      : append(kvcache_append_kernel<0, true, false, KVF>);
+  if (c.dtype == B200K_BF16)
+    return !c.rotary ? append(kvcache_append_kernel<1, false, false, KVF>)
+                     : c.interleaved ? append(kvcache_append_kernel<1, true, true, KVF>)
+                                     : append(kvcache_append_kernel<1, true, false, KVF>);
+  return !c.rotary ? append(kvcache_append_kernel<0, false, false, KVF>)
+                   : c.interleaved ? append(kvcache_append_kernel<0, true, true, KVF>)
+                                   : append(kvcache_append_kernel<0, true, false, KVF>);
 }
 
-// Everything of an append call after its argument checks: the workspace check, the append kernel, then the decode.
-static int kvcache_append_launch(const char* fn, const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
-                                 const int* cache_seqlens, const int* block_table, const void* K_new, const void* V_new,
-                                 int64_t L_new, const void* rotary_cos, const void* rotary_sin, int64_t rotary_seqlen,
-                                 int64_t rotary_dim, int rotary_interleaved, int64_t B, int64_t Lq, int64_t H,
-                                 int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
-                                 float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
-                                 void* stream, int kv_dtype, const float* k_scale, const float* v_scale) {
-  int rc;
-  const int64_t capacity = pages_per_seq * page_size;
-  const bool rotary = rotary_cos != nullptr;
+// A decode, append or fp8 call: its checks, the workspace check, then the append kernel when the call has new rows, the
+// decode kernel on the grid (Q read through a 3-D map), and the combine kernel when the call is split.  lse (null, or
+// [B, Lq, H] fp32) is written by the decode kernel unsplit and by the combine kernel split.
+static int kvcache_run(const KvCall& c) {
+  int rc = kvcache_args(c);
+  DeviceInfo di;
+  if (rc || (rc = get_device_info(&di))) return rc;
+  const KvcacheGrid g = kvcache_grid(c, di.sm_count);
+  if (g.bytes > 0 && (!c.workspace || c.workspace_bytes < g.bytes))
+    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", c.fn, g.bytes,
+                     c.workspace ? c.workspace_bytes : size_t(0));
+  cudaStream_t s = static_cast<cudaStream_t>(c.stream);
+  uint8_t* ws = static_cast<uint8_t*>(c.workspace);
+  return with_kv_format(c.kv_dtype, [&](auto kvf) {
+    constexpr int KVF = decltype(kvf)::value;
+    const void* Q = c.Q;
+    const int* seqlens = c.seqlens;
+    if (c.append) {
+      // the append entry points take the caches writable
+      const KvAppend a = {.q = static_cast<const uint16_t*>(c.Q), .k_new = static_cast<const uint16_t*>(c.K_new),
+                          .v_new = static_cast<const uint16_t*>(c.V_new), .cos = static_cast<const uint16_t*>(c.cos),
+                          .sin = static_cast<const uint16_t*>(c.sin),
+                          .q_out = c.rotary ? reinterpret_cast<uint16_t*>(ws + g.q) : nullptr,
+                          .k_cache = static_cast<uint16_t*>(const_cast<void*>(c.K_cache)),
+                          .v_cache = static_cast<uint16_t*>(const_cast<void*>(c.V_cache)), .seqlens = c.seqlens,
+                          .table = c.table, .lens_out = reinterpret_cast<int*>(ws), .kv_rows = c.B * c.L_new * c.H_kv,
+                          .q_rows = c.rotary ? c.B * c.Lq * c.H : 0, .rotary_seqlen = c.rotary_seqlen,
+                          .B = int(c.B), .L_new = int(c.L_new), .Lq = int(c.Lq), .H = int(c.H), .H_kv = int(c.H_kv),
+                          .D = int(c.D), .page_size = int(c.page_size), .pages_per_seq = int(c.pages_per_seq),
+                          .rotary_dim = c.rotary ? int(c.rotary_dim) : 0, .causal = c.causal ? 1 : 0,
+                          .k_scale = c.k_scale, .v_scale = c.v_scale};
+      if ((rc = launch_append<KVF>(a, c, s))) return rc;
+      // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
+      if (c.rotary) Q = a.q_out;
+      seqlens = a.lens_out;
+    }
+    return run_attn_cfg<1, false>(c.dtype, c.D, [&](auto cfg) {
+      using Cfg = decltype(cfg);
+      const long long rows = c.B * c.Lq * c.H;
+      float* part = g.splits > 1 ? reinterpret_cast<float*>(ws + g.part) : nullptr;
+      // a tile is one box of BN cache rows, or BN / page_size boxes (one per page) when pages are smaller
+      const AttnDecode<Cfg> d = {.seqlens = seqlens, .table = c.table, .part = part,
+                                 .lse = part ? part + size_t(g.splits) * size_t(rows) * size_t(c.D) : nullptr,
+                                 .rows = rows, .H = int(c.H), .causal = c.causal ? 1 : 0, .Lq = int(c.Lq),
+                                 .group = int(c.H / c.H_kv), .hb = g.hb, .T = g.T, .nhb = g.nhb,
+                                 .page_size = int(c.page_size), .pages_per_seq = int(c.pages_per_seq),
+                                 .box_rows = c.table && c.page_size < Cfg::BN ? int(c.page_size) : Cfg::BN,
+                                 .oob = int(c.num_pages * c.page_size)};
+      const int elem = KVF ? 1 : 2;
+      const AttnTensor qkv[3] = {{Q, c.B * c.Lq, c.H, c.D, g.T, g.hb},
+                                 {c.K_cache, c.num_pages * c.page_size, c.H_kv, c.D, d.box_rows, 1, elem},
+                                 {c.V_cache, c.num_pages * c.page_size, c.H_kv, c.D, d.box_rows, 1, elem}};
+      const dim3 grid(unsigned(g.splits), unsigned(g.qtiles * g.nhb), unsigned(c.B * c.H_kv));
+      const auto mode = kv_mode<KVF>(d, c);
+      if (g.splits == 1) return launch_mode<Cfg>(qkv, grid, c.O, c.D, c.scale, mode, c.lse, s, di);
+      if ((rc = launch_attn<Cfg>(qkv, grid, c.O, c.D, c.scale, mode, s, di))) return rc;
+      const long long work = d.rows * (c.D / 2);
+      const unsigned blocks = unsigned((work + 255) / 256);
+      if (c.lse)
+        attn_combine_kernel<Cfg::DT, float, true><<<blocks, 256, 0, s>>>(d.part, d.lse, c.O, d.rows, int(c.D), g.splits,
+                                                                         c.lse);
+      else
+        attn_combine_kernel<Cfg::DT><<<blocks, 256, 0, s>>>(d.part, d.lse, c.O, d.rows, int(c.D), g.splits);
+      B200K_CHECK_CUDA(cudaGetLastError());
+      return B200K_OK;
+    });
+  });
+}
+
+// The workspace queries: the bytes a call of c's shapes needs on the current device.
+static int kvcache_workspace_bytes(const KvCall& c, size_t* bytes) {
+  if (!bytes) return set_error(B200K_EARG, "%s: null pointer", c.fn);
+  int rc = check_headdim(c.fn, c.D);
+  DeviceInfo di;
+  if (rc || (rc = kvcache_check(c)) || (rc = get_device_info(&di))) return rc;
+  *bytes = kvcache_grid(c, di.sm_count).bytes;
+  return B200K_OK;
+}
+
+// Packed queries over paged caches (b200k_fa2_varlen_paged), and with kv_dtype and its scales, over fp8 pages.
+static int varlen_paged(const KvCall& c) {
+  const char* fn = c.fn;
+  if (!c.Q || !c.K_cache || !c.V_cache || !c.O || !c.cu_seqlens_q || !c.seqlens || !c.table)
+    return set_error(B200K_EARG, "%s: null pointer", fn);
+  if (c.dtype != B200K_F16 && c.dtype != B200K_BF16)
+    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, c.dtype);
+  int rc = c.kv_dtype ? fp8_args(c) : B200K_OK;
+  if (rc || (rc = check_headdim(fn, c.D))) return rc;
+  if (c.B < 1 || c.H < 1 || c.H_kv < 1 || c.H % c.H_kv != 0)
+    return set_error(B200K_ESHAPE, "%s: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)", fn,
+                     (long long)c.B, (long long)c.H, (long long)c.H_kv);
+  if ((rc = check_page_counts(c)) || (rc = check_page_size(c))) return rc;
+  if (c.total_q < 1 || c.total_q > INT32_MAX || c.Lq < 1 || c.Lq > c.total_q)
+    return set_error(B200K_ESHAPE, "%s: need 1 <= total_q <= 2^31 - 1 and 1 <= max_seqlen_q <= total_q (got total_q=%lld "
+                     "max_seqlen_q=%lld)", fn, (long long)c.total_q, (long long)c.Lq);
+  if (c.B > 65535 || c.H > 65535 || c.B * c.H > 65535)
+    return set_error(B200K_ESHAPE, "%s: B * H = %lld CTAs per query tile, the grid allows 65535", fn,
+                     (long long)c.B * (long long)c.H);
+  if ((rc = check_align(fn, {{c.Q, "Q", 16}, {c.K_cache, "K_cache", 16}, {c.V_cache, "V_cache", 16}, {c.O, "O", 4},
+                             {c.lse, "lse", 4}, {c.cu_seqlens_q, "cu_seqlens_q", 4}, {c.seqlens, "cu_seqlens_k", 4},
+                             {c.table, "block_table", 4}})))
+    return rc;
   DeviceInfo di;
   if ((rc = get_device_info(&di))) return rc;
-  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, capacity, di.sm_count);
-  const AppendLayout lay = append_layout(B, Lq, H, D, rotary, g);
-  if (!workspace || workspace_bytes < lay.bytes)
-    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, lay.bytes,
-                     workspace ? workspace_bytes : size_t(0));
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  uint8_t* ws = static_cast<uint8_t*>(workspace);
-  KvAppend a;
-  a.q = static_cast<const uint16_t*>(Q);
-  a.k_new = static_cast<const uint16_t*>(K_new);
-  a.v_new = static_cast<const uint16_t*>(V_new);
-  a.cos = static_cast<const uint16_t*>(rotary_cos);
-  a.sin = static_cast<const uint16_t*>(rotary_sin);
-  a.q_out = rotary ? reinterpret_cast<uint16_t*>(ws + lay.q) : nullptr;
-  a.k_cache = static_cast<uint16_t*>(K_cache);
-  a.v_cache = static_cast<uint16_t*>(V_cache);
-  a.seqlens = cache_seqlens;
-  a.table = block_table;
-  a.lens_out = reinterpret_cast<int*>(ws);
-  a.kv_rows = B * L_new * H_kv;
-  a.q_rows = rotary ? B * Lq * H : 0;
-  a.rotary_seqlen = rotary_seqlen;
-  a.B = int(B);
-  a.L_new = int(L_new);
-  a.Lq = int(Lq);
-  a.H = int(H);
-  a.H_kv = int(H_kv);
-  a.D = int(D);
-  a.page_size = int(page_size);
-  a.pages_per_seq = int(pages_per_seq);
-  a.rotary_dim = rotary ? int(rotary_dim) : 0;
-  a.causal = causal ? 1 : 0;
-  a.k_scale = k_scale;
-  a.v_scale = v_scale;
-  const long long items = (2 * a.kv_rows + a.q_rows) * (D / 8);
-  const long long blocks = ((items > B ? items : B) + 255) / 256;
-  const dim3 grid(unsigned(blocks < 65535 ? blocks : 65535));
-  rc = kv_dtype == B200K_FP8_E4M3   ? launch_append<B200K_FP8_E4M3>(a, dtype, rotary, rotary_interleaved, grid, s)
-       : kv_dtype == B200K_FP8_E5M2 ? launch_append<B200K_FP8_E5M2>(a, dtype, rotary, rotary_interleaved, grid, s)
-                                    : launch_append<0>(a, dtype, rotary, rotary_interleaved, grid, s);
-  if (rc) return rc;
-  // kernel boundaries order the cache writes above before the decode kernel's TMA reads of the caches
-  return kvcache_launch(rotary ? a.q_out : Q, K_cache, V_cache, O, lse, a.lens_out, block_table, B, Lq, H, H_kv, D, num_pages,
-                        page_size, pages_per_seq, scale, dtype, causal, g, ws + lay.part, s, di, kv_dtype, k_scale, v_scale);
+  cudaStream_t s = static_cast<cudaStream_t>(c.stream);
+  return with_kv_format(c.kv_dtype, [&](auto kvf) {
+    constexpr int KVF = decltype(kvf)::value;
+    return run_attn_cfg<2, false>(c.dtype, c.D, [&](auto cfg) {
+      using Cfg = decltype(cfg);
+      const int box_rows = c.page_size < Cfg::BN ? int(c.page_size) : Cfg::BN;
+      const int64_t cache_rows = c.num_pages * c.page_size;
+      const int elem = KVF ? 1 : 2;
+      const AttnTensor qkv[3] = {{c.Q, c.total_q, c.H, c.D, Cfg::BM, 1},
+                                 {c.K_cache, cache_rows, c.H_kv, c.D, box_rows, 1, elem},
+                                 {c.V_cache, cache_rows, c.H_kv, c.D, box_rows, 1, elem}};
+      const dim3 grid(unsigned((c.Lq + Cfg::BM - 1) / Cfg::BM), 1, unsigned(c.B * c.H));
+      const AttnPackedPaged<Cfg> args = {
+          {c.cu_seqlens_q, c.seqlens, int(c.H), int(c.H / c.H_kv), int(c.total_q), c.causal ? 1 : 0},
+          c.table, int(c.page_size), int(c.pages_per_seq), box_rows, int(cache_rows)};
+      return launch_mode<Cfg>(qkv, grid, c.O, c.D, c.scale, kv_mode<KVF>(args, c), c.lse, s, di);
+    });
+  });
 }
-
 
 }  // namespace b200k
 
@@ -1160,69 +1223,16 @@ extern "C" int b200k_fa2_fwd_varlen_lse(const void* Q, const void* K, const void
   });
 }
 
-namespace b200k {
-
-// b200k_fa2_varlen_paged, and with kv_dtype = B200K_FP8_E4M3 / B200K_FP8_E5M2 and its scales, the fp8 call.
-static int varlen_paged(const char* fn, const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
-                        const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table, int64_t B,
-                        int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D, int64_t num_pages,
-                        int64_t page_size, int64_t pages_per_seq, float scale, int dtype, int causal, void* stream,
-                        int kv_dtype, const float* k_scale, const float* v_scale) {
-  if (!Q || !K_cache || !V_cache || !O || !cu_seqlens_q || !cu_seqlens_k || !block_table)
-    return set_error(B200K_EARG, "%s: null pointer", fn);
-  if (dtype != B200K_F16 && dtype != B200K_BF16)
-    return set_error(B200K_EDTYPE, "%s: dtype %d not supported (f16, bf16)", fn, dtype);
-  int rc = kv_dtype ? fp8_args(fn, kv_dtype, k_scale, v_scale) : B200K_OK;
-  if (rc || (rc = check_headdim(fn, D))) return rc;
-  if (B < 1 || H < 1 || H_kv < 1 || H % H_kv != 0)
-    return set_error(B200K_ESHAPE, "%s: need B, H, H_kv >= 1 and H %% H_kv == 0 (got B=%lld H=%lld H_kv=%lld)", fn,
-                     (long long)B, (long long)H, (long long)H_kv);
-  if ((rc = check_page_counts(fn, num_pages, page_size, pages_per_seq)) || (rc = check_page_size(fn, page_size)))
-    return rc;
-  if (total_q < 1 || total_q > INT32_MAX || max_seqlen_q < 1 || max_seqlen_q > total_q)
-    return set_error(B200K_ESHAPE, "%s: need 1 <= total_q <= 2^31 - 1 and 1 <= max_seqlen_q <= total_q (got total_q=%lld "
-                     "max_seqlen_q=%lld)", fn, (long long)total_q, (long long)max_seqlen_q);
-  if (B > 65535 || H > 65535 || B * H > 65535)
-    return set_error(B200K_ESHAPE, "%s: B * H = %lld CTAs per query tile, the grid allows 65535", fn,
-                     (long long)B * (long long)H);
-  if ((rc = check_align(fn, {{Q, "Q", 16}, {K_cache, "K_cache", 16}, {V_cache, "V_cache", 16}, {O, "O", 4}, {lse, "lse", 4},
-                             {cu_seqlens_q, "cu_seqlens_q", 4}, {cu_seqlens_k, "cu_seqlens_k", 4},
-                             {block_table, "block_table", 4}})))
-    return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  cudaStream_t s = static_cast<cudaStream_t>(stream);
-  return run_attn_cfg<2, false>(dtype, D, [&](auto cfg) {
-    using Cfg = decltype(cfg);
-    const int box_rows = page_size < Cfg::BN ? int(page_size) : Cfg::BN;
-    const int64_t cache_rows = num_pages * page_size;
-    const int elem = kv_dtype ? 1 : 2;
-    const AttnTensor qkv[3] = {{Q, total_q, H, D, Cfg::BM, 1},
-                               {K_cache, cache_rows, H_kv, D, box_rows, 1, elem},
-                               {V_cache, cache_rows, H_kv, D, box_rows, 1, elem}};
-    const dim3 grid(unsigned((max_seqlen_q + Cfg::BM - 1) / Cfg::BM), 1, unsigned(B * H));
-    const AttnPackedPaged<Cfg> args = {{cu_seqlens_q, cu_seqlens_k, int(H), int(H / H_kv), int(total_q), causal ? 1 : 0},
-                                       block_table, int(page_size), int(pages_per_seq), box_rows, int(cache_rows)};
-    if (kv_dtype == B200K_FP8_E4M3)
-      return launch_mode<Cfg>(qkv, grid, O, D, scale, Fp8Kv<AttnPackedPaged<Cfg>, B200K_FP8_E4M3>{args, k_scale, v_scale},
-                              lse, s, di);
-    if (kv_dtype == B200K_FP8_E5M2)
-      return launch_mode<Cfg>(qkv, grid, O, D, scale, Fp8Kv<AttnPackedPaged<Cfg>, B200K_FP8_E5M2>{args, k_scale, v_scale},
-                              lse, s, di);
-    return launch_mode<Cfg>(qkv, grid, O, D, scale, args, lse, s, di);
-  });
-}
-
-}  // namespace b200k
-
 extern "C" int b200k_fa2_varlen_paged(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
                                       const int* cu_seqlens_q, const int* cu_seqlens_k, const int* block_table,
                                       int64_t B, int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv,
                                       int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
                                       float scale, int dtype, int causal, void* stream) {
-  return b200k::varlen_paged("b200k_fa2_varlen_paged", Q, K_cache, V_cache, O, lse, cu_seqlens_q, cu_seqlens_k,
-                             block_table, B, max_seqlen_q, total_q, H, H_kv, D, num_pages, page_size, pages_per_seq,
-                             scale, dtype, causal, stream, 0, nullptr, nullptr);
+  return b200k::varlen_paged({.fn = "b200k_fa2_varlen_paged", .Q = Q, .K_cache = K_cache, .V_cache = V_cache, .O = O,
+                              .lse = lse, .cu_seqlens_q = cu_seqlens_q, .seqlens = cu_seqlens_k, .table = block_table,
+                              .B = B, .Lq = max_seqlen_q, .total_q = total_q, .H = H, .H_kv = H_kv, .D = D,
+                              .num_pages = num_pages, .page_size = page_size, .pages_per_seq = pages_per_seq,
+                              .scale = scale, .dtype = dtype, .causal = causal, .stream = stream});
 }
 
 extern "C" int b200k_fa2_varlen_paged_fp8(const void* Q, const void* K_cache, const void* V_cache, void* O, float* lse,
@@ -1231,21 +1241,19 @@ extern "C" int b200k_fa2_varlen_paged_fp8(const void* Q, const void* K_cache, co
                                           int64_t max_seqlen_q, int64_t total_q, int64_t H, int64_t H_kv, int64_t D,
                                           int64_t num_pages, int64_t page_size, int64_t pages_per_seq, float scale,
                                           int dtype, int causal, void* stream) {
-  return b200k::varlen_paged("b200k_fa2_varlen_paged_fp8", Q, K_cache, V_cache, O, lse, cu_seqlens_q, cu_seqlens_k,
-                             block_table, B, max_seqlen_q, total_q, H, H_kv, D, num_pages, page_size, pages_per_seq,
-                             scale, dtype, causal, stream, kv_dtype, k_scale, v_scale);
+  return b200k::varlen_paged({.fn = "b200k_fa2_varlen_paged_fp8", .Q = Q, .K_cache = K_cache, .V_cache = V_cache, .O = O,
+                              .lse = lse, .cu_seqlens_q = cu_seqlens_q, .seqlens = cu_seqlens_k, .table = block_table,
+                              .k_scale = k_scale, .v_scale = v_scale, .kv_dtype = kv_dtype, .B = B, .Lq = max_seqlen_q,
+                              .total_q = total_q, .H = H, .H_kv = H_kv, .D = D, .num_pages = num_pages,
+                              .page_size = page_size, .pages_per_seq = pages_per_seq, .scale = scale, .dtype = dtype,
+                              .causal = causal, .stream = stream});
 }
 
 extern "C" int b200k_fa2_fwd_kvcache_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                                      int64_t max_seqlen_k, size_t* bytes) {
-  using namespace b200k;
-  if (!bytes) return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache_workspace_bytes: null pointer");
-  int rc = check_headdim("b200k_fa2_fwd_kvcache_workspace_bytes", D);
-  if (rc || (rc = kvcache_check("b200k_fa2_fwd_kvcache_workspace_bytes", B, Lq, H, H_kv, max_seqlen_k))) return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  *bytes = kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count).workspace;
-  return B200K_OK;
+  return b200k::kvcache_workspace_bytes({.fn = "b200k_fa2_fwd_kvcache_workspace_bytes", .B = B, .Lq = Lq, .H = H,
+                                         .H_kv = H_kv, .D = D, .page_size = max_seqlen_k, .pages_per_seq = 1},
+                                        bytes);
 }
 
 extern "C" int b200k_fa2_fwd_kvcache(const void* Q, const void* K_cache, const void* V_cache, void* O,
@@ -1263,34 +1271,20 @@ extern "C" int b200k_fa2_fwd_kvcache_lse(const void* Q, const void* K_cache, con
                                          int64_t H, int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size,
                                          int64_t pages_per_seq, float scale, int dtype, int causal, void* workspace,
                                          size_t workspace_bytes, void* stream) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_fwd_kvcache";
-  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
-                        pages_per_seq, dtype);
-  if (rc || (rc = check_align(fn, {{workspace, "workspace", 16}})) ||
-      (rc = check_lse("b200k_fa2_fwd_kvcache_lse", lse)))
-    return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
-  if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
-    return set_error(B200K_EARG, "b200k_fa2_fwd_kvcache: %zu workspace bytes needed, %zu given", g.workspace,
-                     workspace ? workspace_bytes : size_t(0));
-  return kvcache_launch(Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
-                        pages_per_seq, scale, dtype, causal, g, workspace, static_cast<cudaStream_t>(stream), di);
+  return b200k::kvcache_run({.fn = "b200k_fa2_fwd_kvcache", .lse_fn = "b200k_fa2_fwd_kvcache_lse", .Q = Q,
+                             .K_cache = K_cache, .V_cache = V_cache, .O = O, .lse = lse, .seqlens = cache_seqlens,
+                             .table = block_table, .B = B, .Lq = Lq, .H = H, .H_kv = H_kv, .D = D,
+                             .num_pages = num_pages, .page_size = page_size, .pages_per_seq = pages_per_seq,
+                             .scale = scale, .dtype = dtype, .causal = causal, .workspace = workspace,
+                             .workspace_bytes = workspace_bytes, .stream = stream});
 }
 
 extern "C" int b200k_fa2_fwd_kvcache_append_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                                             int64_t max_seqlen_k, int rotary, size_t* bytes) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_fwd_kvcache_append_workspace_bytes";
-  if (!bytes) return set_error(B200K_EARG, "%s: null pointer", fn);
-  int rc = check_headdim(fn, D);
-  if (rc || (rc = kvcache_check(fn, B, Lq, H, H_kv, max_seqlen_k))) return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  *bytes = append_layout(B, Lq, H, D, rotary != 0, kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count)).bytes;
-  return B200K_OK;
+  return b200k::kvcache_workspace_bytes({.fn = "b200k_fa2_fwd_kvcache_append_workspace_bytes", .append = true,
+                                         .rotary = rotary != 0, .B = B, .Lq = Lq, .H = H, .H_kv = H_kv, .D = D,
+                                         .page_size = max_seqlen_k, .pages_per_seq = 1},
+                                        bytes);
 }
 
 extern "C" int b200k_fa2_fwd_kvcache_append(const void* Q, void* K_cache, void* V_cache, void* O, const int* cache_seqlens,
@@ -1314,20 +1308,15 @@ extern "C" int b200k_fa2_fwd_kvcache_append_lse(const void* Q, void* K_cache, vo
                                                 int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
                                                 float scale, int dtype, int causal, void* workspace,
                                                 size_t workspace_bytes, void* stream) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_fwd_kvcache_append";
-  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
-                        pages_per_seq, dtype);
-  if (rc) return rc;
-  const int64_t capacity = pages_per_seq * page_size;
-  if ((rc = append_args(fn, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, capacity, rotary_seqlen, rotary_dim,
-                        workspace)) ||
-      (rc = check_lse("b200k_fa2_fwd_kvcache_append_lse", lse)))
-    return rc;
-  return kvcache_append_launch(fn, Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, K_new, V_new, L_new,
-                               rotary_cos, rotary_sin, rotary_seqlen, rotary_dim, rotary_interleaved, B, Lq, H, H_kv, D,
-                               num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace, workspace_bytes,
-                               stream, 0, nullptr, nullptr);
+  return b200k::kvcache_run({.fn = "b200k_fa2_fwd_kvcache_append", .lse_fn = "b200k_fa2_fwd_kvcache_append_lse",
+                             .append = true, .rotary = rotary_cos != nullptr, .Q = Q, .K_cache = K_cache,
+                             .V_cache = V_cache, .O = O, .lse = lse, .seqlens = cache_seqlens, .table = block_table,
+                             .K_new = K_new, .V_new = V_new, .L_new = L_new, .cos = rotary_cos, .sin = rotary_sin,
+                             .rotary_seqlen = rotary_seqlen, .rotary_dim = rotary_dim, .interleaved = rotary_interleaved,
+                             .B = B, .Lq = Lq, .H = H, .H_kv = H_kv, .D = D, .num_pages = num_pages,
+                             .page_size = page_size, .pages_per_seq = pages_per_seq, .scale = scale, .dtype = dtype,
+                             .causal = causal, .workspace = workspace, .workspace_bytes = workspace_bytes,
+                             .stream = stream});
 }
 
 extern "C" int b200k_attn_merge(const void* O_parts, const float* lse_parts, void* O, float* lse, int64_t S, int64_t rows,
@@ -1377,16 +1366,10 @@ extern "C" int b200k_ffpa_fwd_f16(const void* Q, const void* K, const void* V, v
 
 extern "C" int b200k_fa2_kvcache_fp8_workspace_bytes(int64_t B, int64_t Lq, int64_t H, int64_t H_kv, int64_t D,
                                                      int64_t max_seqlen_k, int append, int rotary, size_t* bytes) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_kvcache_fp8_workspace_bytes";
-  if (!bytes) return set_error(B200K_EARG, "%s: null pointer", fn);
-  int rc = check_headdim(fn, D);
-  if (rc || (rc = kvcache_check(fn, B, Lq, H, H_kv, max_seqlen_k))) return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, max_seqlen_k, di.sm_count);
-  *bytes = append ? append_layout(B, Lq, H, D, rotary != 0, g).bytes : g.workspace;
-  return B200K_OK;
+  return b200k::kvcache_workspace_bytes({.fn = "b200k_fa2_kvcache_fp8_workspace_bytes", .append = append != 0,
+                                         .rotary = rotary != 0, .B = B, .Lq = Lq, .H = H, .H_kv = H_kv, .D = D,
+                                         .page_size = max_seqlen_k, .pages_per_seq = 1},
+                                        bytes);
 }
 
 extern "C" int b200k_fa2_kvcache_fp8(const void* Q, void* K_cache, void* V_cache, void* O, float* lse,
@@ -1397,30 +1380,14 @@ extern "C" int b200k_fa2_kvcache_fp8(const void* Q, void* K_cache, void* V_cache
                                      int64_t H_kv, int64_t D, int64_t num_pages, int64_t page_size, int64_t pages_per_seq,
                                      float scale, int dtype, int causal, void* workspace, size_t workspace_bytes,
                                      void* stream) {
-  using namespace b200k;
-  const char* fn = "b200k_fa2_kvcache_fp8";
-  int rc = kvcache_args(fn, Q, K_cache, V_cache, O, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
-                        pages_per_seq, dtype);
-  if (rc || (rc = fp8_args(fn, kv_dtype, k_scale, v_scale)) || (rc = check_lse(fn, lse))) return rc;
-  if (K_new || V_new) {
-    if ((rc = append_args(fn, K_new, V_new, rotary_cos, rotary_sin, B, L_new, D, pages_per_seq * page_size, rotary_seqlen,
-                          rotary_dim, workspace)))
-      return rc;
-    return kvcache_append_launch(fn, Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, K_new, V_new, L_new,
-                                 rotary_cos, rotary_sin, rotary_seqlen, rotary_dim, rotary_interleaved, B, Lq, H, H_kv,
-                                 D, num_pages, page_size, pages_per_seq, scale, dtype, causal, workspace,
-                                 workspace_bytes, stream, kv_dtype, k_scale, v_scale);
-  }
-  if (rotary_cos || rotary_sin)
-    return set_error(B200K_EARG, "%s: rotary_cos / rotary_sin rotate appended keys and need K_new / V_new", fn);
-  if ((rc = check_align(fn, {{workspace, "workspace", 16}}))) return rc;
-  DeviceInfo di;
-  if ((rc = get_device_info(&di))) return rc;
-  const KvcacheGrid g = kvcache_grid(B, Lq, H, H_kv, D, pages_per_seq * page_size, di.sm_count);
-  if (g.workspace > 0 && (!workspace || workspace_bytes < g.workspace))
-    return set_error(B200K_EARG, "%s: %zu workspace bytes needed, %zu given", fn, g.workspace,
-                     workspace ? workspace_bytes : size_t(0));
-  return kvcache_launch(Q, K_cache, V_cache, O, lse, cache_seqlens, block_table, B, Lq, H, H_kv, D, num_pages, page_size,
-                        pages_per_seq, scale, dtype, causal, g, workspace, static_cast<cudaStream_t>(stream), di, kv_dtype,
-                        k_scale, v_scale);
+  return b200k::kvcache_run({.fn = "b200k_fa2_kvcache_fp8", .lse_fn = "b200k_fa2_kvcache_fp8", .fp8 = true,
+                             .append = K_new || V_new, .rotary = rotary_cos != nullptr, .Q = Q, .K_cache = K_cache,
+                             .V_cache = V_cache, .O = O, .lse = lse, .seqlens = cache_seqlens, .table = block_table,
+                             .k_scale = k_scale, .v_scale = v_scale, .kv_dtype = kv_dtype, .K_new = K_new,
+                             .V_new = V_new, .L_new = L_new, .cos = rotary_cos, .sin = rotary_sin,
+                             .rotary_seqlen = rotary_seqlen, .rotary_dim = rotary_dim, .interleaved = rotary_interleaved,
+                             .B = B, .Lq = Lq, .H = H, .H_kv = H_kv, .D = D, .num_pages = num_pages,
+                             .page_size = page_size, .pages_per_seq = pages_per_seq, .scale = scale, .dtype = dtype,
+                             .causal = causal, .workspace = workspace, .workspace_bytes = workspace_bytes,
+                             .stream = stream});
 }

@@ -7,13 +7,16 @@ see the same arguments.
   1. Seeded random inputs through both builds; every output (and, for append, both caches) must have the same bits:
      dense f16 / bf16 at D 32 - 128 (causal, key padding, ragged N), V stored [B,H,D,N], FFPA at D 160 - 1024, packed
      GQA / MQA with empty sequences, decode on contiguous caches and pages of 16 / 64 / 256 at one split and at many
-     (G = 72 among them: two 64-row head tiles), and append with and without rotary; the backward's dQ, dK and dV,
-     dense f16 / bf16 at D 64 and 128 (causal, key padding, ragged N) and packed GQA with empty sequences and Lq != Lk.
+     (G = 72 among them: two 64-row head tiles), and append with and without rotary; decode and rotary append with
+     lse over 16-bit and fp8 (e4m3 / e5m2, with and without scales) caches, at one split and at many; packed prefill
+     over 16-bit and fp8 pages of 16 and 256; the backward's dQ, dK and dV, dense f16 / bf16 at D 64 and 128 (causal,
+     key padding, ragged N) and packed GQA with empty sequences and Lq != Lk.
   2. Time per call of each build, alternating, one CUDA graph of `iters` calls per build per round: bench.py's
      attention shapes (dense (4, 48, 8192, 64) and (4, 64, 8192, 128), FFPA (1, 32, 4096, 512)), packed GQA (4 x 8192
      tokens, H 64, H_kv 8, D 128, causal) and decode against an 8K cache at B 1 and 64; the backward at the dense
-     shapes and the packed GQA one, causal and not.  Each line gives the median and min - max of both builds and
-     whether the new median lies inside the base's min - max.
+     shapes and the packed GQA one, causal and not.  Then decode and append at B 1 against an 8K cache, call by call
+     without a graph, so the host's share of each call counts.  Each line gives the median and min - max of both
+     builds and whether the new median lies inside the base's min - max.
 
 The first line names the GPU, its power limit and its maximum SM clock, read in the same run.
 
@@ -151,6 +154,54 @@ def equal_cases(torch, ops):
                     return [o, kc, vc]
                 cases.append(("append %s rotary=%s B=%d H_kv=%d" % (kind, rotary, B, H_kv), run))
 
+    # decode and append with lse, 16-bit or fp8 caches (e4m3 / e5m2, with and without per-head scales), at one split
+    # (B 16, H_kv 8) and at many (B 1, H_kv 1); appends with NeoX or interleaved rotary
+    for kvdt in (None, torch.float8_e4m3fn, torch.float8_e5m2):
+        for scaled in ((False,) if kvdt is None else (False, True)):
+            for B, H_kv in ((16, 8), (1, 1)):
+                for rotary in (None, "neox", "interleaved"):
+                    torch.manual_seed(40 + B + scaled + (rotary is None))
+                    Lq, G, D, S, L_new, ps = 2, 4, 128, 1024, 2, 64
+                    q, kn, vn = rn(B, Lq, G * H_kv, D), rn(B, L_new, H_kv, D), rn(B, L_new, H_kv, D)
+                    kc0, vc0, table = paged(rn(B, S, H_kv, D), rn(B, S, H_kv, D), ps, B)
+                    if kvdt is not None:
+                        kc0, vc0 = kc0.to(kvdt), vc0.to(kvdt)
+                    lens = i32(torch.randint(0, S - L_new + 1, (B,)).tolist())
+                    kw = dict(k_scale=torch.rand(H_kv, device=dev) + 0.5, v_scale=torch.rand(H_kv, device=dev) + 0.5) \
+                        if scaled else {}
+                    if rotary:
+                        theta = torch.rand(S, 32, device=dev) * 6.283
+                        kw.update(k=kn, v=vn, rotary_cos=theta.cos().half(), rotary_sin=theta.sin().half(),
+                                  rotary_interleaved=rotary == "interleaved")
+
+                    def run(q=q, kc0=kc0, vc0=vc0, lens=lens, table=table, kw=kw):
+                        kc, vc = kc0.clone(), vc0.clone()
+                        o, lse = torch.full_like(q, float("nan")), torch.full(q.shape[:-1], float("nan"), device=dev)
+                        ops.fa2_fwd_kvcache(q, kc, vc, o, lens, table, causal=True, lse=lse, **kw)
+                        return [o, lse, kc, vc]
+                    cases.append(("kvcache lse %s scaled=%d B=%d H_kv=%d %s" % (
+                        str(kvdt)[6:] or "f16", scaled, B, H_kv, "rotary=%s" % rotary if rotary else "decode"), run))
+
+    # packed prefill over paged caches, 16-bit or fp8, with and without lse
+    for kvdt in (None, torch.float8_e4m3fn, torch.float8_e5m2):
+        for ps in (16, 256):
+            for causal in (False, True):
+                torch.manual_seed(50 + ps + causal)
+                H_kv, D, S = 4, 128, 768
+                q = rn(sum(lq), 16, D)
+                kc, vc, table = paged(rn(len(lk), S, H_kv, D), rn(len(lk), S, H_kv, D), ps, ps + causal)
+                kw = {}
+                if kvdt is not None:
+                    kc, vc = kc.to(kvdt), vc.to(kvdt)
+                    kw = dict(k_scale=torch.rand(H_kv, device=dev) + 0.5, v_scale=torch.rand(H_kv, device=dev) + 0.5)
+
+                def run(q=q, kc=kc, vc=vc, table=table, causal=causal, kw=kw):
+                    o = torch.full_like(q, float("nan"))
+                    lse = torch.full(q.shape[:-1], float("nan"), device=dev) if causal else None
+                    ops.fa2_fwd_varlen(q, kc, vc, o, cq, ck, max(lq), causal=causal, lse=lse, block_table=table, **kw)
+                    return [o] + ([lse] if causal else [])
+                cases.append(("paged prefill %s page=%d causal=%d" % (str(kvdt)[6:] or "f16", ps, causal), run))
+
     # backward: o and lse from the in-tree forward, so both builds take the same inputs
     for dt in (torch.float16, torch.bfloat16):
         for D in (64, 128):
@@ -237,6 +288,22 @@ def timed_cases(torch, ops):
     return cases
 
 
+def eager_cases(torch, ops):
+    """(name, flop, run) timed call by call without a graph, so the host's share of a call of about 10 us shows:
+    decode and append (one new token, no rotary) at B 1 against an 8K cache."""
+    dev = "cuda"
+    S, H, H_kv, D = 8192, 32, 8, 128
+    q = torch.randn(1, 1, H, D, dtype=torch.half, device=dev)
+    kc, vc = [torch.randn(1, S, H_kv, D, dtype=torch.half, device=dev) for _ in range(2)]
+    kn, vn = [torch.randn(1, 1, H_kv, D, dtype=torch.half, device=dev) for _ in range(2)]
+    o = torch.empty_like(q)
+    lens = torch.full((1,), S - 1, dtype=torch.int32, device=dev)
+    return [("eager decode B 1 Lq 1 H 32 H_kv 8 D 128, 8K cache", 4.0 * H * S * D,
+             lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens)),
+            ("eager append B 1 L_new 1 H 32 H_kv 8 D 128, 8K cache", 4.0 * H * S * D,
+             lambda: ops.fa2_fwd_kvcache(q, kc, vc, o, lens, k=kn, v=vn))]
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--build-base", metavar="REV", help="build REV's library into build_ab/base and exit")
@@ -257,7 +324,8 @@ def main():
           flush=True)
 
     bad, slow = compare_and_time(torch, libs, equal_cases(torch, ops), timed_cases(torch, ops), args.rounds)
-    print(json.dumps({"differing_cases": bad, "new_median_above_base_max": slow}), flush=True)
+    _, slow_eager = compare_and_time(torch, libs, [], eager_cases(torch, ops), args.rounds, graph=False)
+    print(json.dumps({"differing_cases": bad, "new_median_above_base_max": slow + slow_eager}), flush=True)
     sys.exit(1 if bad else 0)
 
 

@@ -143,10 +143,11 @@ def same_bits(a, b):
     return a.dtype == b.dtype and a.shape == b.shape and torch.equal(*raw)
 
 
-def compare_and_time(torch, libs, cases, timed, rounds, unit=("tflops", 1e-12)):
+def compare_and_time(torch, libs, cases, timed, rounds, unit=("tflops", 1e-12), graph=True):
     """Runs each (name, run) of `cases` through libs["base"] and libs["new"] and prints the ones whose outputs differ
     in any bit, then times each (name, work, fn) of `timed` (a rate in `unit` = (name, scale) is work / time * scale):
-    one CUDA graph per build, sized to about 100 ms, the builds alternating and swapping order every other round.
+    one CUDA graph per build (or, with graph=False, eager calls, host cost included), sized to about 100 ms, the
+    builds alternating and swapping order every other round.
     Returns (differing cases, timed cases whose new median lies above the base's maximum)."""
     bad = 0
     for name, run in cases:
@@ -172,7 +173,7 @@ def compare_and_time(torch, libs, cases, timed, rounds, unit=("tflops", 1e-12)):
         with using(libs["base"]):  # about 100 ms of work per build per round
             per_call = time_rounds({"base": fn}, 3, 1)["base"][0]
         iters = max(3, min(2000, int(0.1 / per_call)))
-        times = time_rounds({key: on(lib, fn) for key, lib in libs.items()}, iters, rounds, graph=True, swap=True)
+        times = time_rounds({key: on(lib, fn) for key, lib in libs.items()}, iters, rounds, graph=graph, swap=True)
         us = {k: [s * 1e6 for s in stats(v)] for k, v in times.items()}  # median, min, max
         line = {"case": name, "iters_per_round": iters}
         for k, (med, lo, hi) in us.items():
