@@ -147,20 +147,7 @@ def make_case(dtype, B, H, N, D, causal, lens=None, seed=0, k=0, W=3, nnz=2, fra
 
     V = ri(-8, 9, (BH, N, D))
     V[..., 0] = 1
-    O = ri(-8, 9, (BH, N, D))
-    dO = torch.zeros(BH, N, D, dtype=torch.long)
-    dO.scatter_add_(2, ri(1, D, (BH, N, nnz)), 2 * ri(0, 2, (BH, N, nnz)) - 1)      # normal: two +-1 entries
-    R = max(1, round(2 * ROUND_MASS[dtype] / (D - 1)))
-    big = ri(-R, R + 1, (BH, N, D))
-    big[..., 0] = 0
-    rnd = (kind == 1).view(BH, N, 1)
-    dO = torch.where(rnd, big, dO)
-    O = torch.where(rnd & (big != 0), -16 * big.sign(), O)
-    fr_ = (kind == 2).view(BH, N, 1)
-    e0 = torch.zeros(1, 1, D, dtype=torch.long)
-    e0[..., 0] = 1
-    dO = torch.where(fr_, e0, dO)
-    O[..., 0] = torch.where(kind == 2, 1, O[..., 0])
+    dO, O = row_values(kind.view(-1), D, dtype, nnz, ri)
 
     q = torch.zeros(BH, N, D)
     q.scatter_(2, col.view(BH, N, 1), 2.0 ** k)
@@ -169,6 +156,26 @@ def make_case(dtype, B, H, N, D, causal, lens=None, seed=0, k=0, W=3, nnz=2, fra
                scale=ga.scale_exact(k), causal=causal, col=col.view(B, H, N), t=(eighths / 8.0).view(B, H, N),
                kind=kind.view(B, H, N))
     return out
+
+
+def row_values(kind, D, dtype, nnz, ri):
+    """(dO, O) long [R, D] for rows of the given kinds (0 normal, 1 round, 2 frac), with V[:, 0] = 1 assumed; ri(lo, hi,
+    shape) draws integers."""
+    R = kind.numel()
+    O = ri(-8, 9, (R, D))
+    dO = torch.zeros(R, D, dtype=torch.long)
+    dO.scatter_add_(1, ri(1, D, (R, nnz)), 2 * ri(0, 2, (R, nnz)) - 1)              # normal: two +-1 entries
+    M = max(1, round(2 * ROUND_MASS[dtype] / (D - 1)))
+    big = ri(-M, M + 1, (R, D))
+    big[:, 0] = 0
+    rnd = (kind == 1).view(R, 1)
+    dO = torch.where(rnd, big, dO)
+    O = torch.where(rnd & (big != 0), -16 * big.sign(), O)
+    e0 = torch.zeros(1, D, dtype=torch.long)
+    e0[:, 0] = 1
+    dO = torch.where((kind == 2).view(R, 1), e0, dO)
+    O[:, 0] = torch.where(kind == 2, 1, O[:, 0])
+    return dO, O
 
 
 def _pack(dtype, shape, ints):
@@ -188,7 +195,25 @@ def make_forward_case(dtype, B, H, N, D, lens=None, seed=0, k=0):
     2^-4, so O, Delta and dS stay within a few bits.  Returns make_case's dict without o and lse, and t per row."""
     g = torch.Generator().manual_seed(seed)
     BH = B * H
-    kv = kv_lens(lens, B, N).repeat_interleave(H)
+    K, top = forward_keys(BH, N, D, kv_lens(lens, B, N).repeat_interleave(H), g)
+    col = torch.randint(0, D, (BH, N), generator=g)
+    q = torch.zeros(BH, N, D)
+    q.scatter_(2, col.view(BH, N, 1), 2.0 ** k)
+    V = torch.randint(-8, 9, (BH, N, D), generator=g)
+    dO = torch.zeros(BH, N, D, dtype=torch.long)
+    dO.scatter_add_(2, torch.randint(0, D, (BH, N, 2), generator=g), 2 * torch.randint(0, 2, (BH, N, 2), generator=g) - 1)
+    out = _pack(dtype, (B, H, N, D), dict(q=q, k=K, v=V, do=dO))
+    t = top.gather(1, col)
+    assert int(t.abs().max()) <= 12
+    out.update(seqlens=None if lens is None else torch.as_tensor(lens, dtype=torch.int32), scale=ga.scale_exact(k),
+               causal=False, col=col.view(B, H, N), t=t.view(B, H, N).double(), kind=torch.zeros(B, H, N, dtype=torch.long))
+    return out
+
+
+def forward_keys(BH, N, D, kv, g):
+    """(K long [BH, N, D], top [BH, D]) of make_forward_case: head bh has kv[bh] keys (DECOY on the key after them when
+    kv[bh] < N), and column c of it holds 2^u - x keys at grade m, 2x at m - 1 and FAR elsewhere; top = m + u, the lse2
+    of a row that reads column c."""
     K = torch.randint(-4, 5, (BH, N, D), generator=g)
     top = torch.zeros(BH, D, dtype=torch.long)
     for bh in range(BH):
@@ -204,18 +229,7 @@ def make_forward_case(dtype, B, H, N, D, lens=None, seed=0, k=0):
             K[bh, perm[:2 ** u - x], c] = m
             K[bh, perm[2 ** u - x:2 ** u + x], c] = m - 1
             top[bh, c] = m + u
-    col = torch.randint(0, D, (BH, N), generator=g)
-    q = torch.zeros(BH, N, D)
-    q.scatter_(2, col.view(BH, N, 1), 2.0 ** k)
-    V = torch.randint(-8, 9, (BH, N, D), generator=g)
-    dO = torch.zeros(BH, N, D, dtype=torch.long)
-    dO.scatter_add_(2, torch.randint(0, D, (BH, N, 2), generator=g), 2 * torch.randint(0, 2, (BH, N, 2), generator=g) - 1)
-    out = _pack(dtype, (B, H, N, D), dict(q=q, k=K, v=V, do=dO))
-    t = top.gather(1, col)
-    assert int(t.abs().max()) <= 12
-    out.update(seqlens=None if lens is None else torch.as_tensor(lens, dtype=torch.int32), scale=ga.scale_exact(k),
-               causal=False, col=col.view(B, H, N), t=t.view(B, H, N).double(), kind=torch.zeros(B, H, N, dtype=torch.long))
-    return out
+    return K, top
 
 
 def forward_lse(t):
@@ -262,13 +276,23 @@ def closed_form(q, k, v, o, lse, do, scale, causal, seqlens, rounded=True):
     """((dq, dk, dv) in q's dtype, info) from the six inputs, in fp64 on q's device, every step asserted exact (see the
     module docstring).  rounded=False gives the fp64 gradients of the same P and dS without the dtype roundings and
     with the exact scale (scale_log2 ln 2), for comparison with attn_bwd_oracle.grads_given."""
-    dtype, dev = q.dtype, q.device
     B, H, N, D = q.shape
-    Q, K, V, O, dO = (t.double() for t in (q, k, v, o, do))
-    vis = visible(B, H, N, causal, None if seqlens is None else seqlens.cpu()).to(dev)
+    vis = visible(B, H, N, causal, None if seqlens is None else seqlens.cpu()).to(q.device)
+    lse2 = (lse.float() * torch.tensor(LOG2E_F32, dtype=torch.float32, device=q.device)).double()
+    return closed_form_core(*(t.double() for t in (q, k, v, o, do)), lse2, vis, scale, q.dtype, rounded)
+
+
+def closed_form_core(Q, K, V, O, dO, lse2, vis, scale, dtype, rounded=True, group=1):
+    """closed_form on fp64 operands: Q, O, dO [..., H, Lq, D], K, V [..., H / group, Lk, D] (query head h reads K/V head
+    h // group), lse2 [..., H, Lq] as the prep writes it, vis [..., H, Lq, Lk] (or broadcastable) the keys each row sees.
+    dK and dV sum over the group: their windows are those of the group's G * Lq terms.  info adds ds_group, the keys
+    whose dK sums nonzero dS~ from two or more heads."""
+    dev = Q.device
+    H, Lq, Lk = Q.size(-3), Q.size(-2), K.size(-2)
+    vis = vis.expand(*Q.shape[:-1], Lk)
+    Kx, Vx = (t.repeat_interleave(group, dim=-3) for t in (K, V))
     sl = float(np.float32(scale) * np.float32(LOG2E_F32))
-    lse2 = (lse.float() * torch.tensor(LOG2E_F32, dtype=torch.float32, device=dev)).double()
-    S = Q @ K.transpose(-1, -2)
+    S = Q @ Kx.transpose(-1, -2)
     x = torch.where(vis, S * sl - lse2.unsqueeze(-1), torch.full_like(S, float("-inf")))
     xv = x[vis]
     assert bool((xv * 8 == (xv * 8).round()).all()), "a score exponent is not a multiple of 1/8"
@@ -280,9 +304,9 @@ def closed_form(q, k, v, o, lse, do, scale, causal, seqlens, rounded=True):
     assert bool(torch.isin(eighth[frac], torch.tensor(ga.fractional_grades(dtype), device=dev)).all())
     Pr = P.to(dtype).double() if rounded else P
 
-    _window(dO.abs() @ V.abs().transpose(-1, -2), _maxG(dO, -1) + _maxG(V, -1).transpose(-1, -2), "dP")
+    _window(dO.abs() @ Vx.abs().transpose(-1, -2), _maxG(dO, -1) + _maxG(Vx, -1).transpose(-1, -2), "dP")
     _window((dO * O).abs().sum(-1), _maxG(dO, -1).squeeze(-1) + _maxG(O, -1).squeeze(-1), "Delta")
-    dP = dO @ V.transpose(-1, -2)
+    dP = dO @ Vx.transpose(-1, -2)
     Delta = (dO * O).sum(-1)
     dd = torch.where(vis, dP - Delta.unsqueeze(-1), torch.zeros_like(dP))
     assert torch.equal(dd.float().double(), dd), "dP - Delta is not an fp32 value"
@@ -291,12 +315,16 @@ def closed_form(q, k, v, o, lse, do, scale, causal, seqlens, rounded=True):
     assert torch.equal(torch.where(frac, 0.0, dS).float().double(), torch.where(frac, 0.0, dS)), "dS not fp32"
     dSr = dS.float().to(dtype).double() if rounded else dS
 
-    dq, dk, dv = dSr @ K, dSr.transpose(-1, -2) @ Q, Pr.transpose(-1, -2) @ dO
+    # the group's heads side by side as G * Lq rows of one K/V head (heads h = kv head * G + g are adjacent)
+    fold = lambda t: t.reshape(*t.shape[:-3], H // group, group * Lq, t.size(-1))  # noqa: E731
+    dSf, Prf, Qf, dOf = fold(dSr), fold(Pr), fold(Q), fold(dO)
+    dq, dk, dv = dSr @ Kx, dSf.transpose(-1, -2) @ Qf, Prf.transpose(-1, -2) @ dOf
     if not rounded:
         return (dq * (sl * math.log(2)), dk * (sl * math.log(2)), dv), {}
     info = dict(
-        win_dq=_window_mm(dSr, K, "dQ"), win_dk=_window_mm(dSr.transpose(-1, -2), Q, "dK"),
-        win_dv=_window_mm(Pr.transpose(-1, -2), dO, "dV"))
+        win_dq=_window_mm(dSr, Kx, "dQ"), win_dk=_window_mm(dSf.transpose(-1, -2), Qf, "dK"),
+        win_dv=_window_mm(Prf.transpose(-1, -2), dOf, "dV"),
+        ds_group=int(((dSr != 0).any(-2).reshape(*dSr.shape[:-3], H // group, group, Lk).sum(-2) >= 2).sum()))
     for name, t in (("dQ", dq), ("dK", dk), ("dV", dv)):
         assert torch.equal(t.float().double(), t), name + " sum is not an fp32 value"
     s32 = torch.tensor(float(np.float32(scale)), dtype=torch.float32, device=dev)
