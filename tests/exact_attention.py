@@ -1,5 +1,5 @@
 """Exact-answer inputs for attention, shared by every mode (dense, FFPA, packed, KV-cache decode, append), used by
-test_gpu_attention_exact.py and checked against varlen_oracle in test_attention_exact_cpu.py.
+test_gpu_attention_exact.py and checked against attention_ref in test_attention_exact_cpu.py.
 
 Row r of Q is A * e_c: one non-zero column c, chosen per row.  Within one block of keys (one (sequence, K/V head)),
 column c of K is A at one key, the column's needle, and 0 everywhere else.  The score of row r is then A^2 at its needle

@@ -275,7 +275,7 @@ def _window_mm(A, B, what):
 def closed_form(q, k, v, o, lse, do, scale, causal, seqlens, rounded=True):
     """((dq, dk, dv) in q's dtype, info) from the six inputs, in fp64 on q's device, every step asserted exact (see the
     module docstring).  rounded=False gives the fp64 gradients of the same P and dS without the dtype roundings and
-    with the exact scale (scale_log2 ln 2), for comparison with attn_bwd_oracle.grads_given."""
+    with the exact scale (scale_log2 ln 2), for comparison with attention_ref.dense_grads_given."""
     B, H, N, D = q.shape
     vis = visible(B, H, N, causal, None if seqlens is None else seqlens.cpu()).to(q.device)
     lse2 = (lse.float() * torch.tensor(LOG2E_F32, dtype=torch.float32, device=q.device)).double()

@@ -22,9 +22,9 @@ from __future__ import annotations
 import numpy as np
 import torch
 
+import attention_ref as ar
 import graded_attention as ga
 import graded_attention_bwd as gb
-import varlen_bwd_oracle as vo
 
 LOG2E_F32 = ga.LOG2E_F32
 DECOY = ga.DECOY
@@ -154,7 +154,7 @@ def forward_outputs(case):
     G = q.size(1) // k.size(1)
     sl = float(np.float32(case["scale"]) * np.float32(LOG2E_F32))
     o = torch.zeros(q.shape, dtype=torch.float64)
-    for q0, q1, k0, k1 in vo.seqs(case["cu_q"], case["cu_k"]):
+    for q0, q1, k0, k1 in ar.seqs(case["cu_q"], case["cu_k"]):
         if q1 > q0 and k1 > k0:
             kk, vv = (x[k0:k1].double().repeat_interleave(G, dim=1) for x in (k, v))
             x = torch.einsum("qhd,khd->hqk", q[q0:q1].double(), kk) * sl - case["t"][q0:q1].t().unsqueeze(-1)
@@ -175,20 +175,21 @@ def closed_form(case, rounded=True):
     """((dq, dk, dv), info): graded_attention_bwd.closed_form_core one sequence at a time on the case's device, K/V
     expanded over the group and dK / dV summed back, bottom-right causal mask; everything outside the sequences, keys of
     an empty query sequence and rows of an empty key sequence +0.  rounded=False: the fp64 gradients (as in
-    closed_form_core) for comparison with varlen_bwd_oracle.grads_given.  info: counts summed, windows maximised."""
+    closed_form_core) for comparison with attention_ref.packed_grads_given.  info: counts summed, windows maximised."""
     q, k, v, o, do = (case[n] for n in ("q", "k", "v", "o", "do"))
     H, H_kv = q.size(1), k.size(1)
     out_dt = q.dtype if rounded else torch.float64
     dq, dk, dv = (torch.zeros(t.shape, dtype=out_dt, device=q.device) for t in (q, k, v))
     l2 = lse2_of(case["lse"]).double()
     info: dict = {}
-    for q0, q1, k0, k1 in vo.seqs(case["cu_q"].cpu(), case["cu_k"].cpu()):
+    for q0, q1, k0, k1 in ar.seqs(case["cu_q"].cpu(), case["cu_k"].cpu()):
         if q1 == q0 or k1 == k0:
             continue
         seq = lambda t, a, b: t[a:b].double().transpose(0, 1)  # noqa: E731
         (a, b, c), inf = gb.closed_form_core(
             seq(q, q0, q1), seq(k, k0, k1), seq(v, k0, k1), seq(o, q0, q1), seq(do, q0, q1), l2[q0:q1].t(),
-            vo.visible(q1 - q0, k1 - k0, case["causal"], q.device), case["scale"], q.dtype, rounded, group=H // H_kv)
+            ar.visible(q1 - q0, k1 - k0, k1 - k0 - (q1 - q0) if case["causal"] else None, q.device), case["scale"],
+            q.dtype, rounded, group=H // H_kv)
         dq[q0:q1], dk[k0:k1], dv[k0:k1] = a.transpose(0, 1), b.transpose(0, 1), c.transpose(0, 1)
         for key, val in inf.items():
             info[key] = max(info.get(key, 0), val) if key.startswith("win") else info.get(key, 0) + val

@@ -1,12 +1,12 @@
 """CPU reference for KV-cache decode with append and rotary (b200k_fa2_fwd_kvcache_append), used by
-test_attention_kvcache_append_cpu.py and test_gpu_attention_kvcache_append.py.  Built on kvcache_oracle: the new rows
-are rotated in fp64 and rounded once to the dtype, written into a copy of the cache through the table, and
-kvcache_oracle.attention_kvcache runs on the rotated Q with the lengths plus L_new."""
+test_attention_kvcache_append_cpu.py and test_gpu_attention_kvcache_append.py.  The new rows are rotated in fp64 and
+rounded once to the dtype, written into a copy of the cache through the table, and attention_ref.kvcache runs on the
+rotated Q with the lengths plus L_new."""
 from __future__ import annotations
 
 import torch
 
-import kvcache_oracle
+import attention_ref
 
 
 def rotate(x: torch.Tensor, cos: torch.Tensor, sin: torch.Tensor, pos: torch.Tensor, interleaved: bool) -> torch.Tensor:
@@ -76,5 +76,5 @@ def attention_append(q, k_cache, v_cache, cache_seqlens, k_new, v_new, block_tab
     vc = write(v_cache, v_new, cache_seqlens, block_table)
     cap = kc.size(1) * (1 if block_table is None else block_table.size(1))
     lens = (base + L_new).clamp(max=cap).to(torch.int32)
-    o = kvcache_oracle.attention_kvcache(q.cpu(), kc, vc, lens, block_table, scale=scale, causal=causal)
+    o = attention_ref.kvcache(q.cpu(), kc, vc, lens, block_table, scale=scale, causal=causal)[0].to(q.dtype)
     return o, kc, vc

@@ -1,12 +1,9 @@
-"""CPU reference for KV-cache decode attention (b200k_fa2_fwd_kvcache), used by test_attention_kvcache_cpu.py and
-test_gpu_attention_kvcache.py.  No new oracle: each sequence's keys are gathered from the cache through its block table
-into packed K/V with cu_seqlens, and varlen_oracle.attention_varlen computes the attention, with Q [B, Lq, H, D] as
-B packed sequences of Lq tokens."""
+"""KV caches for decode attention (b200k_fa2_fwd_kvcache): each sequence's keys gathered from the cache through its block
+table into packed K/V with cu_seqlens (attention_ref.kvcache attends over them), and a contiguous cache copied into the
+pages of a shuffled table."""
 from __future__ import annotations
 
 import torch
-
-import varlen_oracle
 
 
 def gather(k_cache: torch.Tensor, v_cache: torch.Tensor, cache_seqlens, block_table=None):
@@ -28,17 +25,6 @@ def gather(k_cache: torch.Tensor, v_cache: torch.Tensor, cache_seqlens, block_ta
             vs.append(vc[page, slot])
     cu = torch.tensor([0] + torch.tensor(lens, dtype=torch.int64).cumsum(0).tolist(), dtype=torch.int32)
     return torch.cat(ks), torch.cat(vs), cu
-
-
-def attention_kvcache(q: torch.Tensor, k_cache, v_cache, cache_seqlens, block_table=None, scale=None,
-                      causal: bool = False) -> torch.Tensor:
-    """O [B, Lq, H, D] in q's dtype, on the CPU: token t of sequence b sees key j iff j <= t + Lk_b - Lq when causal;
-    rows that see no key are 0."""
-    B, Lq, H, D = q.shape
-    k, v, cu_k = gather(k_cache, v_cache, cache_seqlens, block_table)
-    cu_q = torch.arange(B + 1, dtype=torch.int32) * Lq
-    out = varlen_oracle.attention_varlen(q.cpu().reshape(B * Lq, H, D), k, v, cu_q, cu_k, scale=scale, causal=causal)
-    return out.view(B, Lq, H, D)
 
 
 def paged_copy(k_cache: torch.Tensor, v_cache: torch.Tensor, page_size: int, spare_pages: int = 3, seed: int = 0,

@@ -1,5 +1,5 @@
-"""CPU: the attention backward.  The fp64 reference (attn_bwd_oracle.py) against torch.autograd on its own forward and
-gradcheck; every argument check of b200k_fa2_bwd before any CUDA call (fake pointers, never dereferenced); the workspace
+"""CPU: the attention backward.  The fp64 reference (attention_ref.py, dense layout) against torch.autograd on its own
+forward and gradcheck; every argument check of b200k_fa2_bwd before any CUDA call (fake pointers, never dereferenced); the workspace
 size; the checks of the fa2_bwd wrapper."""
 import ctypes
 import os
@@ -9,7 +9,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import attn_bwd_oracle as bo  # noqa: E402
+import attention_ref as ar  # noqa: E402
 
 from b200k import _loader as L  # noqa: E402
 
@@ -23,9 +23,9 @@ def test_reference_gradients_are_torch_autograd_of_the_reference_forward(causal,
     B, H, N, D = 2, 3, 7, 8
     q, k, v, do = [torch.randn(B, H, N, D, generator=g, dtype=torch.float64) for _ in range(4)]
     qa, ka, va = [t.clone().requires_grad_() for t in (q, k, v)]
-    o, lse = bo.forward(qa, ka, va, 0.3, causal, seqlens)
+    o, lse = ar.dense(qa, ka, va, 0.3, causal, seqlens)
     o.backward(do)
-    dq, dk, dv, o64, lse64 = bo.grads(q, k, v, do, 0.3, causal, seqlens)
+    dq, dk, dv, o64, lse64 = ar.dense_grads(q, k, v, do, 0.3, causal, seqlens)
     for got, want in ((dq, qa.grad), (dk, ka.grad), (dv, va.grad), (o64, o), (lse64, lse)):
         assert torch.allclose(got, want.detach(), rtol=1e-12, atol=1e-12)
     # keys no row sees have zero dK and dV
@@ -38,7 +38,7 @@ def test_reference_gradients_are_torch_autograd_of_the_reference_forward(causal,
 def test_reference_forward_passes_gradcheck(causal):
     g = torch.Generator().manual_seed(2)
     q, k, v = [torch.randn(2, 1, 5, 4, generator=g, dtype=torch.float64, requires_grad=True) for _ in range(3)]
-    assert torch.autograd.gradcheck(lambda a, b, c: bo.forward(a, b, c, None, causal, SL)[0], (q, k, v))
+    assert torch.autograd.gradcheck(lambda a, b, c: ar.dense(a, b, c, None, causal, SL)[0], (q, k, v))
 
 
 # ------------------------------------------------------------------------------------------------ the C entry points

@@ -1,5 +1,5 @@
 """CPU: the constructions of graded_attention_bwd.py.  The lse and scale identities hold (and the targets with no exact
-lse are the known ones); the closed form is attn_bwd_oracle.grads_given within fp64; the three kernels' arithmetic,
+lse are the known ones); the closed form is attention_ref.dense_grads_given within fp64; the three kernels' arithmetic,
 emulated in fp32, gives the closed form bit for bit on every case the GPU test runs; the rounding paths are exercised;
 and each way the backward could be subtly wrong (graded_attention_bwd.MUTATIONS) changes at least one expected bit of
 one of those cases:
@@ -28,7 +28,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import attn_bwd_oracle as bo  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import graded_attention as ga  # noqa: E402
 import graded_attention_bwd as gb  # noqa: E402
 
@@ -116,7 +116,7 @@ def _check_grads_given(x, args):
     got, _ = gb.closed_form(*args, rounded=False)
     sl2 = float(np.float32(scale) * np.float32(ga.LOG2E_F32))
     lse_n = torch.from_numpy(gb.lse2_of(lse.numpy())).double() * math.log(2)
-    want = bo.grads_given(q, k, v, o, lse_n, do, sl2 * math.log(2), causal, sl)
+    want = ar.dense_grads_given(q, k, v, o, lse_n, do, sl2 * math.log(2), causal, sl)
     for a, w in zip(got, want):
         assert torch.allclose(a, w, rtol=1e-12, atol=1e-12 * float(w.abs().max() + 1))
 

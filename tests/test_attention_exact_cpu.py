@@ -1,7 +1,7 @@
-"""CPU: the exact-answer construction of exact_attention.py against varlen_oracle.attention_varlen (fp32 softmax,
-rounded once) on packed sequences with grouped K/V heads, empty sequences, Lq != Lk, causal and decoy needles in the
+"""CPU: the exact-answer construction of exact_attention.py against attention_ref.packed (fp64, rounded once)
+on packed sequences with grouped K/V heads, empty sequences, Lq != Lk, causal and decoy needles in the
 next sequence's first key.  Needle rows and rows that see no key agree bit for bit; rows that average their keys agree
-within one ulp of the dtype (the oracle's fp32 softmax weights are 1 / n rounded, summed in its own order) plus 2^-20
+within one ulp of the dtype (the reference's weights are 1 / n rounded, summed in its own order) plus 2^-20
 for sums that cancel to 0."""
 import os
 import sys
@@ -10,8 +10,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the helpers sit next to this file
+import attention_ref as ar  # noqa: E402
 import exact_attention as ex  # noqa: E402
-import varlen_oracle  # noqa: E402
 
 
 def pack(lq, lk, H, H_kv, D, dtype, causal, seed):
@@ -56,8 +56,7 @@ def test_closed_form_matches_the_varlen_oracle(D, dtype, causal):
     lq, lk = [5, 0, 40, 1, 33, 7], [9, 3, 0, 70, 33, 2]
     H, H_kv = 4, 2
     q, k, v, cu_q, cu_k, want, mean = pack(lq, lk, H, H_kv, D, dtype, causal, seed=D + causal)
-    src = (lambda t: t.double()) if dtype == torch.float16 else (lambda t: t)   # the oracle returns fp16 for fp64 input
-    ref = varlen_oracle.attention_varlen(src(q), src(k), src(v), cu_q, cu_k, causal=causal)
+    ref = ar.packed(q, k, v, cu_q, cu_k, causal=causal)[0].to(dtype)
     assert ref.dtype == dtype
     exact = ~mean
     assert int(exact.sum()) > 0 and int(mean.sum()) > 0

@@ -1,5 +1,5 @@
-"""CPU: the constructions of graded_attention.py.  The scale trick is exact; the closed form agrees with varlen_oracle and
-kvcache_oracle; the kernel's loop, emulated in fp32 at tile sizes 64, 128 and 192, gives the closed form bit for bit; and
+"""CPU: the constructions of graded_attention.py.  The scale trick is exact; the closed form agrees with attention_ref's packed
+and kvcache layouts; the kernel's loop, emulated in fp32 at tile sizes 64, 128 and 192, gives the closed form bit for bit; and
 each way the softmax could be subtly wrong (graded_attention.MUTATIONS) is rejected by one of the checks the GPU tests
 apply."""
 import os
@@ -10,10 +10,9 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the helpers and oracles sit next to this file
+import attention_ref as ar  # noqa: E402
 import exact_attention as ex  # noqa: E402
 import graded_attention as ga  # noqa: E402
-import kvcache_oracle  # noqa: E402
-import varlen_oracle  # noqa: E402
 
 DTYPES = [torch.float16, torch.bfloat16]
 EDGES = [0, 1, 15, 16, 63, 64, 127, 128, 129, 191, 192, 255, 256, 383, 384, 511, 512]   # as test_gpu_attention_exact.py
@@ -81,7 +80,7 @@ def _pack(X, lk, H_kv):
 @pytest.mark.parametrize("causal", [False, True])
 def test_closed_form_matches_the_varlen_and_kvcache_oracles(causal, dtype):
     """Packed sequences with grouped heads, and the same blocks as a KV cache with lengths below the capacity (so the
-    decoy column's key exists).  The oracles' softmax is fp32 and natural-base: one ulp of the dtype plus 2^-20."""
+    decoy column's key exists).  The reference's softmax is natural-base: one ulp of the dtype plus 2^-20."""
     g = torch.Generator().manual_seed(5 + causal)
     lq, lk, H, H_kv, D, L, k = [5, 0, 40, 1, 70], [9, 3, 0, 70, 130], 4, 2, 32, 140, 2
     B, W = len(lq), ga.window(L)
@@ -98,9 +97,8 @@ def test_closed_form_matches_the_varlen_and_kvcache_oracles(causal, dtype):
     n = (tok - cu_q[b] + Lk - Lq + 1).clamp(min=0).minimum(Lk) if causal else Lk
     blk = b * H_kv + h // (H // H_kv)
     want, info = ga.expected(G, V, blk, n, cols, dtype)
-    src = (lambda t: t.double()) if dtype == torch.float16 else (lambda t: t)   # the oracle returns fp16 for fp64 input
-    ref = varlen_oracle.attention_varlen(src(q), src(_pack(G.to(dtype), lk, H_kv)), src(_pack(V, lk, H_kv)), cu_q, cu_k,
-                                         scale=ga.scale_exact(k), causal=causal)
+    ref = ar.packed(q, _pack(G.to(dtype), lk, H_kv), _pack(V, lk, H_kv), cu_q, cu_k, scale=ga.scale_exact(k),
+                    causal=causal)[0].to(dtype)
     tol = ga.ulp(want, dtype) + 2.0 ** -20
     assert bool(((ref.view(-1, D).float() - want.float()).abs() <= tol).all())
     assert int(info["decoyed"].sum()) > 0 and int((n == 0).sum()) > 0
@@ -111,8 +109,7 @@ def test_closed_form_matches_the_varlen_and_kvcache_oracles(causal, dtype):
             continue
         rows = (b == bb)
         qd = q[cu_q[bb]:cu_q[bb + 1]].view(1, lq[bb], H, D)
-        ref = kvcache_oracle.attention_kvcache(src(qd), src(kc[bb:bb + 1]), src(vc[bb:bb + 1]), [lk[bb]],
-                                               scale=ga.scale_exact(k), causal=causal)
+        ref = ar.kvcache(qd, kc[bb:bb + 1], vc[bb:bb + 1], [lk[bb]], scale=ga.scale_exact(k), causal=causal)[0].to(dtype)
         assert bool(((ref.view(-1, D).float() - want[rows].float()).abs() <= tol[rows]).all())
 
 

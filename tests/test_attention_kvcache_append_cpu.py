@@ -10,6 +10,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the oracles sit next to this file
+import attention_ref as ar  # noqa: E402
 import kvcache_append_oracle as ko  # noqa: E402
 import kvcache_oracle  # noqa: E402
 
@@ -223,7 +224,7 @@ def test_rows_land_in_their_page_slots_under_a_shuffled_table(page_size):
 
 
 def test_reference_attends_over_old_and_new_keys():
-    """Lengths are taken as base + L_new, with negative lengths as 0, and the result equals kvcache_oracle on a cache
+    """Lengths are taken as base + L_new, with negative lengths as 0, and the result equals attention_ref.kvcache on a cache
     that already holds the new rows."""
     B, Lq, H, H_kv, D, S = 2, 2, 4, 2, 32, 64
     g = torch.Generator().manual_seed(7)
@@ -233,5 +234,5 @@ def test_reference_attends_over_old_and_new_keys():
     lens = torch.tensor([-4, 10], dtype=torch.int32)
     o, k2, v2 = ko.attention_append(q, kc, vc, lens, kn, vn, causal=True)
     assert torch.equal(k2[0, :3], kn[0]) and torch.equal(k2[1, 10:13], kn[1]) and torch.equal(k2[1, :10], kc[1, :10])
-    want = kvcache_oracle.attention_kvcache(q, k2, v2, torch.tensor([3, 13], dtype=torch.int32), causal=True)
+    want = ar.kvcache(q, k2, v2, torch.tensor([3, 13], dtype=torch.int32), causal=True)[0].half()
     assert torch.equal(o, want)

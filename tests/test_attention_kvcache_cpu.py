@@ -9,6 +9,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # kvcache_oracle.py sits next to this file
+import attention_ref as ar  # noqa: E402
 import kvcache_oracle  # noqa: E402
 
 from b200k import _loader as L
@@ -142,7 +143,7 @@ def test_reference_is_varlen_with_lq_tokens_per_sequence():
     q = torch.randn(B, Lq, H, D, generator=g).half()
     kc, vc = [torch.randn(B, 40, H_kv, D, generator=g).half() for _ in range(2)]
     lens = torch.tensor([2, 40], dtype=torch.int32)
-    o = kvcache_oracle.attention_kvcache(q, kc, vc, lens, causal=True)
+    o = ar.kvcache(q, kc, vc, lens, causal=True)[0].half()
     assert o.shape == q.shape
     assert (o[0, 0] == 0).all()                                 # token 0 of sequence 0 sees keys <= 0 + 2 - 3 < 0
     assert torch.equal(o[0, 1], vc[0, 0].repeat_interleave(2, dim=0))   # token 1 sees exactly key 0

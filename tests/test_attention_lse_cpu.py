@@ -1,6 +1,6 @@
 """CPU: the log-sum-exp outputs of the attention calls and b200k_attn_merge.  Argument checks of every new entry point
-(before any CUDA call) and of the ``lse=`` / attn_merge wrappers; the fp64 reference (lse_oracle.py) against
-torch.logsumexp and a direct sum, merging by it; and lse_oracle.emulate_lse(), the lse of
+(before any CUDA call) and of the ``lse=`` / attn_merge wrappers; the fp64 reference (attention_ref.py) against
+torch.logsumexp and a direct sum, merging by it (lse_oracle.merge); and lse_oracle.emulate_lse(), the lse of
 graded_attention.emulate()'s fp32 loop, against it."""
 import ctypes
 import math
@@ -12,9 +12,9 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import attention_ref as ar  # noqa: E402
 import graded_attention as ga  # noqa: E402
 import lse_oracle  # noqa: E402
-import varlen_oracle  # noqa: E402
 
 from b200k import _loader as L  # noqa: E402
 
@@ -163,11 +163,11 @@ def _packed(seed, lens_q, lens_k, H=4, H_kv=2, D=32, extra_q=3):
 
 @pytest.mark.parametrize("causal", [False, True])
 def test_reference_lse_is_the_log_of_the_softmax_denominator(causal):
-    """lse_varlen against a direct fp64 sum per row; -inf for rows that see no key (Lk = 0, causal rows above the
-    bottom-right diagonal), NaN for tokens outside every sequence; lse_dense and lse_kvcache are the same rule."""
+    """The packed lse against a direct fp64 sum per row; -inf for rows that see no key (Lk = 0, causal rows above the
+    bottom-right diagonal) and for tokens outside every sequence; the dense lse is the same rule."""
     lens_q, lens_k = [5, 0, 7, 3], [9, 4, 0, 2]
     q, k, v, cq, ck = _packed(1, lens_q, lens_k)
-    got = lse_oracle.lse_varlen(q, k, cq, ck, causal=causal)
+    got = ar.packed(q, k, v, cq, ck, causal=causal)[1]
     H, D = q.shape[1], q.shape[2]
     for b in range(len(lens_q)):
         for r in range(lens_q[b]):
@@ -177,12 +177,12 @@ def test_reference_lse_is_the_log_of_the_softmax_denominator(causal):
                 s = [float(q[t, h].double() @ k[int(ck[b]) + j, h // 2].double()) / math.sqrt(D) for j in keys]
                 want = math.log(sum(math.exp(x) for x in s)) if s else float("-inf")
                 assert got[t, h].item() == pytest.approx(want, rel=1e-12, abs=1e-12) if s else got[t, h] == want
-    assert torch.isnan(got[int(cq[-1]):]).all()
+    assert (got[int(cq[-1]):] == float("-inf")).all()
     assert (got[int(cq[2]):int(cq[3])] == float("-inf")).all()
     # dense: the same rule with a key-padding mask, against torch.logsumexp of the masked scores
     qd, kd = torch.randn(2, 3, 10, 16, dtype=torch.float64), torch.randn(2, 3, 10, 16, dtype=torch.float64)
     sl = torch.tensor([4, 10])
-    dense = lse_oracle.lse_dense(qd, kd, causal=causal, seqlens_k=sl)
+    dense = ar.dense(qd, kd, kd, causal=causal, seqlens_k=sl)[1]
     for b in range(2):
         for r in range(10):
             n = min(int(sl[b]), r + 1) if causal else int(sl[b])
@@ -217,13 +217,13 @@ def test_reference_merge_of_two_key_ranges_is_the_attention_over_their_union():
         return out
 
     o1, o2, o = attn64(k1, v1, lo), attn64(k2, v2, hi), attn64(k, v, ck)
-    l1 =lse_oracle.lse_varlen(q, k1, cq, lo)
-    l2 = lse_oracle.lse_varlen(q, k2, cq, hi)
+    l1 = ar.packed(q, k1, v1, cq, lo)[1]
+    l2 = ar.packed(q, k2, v2, cq, hi)[1]
     assert (l1[int(cq[1]):int(cq[2])] == float("-inf")).all()       # sequence 1 has no key in its first range
     o1[int(cq[1]):int(cq[2])] = float("nan")
     mo, ml = lse_oracle.merge(torch.stack([o1, o2]), torch.stack([l1, l2]))
     assert torch.allclose(mo, o, rtol=1e-12, atol=1e-12)
-    assert torch.allclose(ml, lse_oracle.lse_varlen(q, k, cq, ck), rtol=1e-12, atol=1e-12)
+    assert torch.allclose(ml, ar.packed(q, k, v, cq, ck)[1], rtol=1e-12, atol=1e-12)
     mo, ml = lse_oracle.merge(torch.full((2, 1, 4), float("nan")), torch.full((2, 1), float("-inf")))
     assert (mo == 0).all() and (ml == float("-inf")).all()
 

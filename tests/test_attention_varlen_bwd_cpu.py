@@ -1,5 +1,5 @@
-"""CPU: the fp64 reference of the packed attention backward (varlen_bwd_oracle.py) against torch autograd, gradcheck and
-the dense reference; b200k_fa2_bwd_varlen's argument checks, all made before any CUDA call (fake pointers, never
+"""CPU: the fp64 reference of the packed attention backward (attention_ref.py, packed layout) against torch autograd and
+gradcheck; b200k_fa2_bwd_varlen's argument checks, all made before any CUDA call (fake pointers, never
 dereferenced); and ops.fa2_bwd_varlen's checks."""
 import ctypes
 import os
@@ -9,14 +9,9 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import attn_bwd_oracle as bo  # noqa: E402
-import varlen_bwd_oracle as vo  # noqa: E402
+import attention_ref as ar  # noqa: E402
 
 from b200k import _loader as L  # noqa: E402
-
-
-def _cu(lens):
-    return torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32)
 
 
 def _inputs(lq, lk, H, H_kv, D, seed):
@@ -31,8 +26,8 @@ def _inputs(lq, lk, H, H_kv, D, seed):
 def test_reference_gradients_are_torch_autograd_of_the_reference_forward(causal, lq, lk, H, H_kv):
     q, k, v, do = _inputs(lq, lk, H, H_kv, 8, sum(lq) + H)
     qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))
-    vo.forward(qa, ka, va, _cu(lq), _cu(lk), None, causal)[0].backward(do)
-    got = vo.grads(q, k, v, do, _cu(lq), _cu(lk), None, causal)[:3]
+    ar.packed(qa, ka, va, ar.cu(lq), ar.cu(lk), None, causal)[0].backward(do)
+    got = ar.packed_grads(q, k, v, do, ar.cu(lq), ar.cu(lk), None, causal)[:3]
     for a, r in zip(got, (qa.grad, ka.grad, va.grad)):
         assert torch.allclose(a, r, rtol=1e-10, atol=1e-12)
 
@@ -42,19 +37,8 @@ def test_reference_forward_passes_gradcheck():
     for t in (q, k, v):
         t.requires_grad_()
     for causal in (False, True):
-        assert torch.autograd.gradcheck(lambda a, b, c: vo.forward(a, b, c, _cu((3, 2)), _cu((2, 4)), None, causal)[0],
+        assert torch.autograd.gradcheck(lambda a, b, c: ar.packed(a, b, c, ar.cu((3, 2)), ar.cu((2, 4)), None, causal)[0],
                                         (q, k, v))
-
-
-@pytest.mark.parametrize("causal", [False, True], ids=["full", "causal"])
-def test_equal_length_mha_is_the_dense_reference(causal):
-    B, H, N, D = 3, 2, 9, 8
-    q, k, v, do = _inputs((N,) * B, (N,) * B, H, H, D, 5)
-    dense = [t.view(B, N, H, D).transpose(1, 2) for t in (q, k, v, do)]
-    want = bo.grads(*dense, None, causal)[:3]
-    got = vo.grads(q, k, v, do, _cu((N,) * B), _cu((N,) * B), None, causal)[:3]
-    for a, w in zip(got, want):
-        assert torch.allclose(a.view(B, N, H, D).transpose(1, 2), w, rtol=1e-12, atol=1e-12)
 
 
 def test_explicit_edges_are_zero_not_nan():
@@ -63,7 +47,7 @@ def test_explicit_edges_are_zero_not_nan():
     q, k, v, do = _inputs(lq, lk, 4, 2, 8, 9)
     q, do = (torch.cat([t, torch.randn(2, 4, 8, dtype=torch.float64)]) for t in (q, do))
     for causal in (False, True):
-        dq, dk, dv, o, lse = vo.grads(q, k, v, do, _cu(lq), _cu(lk), None, causal)
+        dq, dk, dv, o, lse = ar.packed_grads(q, k, v, do, ar.cu(lq), ar.cu(lk), None, causal)
         for t in (dq, dk, dv, o):
             assert not torch.isnan(t).any()
         assert (dk[3:8] == 0).all() and (dv[3:8] == 0).all()        # Lq = 0

@@ -1,4 +1,4 @@
-"""CPU: the constructions of graded_attention_varlen_bwd.py.  The closed form is varlen_bwd_oracle.grads_given within fp64;
+"""CPU: the constructions of graded_attention_varlen_bwd.py.  The closed form is attention_ref.packed_grads_given within fp64;
 the three kernels' arithmetic, emulated in fp32 at tile granularity, gives the closed form bit for bit on every case the
 GPU test runs; the rounding paths and the group sums are exercised; and each way the packed backward could be subtly
 wrong (graded_attention_varlen_bwd.MUTATIONS) changes at least one expected bit of one of those cases.  Besides the
@@ -29,10 +29,10 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import attention_ref as ar  # noqa: E402
 import graded_attention as ga  # noqa: E402
 import graded_attention_bwd as gb  # noqa: E402
 import graded_attention_varlen_bwd as gv  # noqa: E402
-import varlen_bwd_oracle as vo  # noqa: E402
 
 CASES = gv.all_cases() + [gv.grid_case(), gv.big_core()]
 _EXPECTED: dict = {}
@@ -69,8 +69,8 @@ def test_closed_form_is_grads_given(x):
     got, _ = gv.closed_form(x, rounded=False)
     sl2 = float(np.float32(x["scale"]) * np.float32(ga.LOG2E_F32))
     lse_n = torch.from_numpy(gb.lse2_of(x["lse"].numpy())).double() * math.log(2)
-    want = vo.grads_given(x["q"], x["k"], x["v"], x["o"], lse_n, x["do"], x["cu_q"], x["cu_k"], sl2 * math.log(2),
-                          x["causal"])
+    want = ar.packed_grads_given(x["q"], x["k"], x["v"], x["o"], lse_n, x["do"], x["cu_q"], x["cu_k"], sl2 * math.log(2),
+                                 x["causal"])
     for a, w in zip(got, want):
         assert torch.allclose(a, w, rtol=1e-12, atol=1e-12 * float(w.abs().max() + 1))
     if x["causal"]:

@@ -1,5 +1,5 @@
 """CPU: argument validation of the packed variable-length attention entry point (before any CUDA call), the Python
-wrapper's checks, and the CPU reference `varlen_oracle.attention_varlen` against the dense oracle and against
+wrapper's checks, and the packed layout of the CPU reference (attention_ref.py) against the dense oracle and against
 per-sequence SDPA."""
 import ctypes
 import os
@@ -9,8 +9,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # varlen_oracle.py sits next to this file
-import varlen_oracle  # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # attention_ref.py sits next to this file
+import attention_ref as ar  # noqa: E402
 
 from b200k import _loader as L
 from oracle import oracle
@@ -105,7 +105,7 @@ def test_oracle_equal_lengths_matches_dense_oracle(dtype, causal):
     want = oracle.attention(q, k, v, causal=causal)                                  # [B, H, N, D]
     packed = [t.transpose(1, 2).reshape(B * N, H, D) for t in (q, k, v)]
     cu = torch.arange(0, (B + 1) * N, N, dtype=torch.int32)
-    got = varlen_oracle.attention_varlen(*packed, cu, cu, causal=causal)
+    got = ar.packed(*packed, cu, cu, causal=causal)[0].to(dtype)
     assert got.dtype == dtype
     assert torch.allclose(got.float(), want.transpose(1, 2).reshape(B * N, H, D).float(), rtol=1e-2, atol=1e-3)
 
@@ -138,7 +138,7 @@ def test_oracle_matches_sdpa_gqa_with_bottom_right_mask(lq, lk, H, H_kv, causal)
     q, cq = _pack(lq, H, D, torch.float16, seed=sum(lq) + H)
     k, ck = _pack(lk, H_kv, D, torch.float16, seed=sum(lk) + H_kv)
     v, _ = _pack(lk, H_kv, D, torch.float16, seed=sum(lk) + 7)
-    got = varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=causal)
+    got = ar.packed(q, k, v, cq, ck, causal=causal)[0].half()
     want = _sdpa_per_sequence(q, k, v, cq.tolist(), ck.tolist(), causal).half()
     assert torch.allclose(got.float(), want.float(), rtol=1e-3, atol=1e-3)
 
@@ -149,13 +149,13 @@ def test_oracle_rows_that_see_no_key_are_zero():
     q, cq = _pack(lq, H, D, torch.float16, seed=1)
     k, ck = _pack(lk, H, D, torch.float16, seed=2)
     v, _ = _pack(lk, H, D, torch.float16, seed=3)
-    o = varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=True)
+    o = ar.packed(q, k, v, cq, ck, causal=True)[0].half()
     assert torch.isfinite(o.float()).all()
     assert (o[0:4] == 0).all()                 # sequence 0: Lq - Lk = 4 rows before the first key
     assert (o[4:6] != 0).any()
     assert (o[6:10] == 0).all()                # sequence 1: no keys at all
     assert (o[10:13] != 0).any()
-    o = varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=False)
+    o = ar.packed(q, k, v, cq, ck, causal=False)[0].half()
     assert (o[6:10] == 0).all() and (o[0:6] != 0).any()
     # a row that sees exactly one key returns that key's V row
-    assert torch.equal(varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=True)[4], v[0])
+    assert torch.equal(ar.packed(q, k, v, cq, ck, causal=True)[0][4].half(), v[0])

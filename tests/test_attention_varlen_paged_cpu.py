@@ -1,6 +1,6 @@
 """CPU: argument validation of packed attention over paged caches (b200k_fa2_varlen_paged) before any CUDA call, the
-Python wrapper's checks for ops.fa2_fwd_varlen(..., block_table=), and the gather-through-table reference
-(varlen_paged_oracle + varlen_oracle) against a per-sequence reference that reads every key from its page."""
+Python wrapper's checks for ops.fa2_fwd_varlen(..., block_table=), and the paged layout of the reference
+(attention_ref.paged, which gathers through the table) against the packed layout on the keys the pages were made from."""
 import ctypes
 import os
 import sys
@@ -9,7 +9,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the oracles sit next to this file
-import varlen_oracle  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import varlen_paged_oracle as vpo  # noqa: E402
 
 from b200k import _loader as L
@@ -138,16 +138,18 @@ def _pack(lq, lk, H, H_kv, D, seed):
 
 @pytest.mark.parametrize("page_size", [16, 64])
 @pytest.mark.parametrize("causal", [False, True])
-def test_gather_oracle_matches_pages_oracle(page_size, causal):
+def test_paged_reference_reads_the_packed_keys_through_the_table(page_size, causal):
     """Shuffled tables with unlisted pages, Lk not a multiple of the page size, Lk = 0, an empty query sequence, Lq > Lk,
-    and a length past the table's capacity (clamped)."""
+    and a length past the table's capacity (clamped): the paged reference is the packed one on the keys the pages were
+    made from, the last sequence's cut to the capacity."""
     lq, lk = [7, 0, 20, 5, 9], [40, 3, 0, 5, 100]
     q, k, v, cq, ck = _pack(lq, lk, 4, 2, 32, seed=page_size + causal)
     kc, vc, table = vpo.to_pages(k, v, ck, page_size, pages_per_seq=80 // page_size, fill=float("nan"), seed=3)
-    kg, vg, cg = vpo.gather(kc, vc, ck, table)
-    assert vpo.lengths(ck, table.size(1) * page_size)[-1] == table.size(1) * page_size
-    want = varlen_oracle.attention_varlen(q, kg, vg, cq, cg, causal=causal).double()
-    ref, lse = vpo.attention_pages(q, kc, vc, cq, ck, table, causal=causal)
+    cap = table.size(1) * page_size
+    assert vpo.lengths(ck, cap)[-1] == cap
+    cut = ar.cu(lk[:-1] + [cap])
+    want = ar.packed(q, k[:int(cut[-1])], v[:int(cut[-1])], cq, cut, causal=causal)[0].half().double()
+    ref, lse = ar.paged(q, kc, vc, cq, ck, table, causal=causal)
     assert torch.isfinite(ref).all()
     assert torch.allclose(want, ref, rtol=1e-2, atol=1e-3)
     if causal:
@@ -164,6 +166,6 @@ def test_shared_prefix_pages():
     assert (table[0, :2] == table[1, :2]).all()
     kg, vg, cg = vpo.gather(kc, vc, ck, table)
     assert torch.equal(kg, k) and torch.equal(vg, v)
-    want = varlen_oracle.attention_varlen(q, kg, vg, cq, cg).double()
-    ref, _ = vpo.attention_pages(q, kc, vc, cq, ck, table)
+    want = ar.packed(q, k, v, cq, ck)[0].half().double()
+    ref, _ = ar.paged(q, kc, vc, cq, ck, table)
     assert torch.allclose(want, ref, rtol=1e-2, atol=1e-3)

@@ -2,7 +2,7 @@
 
   - exact answers on the needle inputs of exact_attention.py with every row's needle visible: dQ = dK = 0 and dV_j = the
     sum of the dO rows whose needle is j, bit for bit;
-  - random inputs against the fp64 reference (attn_bwd_oracle.py) by flash-attn's rule: the error is at most twice
+  - random inputs against the fp64 reference (attention_ref.py) by flash-attn's rule: the error is at most twice
     that of the same math in the input dtype through torch autograd, plus one ulp of the dtype;
   - two calls and a CUDA-graph replay give the same bits; outputs go into NaN-filled buffers with guards, exactly the
     documented elements change and the inputs do not;
@@ -16,7 +16,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import attn_bwd_oracle as bo  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import exact_attention as ea  # noqa: E402
 
 from b200k import ops  # noqa: E402
@@ -118,17 +118,10 @@ def _check_against_fp64(got, ref, g64, what):
 
 
 def _torch_grads(q, k, v, do, scale, causal, sl):
-    """The same math in q's dtype through torch autograd (the reference forward, masked softmax)."""
+    """The same math in q's dtype through torch autograd (the reference forward)."""
     qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))
-    bo.forward(qa, ka, va, scale, causal, sl)[0].backward(do)
+    ar.dense(qa, ka, va, scale, causal, sl, q.dtype)[0].backward(do)
     return qa.grad, ka.grad, va.grad
-
-
-def _grads64(q, k, v, do, scale, causal, sl):
-    """attn_bwd_oracle.grads one batch at a time (the fp64 score matrices of the largest shape do not fit at once)."""
-    parts = [bo.grads(q[b:b + 1], k[b:b + 1], v[b:b + 1], do[b:b + 1], scale, causal,
-                      sl[b:b + 1] if sl is not None else None)[:3] for b in range(q.size(0))]
-    return [torch.cat(x) for x in zip(*parts)]
 
 
 RANDOM = [(1, 2, 64, 32, None), (2, 3, 77, 64, (50, 77)), (1, 4, 200, 96, None), (2, 2, 333, 128, (333, 100)),
@@ -146,7 +139,7 @@ def test_random_against_fp64(dtype, causal, B, H, N, D, lens):
     o, lse = _fwd(q, k, v, scale, causal, sl)
     got, _ = _bwd(q, k, v, o, lse, do, scale, causal, sl)
     assert all(bool(torch.isfinite(t).all()) for t in got)
-    g64 = _grads64(q, k, v, do, scale, causal, sl)
+    g64 = ar.dense_grads(q, k, v, do, scale, causal, sl)[:3]
     _check_against_fp64(got, _torch_grads(q, k, v, do, scale, causal, sl), g64, (B, H, N, D, lens))
 
 
@@ -203,7 +196,7 @@ def test_attention_autograd(dtype, causal, D):
         assert torch.equal(_bits(a), _bits(b))
     qs, ks, vs = (t.clone().requires_grad_() for t in (q, k, v))
     torch.nn.functional.scaled_dot_product_attention(qs, ks, vs, is_causal=causal).backward(do)
-    g64 = _grads64(q, k, v, do, None, causal, None)
+    g64 = ar.dense_grads(q, k, v, do, None, causal, None)[:3]
     _check_against_fp64((qa.grad, ka.grad, va.grad), (qs.grad, ks.grad, vs.grad), g64, ("sdpa", D))
     # a non-contiguous upstream gradient is made contiguous
     qa.grad = ka.grad = va.grad = None

@@ -17,15 +17,14 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the helpers and oracles sit next to this file
+import attention_ref as ar  # noqa: E402
 import exact_attention as ex  # noqa: E402
 import kvcache_append_oracle as ko  # noqa: E402
 import kvcache_oracle  # noqa: E402
-import varlen_oracle  # noqa: E402
 from oracle import oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DTYPES = [torch.float16, torch.bfloat16]
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
 EDGES = [0, 1, 15, 16, 63, 64, 127, 128, 129, 191, 192, 255, 256, 383, 384, 511, 512]   # box and tile edges
 CHUNK = 1 << 20   # rows per expected-value pass
 
@@ -437,7 +436,7 @@ def _scale_case(mode):
             o = torch.full_like(q, float("nan"))
             ops.fa2_fwd_varlen(q, k, v, o, cq, ck, max(lq), scale=scale, causal=True)
             return o
-        return D, torch.bfloat16, q, call, lambda q, s: varlen_oracle.attention_varlen(q, k, v, cq, ck, scale=s, causal=True)
+        return D, torch.bfloat16, q, call, lambda q, s: ar.packed(q, k, v, cq, ck, scale=s, causal=True)[0].to(q.dtype).cpu()
     if mode in ("decode_split", "decode"):
         B, H, H_kv, D, S = (2, 8, 2, 128, 2048) if mode == "decode_split" else (16, 32, 8, 64, 512)
         assert (_splits(B, 3, H, H_kv, D, S) > 1) == (mode == "decode_split")
@@ -448,7 +447,7 @@ def _scale_case(mode):
             o = torch.full_like(q, float("nan"))
             ops.fa2_fwd_kvcache(q, kc, vc, o, _i32(lens), causal=True, scale=scale)
             return o
-        return D, torch.float16, q, call, lambda q, s: kvcache_oracle.attention_kvcache(q, kc, vc, lens, scale=s, causal=True)
+        return D, torch.float16, q, call, lambda q, s: ar.kvcache(q, kc, vc, lens, scale=s, causal=True)[0].to(q.dtype)
     assert mode == "append_rotary"
     B, Lq, L_new, H, H_kv, D, S, ps = 3, 2, 2, 8, 2, 64, 256, 64
     kc, vc = rn(B, S, H_kv, D), rn(B, S, H_kv, D)
@@ -478,7 +477,7 @@ def test_scale_against_the_reference(mode, factor):
     scale = 1.0 if factor == "1.0" else factor / math.sqrt(D)
     o = call(q, scale)
     assert torch.isfinite(o).all()
-    assert torch.allclose(o.cpu().float(), ref(q, scale).float(), **TOL[dt])
+    assert torch.allclose(o.cpu().float(), ref(q, scale).float(), **ar.TOL[dt])
 
 
 @pytest.mark.parametrize("mode", SCALE_MODES)
@@ -508,7 +507,7 @@ def test_v_stored_dn_same_bits_as_v_stored_nd(D, causal, lens):
     o_nd, o_dn = torch.full_like(q, float("nan")), torch.full_like(q, float("nan"))
     ops.fa2_fwd(q, k, v, o_nd, causal=causal, seqlens_k=sl)
     ops.fa2_fwd(q, k, v.transpose(-1, -2).contiguous(), o_dn, v_is_dn=True, causal=causal, seqlens_k=sl)
-    assert torch.allclose(o_dn.cpu().float(), oracle.attention(q, k, v, causal=causal, seqlens=lens).float(), **TOL[torch.float16])
+    assert torch.allclose(o_dn.cpu().float(), oracle.attention(q, k, v, causal=causal, seqlens=lens).float(), **ar.TOL[torch.float16])
     assert torch.equal(o_dn, o_nd)
 
 

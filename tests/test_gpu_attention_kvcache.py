@@ -1,4 +1,4 @@
-"""GPU: KV-cache decode attention (ops.fa2_fwd_kvcache) against the CPU reference (kvcache_oracle.py), both sides of
+"""GPU: KV-cache decode attention (ops.fa2_fwd_kvcache) against the CPU reference (attention_ref.py), both sides of
 the split rule, bit equality with fa2_fwd_varlen / between paged and contiguous caches / between repeated calls,
 isolation from whatever the cache holds past each length, stores that stay inside O, CUDA graph replay while the
 cache grows, and a full-size run.  Tolerances are those of test_gpu_attention_varlen.py."""
@@ -10,10 +10,10 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # kvcache_oracle.py sits next to this file
+import attention_ref as ar  # noqa: E402
 import kvcache_oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
 LENS = [0, 1, 127, 128, 129, 3000]
 
 
@@ -44,8 +44,8 @@ def _ws(B, Lq, H, H_kv, D, cap):
 
 def _check(o, q, kc, vc, lens, table, causal, dtype):
     assert torch.isfinite(o).all()
-    want = kvcache_oracle.attention_kvcache(q, kc, vc, lens, table, causal=causal)
-    assert torch.allclose(o.cpu().float(), want.float(), **TOL[dtype])
+    want = ar.kvcache(q, kc, vc, lens, table, causal=causal)[0].to(q.dtype)
+    assert torch.allclose(o.cpu().float(), want.float(), **ar.TOL[dtype])
 
 
 @pytest.mark.parametrize("causal", [False, True])
@@ -278,4 +278,4 @@ def test_full_size_paged_gqa_properties():
             s = (qs @ ks.t()) / D ** 0.5
             s = s.masked_fill(j.view(1, n) > torch.arange(Lq, device="cuda").view(Lq, 1) + n - Lq, float("-inf"))
             want = torch.softmax(s, -1) @ vs
-            assert torch.allclose(o[b, :, h].float(), want, **TOL[torch.float16]), (b, h)
+            assert torch.allclose(o[b, :, h].float(), want, **ar.TOL[torch.float16]), (b, h)

@@ -11,11 +11,11 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import attention_ref as ar  # noqa: E402
 import kvcache_fp8_oracle as fo  # noqa: E402
 import kvcache_oracle  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
 NAN8 = 0x7F  # NaN in both formats
 
 
@@ -128,9 +128,9 @@ def test_arbitrary_scales_against_the_reference(dtype, fmt):
     lens = torch.tensor([1, 64, 1000, 1536], dtype=torch.int32, device="cuda")
     o = torch.empty_like(q)
     ops.fa2_fwd_kvcache(q, k8, v8, o, lens, table, causal=True, k_scale=ks, v_scale=vs)
-    want = kvcache_oracle.attention_kvcache(q, fo.dequantize(k8.cpu(), torch.float32, ks),
-                                            fo.dequantize(v8.cpu(), torch.float32, vs), lens, table, causal=True)
-    assert torch.allclose(o.cpu().float(), want.float(), **TOL[dtype])
+    want = ar.kvcache(q, fo.dequantize(k8.cpu(), torch.float32, ks), fo.dequantize(v8.cpu(), torch.float32, vs), lens,
+                      table, causal=True)[0].to(q.dtype)
+    assert torch.allclose(o.cpu().float(), want.float(), **ar.TOL[dtype])
 
 
 @pytest.mark.parametrize("fmt", fo.FORMATS, ids=["e4m3", "e5m2"])

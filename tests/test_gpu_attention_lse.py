@@ -13,6 +13,8 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import attention_poison as ap  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import exact_attention as ea  # noqa: E402
 import graded_attention as ga  # noqa: E402
 import kvcache_oracle  # noqa: E402
@@ -86,7 +88,7 @@ def test_dense_same_o_and_lse(D, dtype, causal, pad, v_dn):
     ops.fa2_fwd(q, k, vv, o1, v_is_dn=v_dn, causal=causal, seqlens_k=sl, lse=lse)
     torch.cuda.synchronize()
     assert torch.equal(o0, o1) and _guards_kept(buf)
-    want = lse_oracle.lse_dense(q, k, causal=causal, seqlens_k=sl)
+    want = ar.dense(q.cpu(), k.cpu(), v.cpu(), causal=causal, seqlens_k=sl)[1]
     _check_lse(lse, want, _random_bound(want, q, k, D ** -0.5, dtype))
 
 
@@ -110,7 +112,8 @@ def test_packed_same_o_and_lse(dtype, H, H_kv, causal):
     ops.fa2_fwd_varlen(q, k, v, o1, cq, ck, max(lq), causal=causal, lse=lse)
     torch.cuda.synchronize()
     assert _same_bits(o0, o1) and _guards_kept(buf)
-    want = lse_oracle.lse_varlen(q, k, cq, ck, causal=causal)
+    want = ar.packed(q.cpu(), k.cpu(), v.cpu(), cq, ck, causal=causal)[1]
+    want = ap.poison(want, ap.packed_masks(cq, ck, want.shape, k.shape)[0], float("nan"))  # past cu[B]: not written
     assert torch.isnan(want[-5:]).all() and (want[cq[1]:cq[2]] == float("-inf")).all()
     _check_lse(lse, want, _random_bound(want, q, k, D ** -0.5, dtype))
 
@@ -151,7 +154,7 @@ def test_decode_same_o_and_lse(B_split, page_size, causal):
     ops.fa2_fwd_kvcache(q, kc, vc, o1, lens, table, causal=causal, lse=lse)
     torch.cuda.synchronize()
     assert torch.equal(o0, o1) and _guards_kept(buf)
-    want = lse_oracle.lse_kvcache(q, kc, vc, lens, table, causal=causal)
+    want = ar.kvcache(q, kc, vc, lens, table, causal=causal)[1]
     _check_lse(lse, want, _random_bound(want, q, kc, D ** -0.5, dtype))
 
 
@@ -186,7 +189,7 @@ def test_append_same_o_and_lse(B, rotary):
     if rotary:   # the rotated q is not an output; every row sees the two new keys at least
         assert torch.isfinite(lse).all()
         return
-    want = lse_oracle.lse_kvcache(q, k1, v1, lens + 2, None, causal=True)
+    want = ar.kvcache(q, k1, v1, lens + 2, None, causal=True)[1]
     _check_lse(lse, want, _random_bound(want, q, k1, D ** -0.5, torch.float16))
 
 
@@ -422,13 +425,11 @@ def test_merge_of_split_key_ranges_matches_one_call(dtype):
     ops.attn_merge(torch.stack(parts), torch.stack(lps), om, lm)
     o1, l1 = torch.empty_like(q), torch.empty(q.shape[:2], device="cuda")
     ops.fa2_fwd_varlen(q, k, v, o1, cq, ck, max(lq), lse=l1)
-    want = lse_oracle.lse_varlen(q, k, cq, ck)
+    ref, want = ar.packed(q.cpu(), k.cpu(), v.cpu(), cq, ck)
     bound = _random_bound(want, q, k, D ** -0.5, dtype)
     _check_lse(lm, want, 2 * bound)
     _check_lse(l1, want, bound)
-    import varlen_oracle
-
-    ref = varlen_oracle.attention_varlen(q, k, v, cq, ck).float()
+    ref = ref.to(dtype).float()
     tol = dict(rtol=2e-2, atol=8e-3) if dtype == torch.bfloat16 else dict(rtol=1e-2, atol=2e-3)
     assert torch.allclose(om.cpu().float(), ref, **tol)
 
@@ -459,12 +460,11 @@ def test_cascade_decode_matches_full_cache():
     full_v = torch.cat([vp.expand(B, P, H_kv, D), vs], 1).contiguous()
     of, lf = torch.empty_like(q), torch.empty(B, Lq, H, device="cuda")
     ops.fa2_fwd_kvcache(q, full_k, full_v, of, lens + P, causal=True, lse=lf)
-    want = lse_oracle.lse_kvcache(q, full_k, full_v, lens + P, causal=True)
+    ref, want = ar.kvcache(q, full_k, full_v, lens + P, causal=True)
     bound = _random_bound(want, q, full_k, D ** -0.5, torch.float16)
     _check_lse(lm, want, 2 * bound)
     _check_lse(lf, want, bound)
-    ref = kvcache_oracle.attention_kvcache(q, full_k, full_v, lens + P, causal=True)
-    assert torch.allclose(om.cpu().float(), ref.float(), rtol=1e-2, atol=2e-3)
+    assert torch.allclose(om.cpu().float(), ref.half().float(), rtol=1e-2, atol=2e-3)
     assert torch.allclose(om.float(), of.float(), rtol=1e-2, atol=2e-3)
 
 
@@ -499,7 +499,7 @@ def test_cuda_graph_append_with_lse_while_the_cache_grows():
         ops.fa2_fwd_kvcache(q, kc, vc, o2, before, causal=True, k=kn, v=vn, lse=l2)
         torch.cuda.synchronize()
         assert torch.equal(o, o2) and torch.equal(lse, l2), step
-    want = lse_oracle.lse_kvcache(q, kc, vc, lens, causal=True)
+    want = ar.kvcache(q, kc, vc, lens, causal=True)[1]
     _check_lse(lse, want, _random_bound(want, q, kc, D ** -0.5, torch.float16))
 
 

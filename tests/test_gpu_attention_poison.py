@@ -21,17 +21,16 @@ import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import attention_poison as ap  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import exact_attention as ea  # noqa: E402
 import graded_attention_bwd as gb  # noqa: E402
 import test_gpu_attention_bwd as tb  # noqa: E402
 import test_gpu_attention_varlen_bwd as tvb  # noqa: E402
-import varlen_bwd_oracle as vo  # noqa: E402
 
 from b200k import ops  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 DTYPES = [torch.float16, torch.bfloat16]
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
 N = 200
 LENS = [1, 63, 64, 65, 127, 128, 129, N - 1, 0, -5]
 H = 2
@@ -91,8 +90,8 @@ def test_dense_forward_poisoned_keys(dtype, D, v_dn, causal):
     q, k, v, _, sl, m = _dense_inputs(dtype, D, seed=D + 2 * causal + v_dn)
     vt = (lambda t: t.transpose(-1, -2).contiguous()) if v_dn else (lambda t: t)  # noqa: E731
     clean, bufs = _dense_fwd(q, k, vt(v), sl, causal, v_dn)
-    o64, lse64 = ap.dense_forward(q, k, v, None, causal, sl)
-    assert torch.allclose(clean[0].float().cpu(), o64.to(dtype).float(), **TOL[dtype])
+    o64, lse64 = ar.dense(q.cpu(), k.cpu(), v.cpu(), None, causal, sl)
+    assert torch.allclose(clean[0].float().cpu(), o64.to(dtype).float(), **ar.TOL[dtype])
     assert torch.allclose(clean[1].double().cpu(), lse64, rtol=0, atol=1e-2)
     _guards_kept(bufs)
     mv = m.transpose(-1, -2) if v_dn else m
@@ -110,7 +109,7 @@ def test_dense_backward_poisoned_keys(dtype, D, causal):
     o, lse = (t.clone() for t in _dense_fwd(q, k, v, sl, causal)[0])  # O 16-byte aligned, as the backward needs
     clean, bufs = tb._bwd(q, k, v, o, lse, do, None, causal, sl)
     _guards_kept(bufs)
-    g64 = ap.dense_grads(q, k, v, do, None, causal, sl)[:3]
+    g64 = ar.dense_grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), None, causal, sl)[:3]
     _grad_rule(clean, tb._torch_grads(q, k, v, do, None, causal, sl), g64, "clean")
     for value in ap.VALUES:
         got, bufs = tb._bwd(q, ap.poison(k, m, value), ap.poison(v, m, value), o, lse, do, None, causal, sl)
@@ -179,17 +178,13 @@ def test_attention_autograd_poisoned_keys(dtype, causal):
 
 
 # ------------------------------------------------------------------------------------------------ packed
-def _cu(lens):
-    return tvb._cu(lens)
-
-
 def _packed_inputs(lq, lk, Hq, H_kv, D, dtype, seed):
     """q, k, v, do with PAD zero tokens past cu_seqlens[B], the cu_seqlens and the masks of the padding."""
     g = torch.Generator(device="cuda").manual_seed(seed)
     z = lambda h: torch.zeros(PAD, h, D, device="cuda", dtype=dtype)  # noqa: E731
     q, do = (torch.cat([torch.randn(sum(lq), Hq, D, generator=g, device="cuda").to(dtype), z(Hq)]) for _ in range(2))
     k, v = (torch.cat([torch.randn(sum(lk), H_kv, D, generator=g, device="cuda").to(dtype), z(H_kv)]) for _ in range(2))
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     mq, mk = ap.packed_masks(cu_q.cpu(), cu_k.cpu(), q.shape, k.shape)
     return q, k, v, do, cu_q, cu_k, mq, mk
 
@@ -229,8 +224,8 @@ def test_packed_forward_poisoned_padding(pack, Hq, H_kv, dtype, D, causal):
     q, k, v, _, cu_q, cu_k, mq, mk = _packed_inputs(lq, lk, Hq, H_kv, D, dtype, seed=D + Hq + causal)
     clean, bufs = _packed_fwd(q, k, v, cu_q, cu_k, 0.0, causal)
     _guards_kept(bufs)
-    o64, lse64 = ap.packed_forward(q, k, v, cu_q, cu_k, None, causal)
-    assert torch.allclose(clean[0].float().cpu(), o64.to(dtype).float(), **TOL[dtype])
+    o64, lse64 = ar.packed(q.cpu(), k.cpu(), v.cpu(), cu_q, cu_k, None, causal)
+    assert torch.allclose(clean[0].float().cpu(), o64.to(dtype).float(), **ar.TOL[dtype])
     assert torch.allclose(clean[1].double().cpu(), lse64.masked_fill(mq[..., 0], 0.0), rtol=0, atol=1e-2)
     for value in ap.VALUES:
         got, bufs = _packed_fwd(ap.poison(q, mq, value), ap.poison(k, mk, value), ap.poison(v, mk, value), cu_q, cu_k,
@@ -250,9 +245,9 @@ def test_packed_backward_poisoned_padding(pack, Hq, H_kv, dtype, D, causal):
     o, lse = (t.clone() for t in _packed_fwd(q, k, v, cu_q, cu_k, 0.0, causal)[0])
     clean, bufs = _packed_bwd(q, k, v, o, lse, do, cu_q, cu_k, causal)
     _guards_kept(bufs)
-    g64 = ap.packed_grads(q, k, v, do, cu_q, cu_k, None, causal)[:3]
+    g64 = ar.packed_grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q, cu_k, None, causal)[:3]
     qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))  # the same math in the dtype through torch autograd
-    vo.forward(qa, ka, va, cu_q.cpu(), cu_k.cpu(), None, causal)[0].backward(do)
+    ar.packed(qa, ka, va, cu_q, cu_k, None, causal, dtype)[0].backward(do)
     _grad_rule(clean, (qa.grad, ka.grad, va.grad), g64, "clean")
     mlse = mq[..., 0]
     for value in ap.VALUES:
@@ -277,7 +272,7 @@ def test_packed_exact_needles_poisoned_padding(H_kv, dtype, causal):
     pad = lambda t: torch.cat([t, torch.zeros(PAD, *t.shape[1:], dtype=t.dtype)]).cuda()  # noqa: E731
     q, k, v, do = (pad(t) for t in (q, k, v, do))
     needle = torch.cat([needle, torch.full((PAD, Hq), -1, dtype=torch.long)]).cuda()
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     mq, mk = ap.packed_masks(cu_q.cpu(), cu_k.cpu(), q.shape, k.shape)
     seen = needle >= 0
     kvh = (torch.arange(Hq, device="cuda") // (Hq // H_kv)).view(1, Hq).expand_as(needle)
@@ -303,7 +298,7 @@ def test_packed_isolation(dtype, D, causal):
     q, k, v, do, cu_q, cu_k, _, _ = _packed_inputs(lq, lk, Hq, H_kv, D, dtype, seed=D + causal)
     o, lse = (t.clone() for t in _packed_fwd(q, k, v, cu_q, cu_k, 0.0, causal)[0])
     clean = _packed_bwd(q, k, v, o, lse, do, cu_q, cu_k, causal)[0]
-    seqs = vo.seqs(cu_q.cpu(), cu_k.cpu())
+    seqs = ar.seqs(cu_q.cpu(), cu_k.cpu())
     mq = torch.zeros(q.shape, dtype=torch.bool)
     mk = torch.zeros(k.shape, dtype=torch.bool)
     for b in (1, 3):

@@ -1,5 +1,5 @@
 """GPU: packed variable-length attention with grouped-query K/V heads (ops.fa2_fwd_varlen) against the CPU reference
-(varlen_oracle.py), bit equality with the dense kernel and with repeated K/V, isolation of the sequences of a pack, clipped
+(attention_ref.py), bit equality with the dense kernel and with repeated K/V, isolation of the sequences of a pack, clipped
 stores, CUDA graph capture, and full-size properties.  Tolerances are those of test_gpu_attention.py."""
 import os
 import sys
@@ -7,22 +7,17 @@ import sys
 import pytest
 import torch
 
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # varlen_oracle.py sits next to this file
-import varlen_oracle  # noqa: E402
+sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # attention_ref.py sits next to this file
+import attention_ref as ar  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
-
-
-def _cu(lens):
-    return torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32, device="cuda")
 
 
 def _pack(lq, lk, H, H_kv, D, dtype, seed):
     torch.manual_seed(seed)
     q = torch.randn(sum(lq), H, D, device="cuda").to(dtype)
     k, v = [torch.randn(sum(lk), H_kv, D, device="cuda").to(dtype) for _ in range(2)]
-    return q, k, v, _cu(lq), _cu(lk)
+    return q, k, v, ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
 
 
 def _run(q, k, v, cq, ck, max_q, causal=False, fill=float("nan")):
@@ -49,8 +44,8 @@ def test_varlen_vs_oracle_dims(D, dtype, causal, group):
     q, k, v, cq, ck = _pack(lq, lk, H, H // group, D, dtype, seed=D + group + 7 * causal)
     o = _run(q, k, v, cq, ck, max(lq), causal)
     assert torch.isfinite(o).all()
-    want = varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=causal)
-    assert torch.allclose(o.cpu().float(), want.float(), **TOL[dtype])
+    want = ar.packed(q, k, v, cq, ck, causal=causal)[0].to(q.dtype).cpu()
+    assert torch.allclose(o.cpu().float(), want.float(), **ar.TOL[dtype])
 
 
 @pytest.mark.parametrize("lq,lk", [
@@ -65,8 +60,8 @@ def test_varlen_packs_vs_oracle(lq, lk, causal):
     q, k, v, cq, ck = _pack(lq, lk, H, H_kv, D, torch.float16, seed=sum(lq) + 3 * sum(lk) + causal)
     o = _run(q, k, v, cq, ck, max(lq), causal)
     assert torch.isfinite(o).all()
-    want = varlen_oracle.attention_varlen(q, k, v, cq, ck, causal=causal)
-    assert torch.allclose(o.cpu().float(), want.float(), **TOL[torch.float16])
+    want = ar.packed(q, k, v, cq, ck, causal=causal)[0].to(q.dtype).cpu()
+    assert torch.allclose(o.cpu().float(), want.float(), **ar.TOL[torch.float16])
     # rows that see no key are exactly 0
     c = cq.tolist()
     for b in range(len(lq)):
@@ -87,7 +82,7 @@ def test_varlen_equal_lengths_same_bits_as_dense(D, causal):
     dense = torch.empty_like(q)
     ops.fa2_fwd(q, k, v, dense, causal=causal)
     pq, pk, pv = [t.transpose(1, 2).contiguous().view(B * N, H, D) for t in (q, k, v)]
-    cu = _cu([N] * B)
+    cu = ar.cu([N] * B, "cuda")
     o = _run(pq, pk, pv, cu, cu, N, causal)
     assert torch.equal(o.view(B, N, H, D).transpose(1, 2), dense)
     # bf16 too
@@ -121,7 +116,7 @@ def test_sequences_are_isolated(causal):
     c, ckl = cq.tolist(), ck.tolist()
     for b in range(len(lq)):
         qs, ks, vs = q[c[b]:c[b + 1]].contiguous(), k[ckl[b]:ckl[b + 1]].contiguous(), v[ckl[b]:ckl[b + 1]].contiguous()
-        alone = _run(qs, ks, vs, _cu([lq[b]]), _cu([lk[b]]), lq[b], causal)
+        alone = _run(qs, ks, vs, ar.cu([lq[b]], "cuda"), ar.cu([lk[b]], "cuda"), lq[b], causal)
         assert torch.equal(alone, o[c[b]:c[b + 1]]), b
         q2, k2, v2 = q.clone(), k.clone(), v.clone()
         for t, lo, hi in ((q2, c[b], c[b + 1]), (k2, ckl[b], ckl[b + 1]), (v2, ckl[b], ckl[b + 1])):
@@ -146,10 +141,10 @@ def test_stores_stay_inside_o():
     o = buf[guard * H * D:(guard + total_q) * H * D].view(total_q, H, D)
     before, after = buf[:guard * H * D], buf[(guard + total_q) * H * D:]
     for causal in (False, True):
-        cq = _cu([600, 400])
+        cq = ar.cu([600, 400], "cuda")
         ops.fa2_fwd_varlen(q, k, v, o, cq, cq, 600, causal=causal)
-        want = varlen_oracle.attention_varlen(q, k, v, cq, cq, causal=causal)
-        assert torch.allclose(o.cpu().float(), want.float(), **TOL[torch.float16])
+        want = ar.packed(q, k, v, cq, cq, causal=causal)[0].to(q.dtype).cpu()
+        assert torch.allclose(o.cpu().float(), want.float(), **ar.TOL[torch.float16])
         # sequence 1 claims tokens [600, 1200): rows past total_q are dropped
         bad = torch.tensor([0, 600, 1200], dtype=torch.int32, device="cuda")
         ops.fa2_fwd_varlen(q, k, v, o, bad, cq, 600, causal=causal)
@@ -196,7 +191,7 @@ def test_full_size_gqa_causal_properties():
     torch.manual_seed(21)
     q = torch.randn(B * N, H, D, dtype=torch.half, device="cuda")
     k, v = [torch.randn(B * N, H_kv, D, dtype=torch.half, device="cuda") for _ in range(2)]
-    cu = _cu([N] * B)
+    cu = ar.cu([N] * B, "cuda")
     ones = torch.ones_like(v)
     assert (_run(q, k, ones, cu, cu, N, causal=True).float() - 1.0).abs().max().item() <= 1e-3
     o = _run(q, k, v, cu, cu, N, causal=True)
@@ -208,4 +203,4 @@ def test_full_size_gqa_causal_properties():
             s = (qs @ ks.t()) / D ** 0.5
             s = s.masked_fill(torch.arange(N, device="cuda").view(1, N) > rows.view(-1, 1), float("-inf"))
             want = torch.softmax(s, -1) @ vs
-            assert torch.allclose(o[b * N + rows, h].float(), want, **TOL[torch.float16]), (b, h)
+            assert torch.allclose(o[b * N + rows, h].float(), want, **ar.TOL[torch.float16]), (b, h)

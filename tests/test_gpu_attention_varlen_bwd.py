@@ -4,7 +4,7 @@
     k, key j = the sum over the group of the dO rows whose needle is j, bit for bit;
   - H_kv = H and equal lengths: the bits of the dense fa2_bwd;
   - each sequence of a packed call has the bits of that sequence passed alone;
-  - random inputs against the fp64 reference (varlen_bwd_oracle.py) by flash-attn's rule;
+  - random inputs against the fp64 reference (attention_ref.py) by flash-attn's rule;
   - rows that see no key, keys no query sees and tokens outside every sequence are +0, nothing is NaN;
   - every element is written once, guards and inputs are untouched, two calls and a graph replay give the same bits,
     a call from a fresh thread works;
@@ -19,18 +19,14 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+import attention_ref as ar  # noqa: E402
 import exact_attention as ea  # noqa: E402
-import varlen_bwd_oracle as vo  # noqa: E402
 
 from b200k import ops  # noqa: E402
 
 pytestmark = pytest.mark.gpu
 GUARD = 30
 DTYPES = [torch.float16, torch.bfloat16]
-
-
-def _cu(lens):
-    return torch.tensor([0] + list(torch.tensor(lens).cumsum(0).tolist()), dtype=torch.int32, device="cuda")
 
 
 def _out(shape, dtype):
@@ -102,7 +98,7 @@ def test_exact_needles(dtype, D, causal, lq, lk, H, H_kv):
     v = torch.randint(-8, 9, k.shape, generator=g).to(dtype)
     do = torch.randint(-8, 9, q.shape, generator=g).to(dtype)
     q, k, v, do, needle = (t.cuda() for t in (q, k, v, do, needle))
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     o, lse = _fwd(q, k, v, cu_q, cu_k, max(lq), None, causal)
     (dq, dk, dv), bufs = _bwd(q, k, v, o, lse, do, cu_q, cu_k, max(lq), max(max(lk), 1), None, causal)
     assert _pos_zero(dq) and _pos_zero(dk)
@@ -131,7 +127,7 @@ def test_equal_lengths_are_the_dense_bits(dtype, D, causal):
     dense = [torch.empty_like(q) for _ in range(3)]
     ops.fa2_bwd(q, k, v, o, lse, do, *dense, causal=causal)
     pk = lambda t: t.transpose(1, 2).reshape(B * N, H, D).contiguous()  # noqa: E731
-    cu = _cu([N] * B)
+    cu = ar.cu([N] * B, "cuda")
     got, _ = _bwd(pk(q), pk(k), pk(v), pk(o), lse.transpose(1, 2).reshape(B * N, H).contiguous(), pk(do), cu, cu, N, N,
                   None, causal)
     for a, d in zip(got, dense):
@@ -156,23 +152,23 @@ def _random(lq, lk, H, H_kv, D, dtype, seed):
 def test_random_against_fp64_and_isolation(dtype, causal, lq, lk, H, H_kv, scale):
     D = 128 if H_kv == 1 else 64
     q, k, v, do = _random(lq, lk, H, H_kv, D, dtype, sum(lq) + H)
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     o, lse = _fwd(q, k, v, cu_q, cu_k, max(lq), scale, causal)
     got, _ = _bwd(q, k, v, o, lse, do, cu_q, cu_k, max(lq), max(lk), scale, causal)
     assert all(bool(torch.isfinite(t).all()) for t in got)
-    g64 = vo.grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), scale, causal)[:3]
+    g64 = ar.packed_grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), scale, causal)[:3]
     qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))  # the same math in the dtype through torch autograd
-    vo.forward(qa, ka, va, cu_q.cpu(), cu_k.cpu(), scale, causal)[0].backward(do)
+    ar.packed(qa, ka, va, cu_q, cu_k, scale, causal, q.dtype)[0].backward(do)
     for name, a, r, w in zip(("dq", "dk", "dv"), got, (qa.grad, ka.grad, va.grad), g64):
         w = w.cuda()
         err, err_ref = (a.double() - w).abs().max().item(), (r.double() - w).abs().max().item()
         eps = ea.ulp(w.abs().max().view(1), a.dtype).item()
         assert err <= 2 * err_ref + eps, (name, err, err_ref, eps)
     # each sequence alone: the same bits
-    for q0, q1, k0, k1 in vo.seqs(cu_q.cpu(), cu_k.cpu()):
+    for q0, q1, k0, k1 in ar.seqs(cu_q.cpu(), cu_k.cpu()):
         if q1 == q0 or k1 == k0:
             continue
-        c1, c2 = _cu([q1 - q0]), _cu([k1 - k0])
+        c1, c2 = ar.cu([q1 - q0], "cuda"), ar.cu([k1 - k0], "cuda")
         sl = [t[q0:q1].contiguous() for t in (q, o, do)] + [t[k0:k1].contiguous() for t in (k, v)]
         alone, _ = _bwd(sl[0], sl[3], sl[4], sl[1], lse[q0:q1].contiguous(), sl[2], c1, c2, q1 - q0, k1 - k0, scale, causal)
         assert torch.equal(_bits(alone[0]), _bits(got[0][q0:q1]))
@@ -189,7 +185,7 @@ def test_edge_rows_bounds_determinism_graph_and_thread(dtype):
     q, k, v, do = _random(lq, lk, H, H_kv, D, dtype, 5)
     q, do = (torch.cat([t, torch.randn(50, H, D, device="cuda").to(dtype)]) for t in (q, do))
     k, v = (torch.cat([t, torch.randn(30, H_kv, D, device="cuda").to(dtype)]) for t in (k, v))
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     o, lse = _fwd(q, k, v, cu_q, cu_k, max(lq), None, True)
     inputs = [t.clone() for t in (q, k, v, o, lse, do, cu_q, cu_k)]
     first, bufs = _bwd(q, k, v, o, lse, do, cu_q, cu_k, max(lq), max(lk), None, True)
@@ -204,7 +200,7 @@ def test_edge_rows_bounds_determinism_graph_and_thread(dtype):
     assert _pos_zero(dq[:110]) and not _pos_zero(dq[110:200])  # rows r < Lq - Lk = 110 see no key
     assert _pos_zero(dq[200:270]) and _pos_zero(dk[90:130]) and _pos_zero(dv[90:130])  # Lk = 0, Lq = 0
     assert _pos_zero(dq[-50:]) and _pos_zero(dk[-30:]) and _pos_zero(dv[-30:])  # outside every sequence
-    g64 = vo.grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), None, True)[:3]
+    g64 = ar.packed_grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), None, True)[:3]
     for a, w in zip(first, g64):
         assert (a.double().cpu() - w).abs().max().item() < 0.1
     # graph replay
@@ -240,7 +236,7 @@ def test_edge_rows_bounds_determinism_graph_and_thread(dtype):
 def test_attention_varlen_autograd(dtype, causal):
     lq, lk, H, H_kv, D = (300, 77, 513), (300, 150, 513), 8, 2, 64
     q, k, v, do = _random(lq, lk, H, H_kv, D, dtype, 3 + causal)
-    cu_q, cu_k = _cu(lq), _cu(lk)
+    cu_q, cu_k = ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
     qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))
     out = ops.attention_varlen(qa, ka, va, cu_q, cu_k, max(lq), max(lk), causal=causal)
     out.backward(do.transpose(0, 1).contiguous().transpose(0, 1))  # a non-contiguous upstream gradient
@@ -248,12 +244,12 @@ def test_attention_varlen_autograd(dtype, causal):
     want, _ = _bwd(q, k, v, o, lse, do, cu_q, cu_k, max(lq), max(lk), None, causal)
     for a, b in zip((qa.grad, ka.grad, va.grad), want):
         assert torch.equal(_bits(a), _bits(b))
-    g64 = vo.grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), None, causal)[:3]
+    g64 = ar.packed_grads(q.cpu(), k.cpu(), v.cpu(), do.cpu(), cu_q.cpu(), cu_k.cpu(), None, causal)[:3]
     ref = [torch.zeros_like(t) for t in (q, k, v)]
-    for q0, q1, k0, k1 in vo.seqs(cu_q.cpu(), cu_k.cpu()):
+    for q0, q1, k0, k1 in ar.seqs(cu_q.cpu(), cu_k.cpu()):
         qs, ks, vs = (t[a:b].transpose(0, 1).unsqueeze(0).clone().requires_grad_() for t, a, b in
                       ((q, q0, q1), (k, k0, k1), (v, k0, k1)))
-        mask = vo.visible(q1 - q0, k1 - k0, causal, "cuda")
+        mask = ar.visible(q1 - q0, k1 - k0, k1 - k0 - (q1 - q0) if causal else None, "cuda")
         torch.nn.functional.scaled_dot_product_attention(qs, ks, vs, attn_mask=mask, enable_gqa=True).backward(
             do[q0:q1].transpose(0, 1).unsqueeze(0))
         for r, t, a, b in zip(ref, (qs, ks, vs), (q0, k0, k0), (q1, k1, k1)):

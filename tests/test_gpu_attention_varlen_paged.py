@@ -9,10 +9,10 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))  # the oracles sit next to this file
+import attention_ref as ar  # noqa: E402
 import varlen_paged_oracle as vpo  # noqa: E402
 
 pytestmark = pytest.mark.gpu
-TOL = {torch.float16: dict(rtol=1e-2, atol=1e-3), torch.bfloat16: dict(rtol=2e-2, atol=4e-3)}
 LQ = [77, 0, 1, 129, 300, 128, 5]
 LK = [300, 5, 0, 128, 129, 1000, 700]   # Lk < Lq, Lk = 0, an empty query sequence, Lk not a multiple of any page
 
@@ -22,15 +22,11 @@ def _ops():
     return ops
 
 
-def _cu(lens):
-    return torch.tensor([0] + torch.tensor(lens).cumsum(0).tolist(), dtype=torch.int32, device="cuda")
-
-
 def _pack(lq, lk, H, H_kv, D, dtype, seed, extra_q=0):
     g = torch.Generator(device="cuda").manual_seed(seed)
     q = torch.randn(sum(lq) + extra_q, H, D, device="cuda", generator=g).to(dtype)
     k, v = [torch.randn(sum(lk), H_kv, D, device="cuda", generator=g).to(dtype) for _ in range(2)]
-    return q, k, v, _cu(lq), _cu(lk)
+    return q, k, v, ar.cu(lq, "cuda"), ar.cu(lk, "cuda")
 
 
 def _paged(q, kc, vc, cq, ck, table, max_q, causal, fill=float("nan")):
@@ -69,9 +65,8 @@ def test_same_bits_as_gathered(page_size, D, dtype, causal):
         assert torch.isfinite(got[0]).all(), group
         _same_bits(got, _gathered(q, kc, vc, cq, ck, table, max(LQ), causal))
         if group == 8 and D == 64:
-            from varlen_oracle import attention_varlen
-            want = attention_varlen(q, k, v, cq, ck, causal=causal)
-            assert torch.allclose(got[0].cpu().float(), want.float(), **TOL[dtype])
+            want = ar.packed(q, k, v, cq, ck, causal=causal)[0].to(q.dtype).cpu()
+            assert torch.allclose(got[0].cpu().float(), want.float(), **ar.TOL[dtype])
 
 
 @pytest.mark.parametrize("poison", [float("nan"), float("inf"), float("-inf")])
@@ -113,7 +108,7 @@ def test_table_shapes(page_size, causal):
         assert (got[0][c[2]:c[2] + 200] == 0).all() and torch.isneginf(got[1][c[2]:c[2] + 200]).all()
     assert (got[0][c[4]:c[5]] == 0).all() and torch.isneginf(got[1][c[4]:c[5]]).all()     # Lk = 0
     # the clamped sequence equals its first 1024 keys given explicitly
-    cut = _cu([lq[5]]), _cu([1024])
+    cut = ar.cu([lq[5]], "cuda"), ar.cu([1024], "cuda")
     o2 = torch.empty_like(q[c[5]:c[6]])
     ops.fa2_fwd_varlen(q[c[5]:c[6]], kc, vc, o2, cut[0], cut[1], lq[5], causal=causal, block_table=table[5:6].clone())
     assert torch.equal(o2.view(torch.int16), got[0][c[5]:c[6]].view(torch.int16))
@@ -170,9 +165,9 @@ def test_agrees_with_decode(B, Lq, H, H_kv, dtype, causal):
     o = torch.empty_like(q).view(B * Lq, H, D)
     table = torch.arange(B, dtype=torch.int32, device="cuda").view(B, 1)
     ck = torch.cat([torch.zeros(1, dtype=torch.int32, device="cuda"), lens.cumsum(0).int()])
-    ops.fa2_fwd_varlen(q.view(B * Lq, H, D), kc, vc, o, _cu([Lq] * B), ck, Lq, causal=causal, block_table=table)
+    ops.fa2_fwd_varlen(q.view(B * Lq, H, D), kc, vc, o, ar.cu([Lq] * B, "cuda"), ck, Lq, causal=causal, block_table=table)
     if ops.fa2_fwd_kvcache_workspace_bytes(B, Lq, H, H_kv, D, S) > 0:   # decode splits the keys across CTAs
-        assert torch.allclose(o.view_as(q).float(), o_dec.float(), **TOL[dtype])
+        assert torch.allclose(o.view_as(q).float(), o_dec.float(), **ar.TOL[dtype])
     else:
         assert torch.equal(o.view_as(q).view(torch.int16), o_dec.view(torch.int16))
 
@@ -193,8 +188,8 @@ def test_cuda_graph_replays_new_lengths_and_tables():
     with torch.cuda.graph(graph):
         ops.fa2_fwd_varlen(q, kc, vc, o, cq, ck, 256, causal=True, lse=lse, block_table=table)
     for seed, (nq, nk) in enumerate([([50, 80, 150, 51], [1000, 80, 64, 1]), ([0, 256, 74, 1], [5, 1024, 700, 0])]):
-        cq.copy_(_cu(nq))
-        ck.copy_(_cu(nk))
+        cq.copy_(ar.cu(nq, "cuda"))
+        ck.copy_(ar.cu(nk, "cuda"))
         g = torch.Generator().manual_seed(seed)
         table.copy_(torch.randperm(kc.size(0), generator=g)[:table.numel()].view_as(table).int())
         o.fill_(float("nan"))

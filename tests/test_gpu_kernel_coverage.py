@@ -10,7 +10,7 @@ be exactly kernel_inventory.launched(case), then checks what the call wrote.
     unsplit rows within the fp64 rule.
   - Append: the cache bytes are the reference rotation (and quantisation) of the new rows, O is the decode call on
     the updated cache.
-  - Backward: attn_bwd_oracle in fp64 by the same rule.  GEMM: integer operands, so the answer is exact.  Bandwidth
+  - Backward: attention_ref in fp64 by the same rule.  GEMM: integer operands, so the answer is exact.  Bandwidth
     kernels: the CPU oracle (oracle/oracle.py), exact where the operation is."""
 import math
 import os
@@ -20,7 +20,7 @@ import pytest
 import torch
 
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-import attn_bwd_oracle as bo  # noqa: E402
+import attention_ref as ar  # noqa: E402
 import exact_attention as ea  # noqa: E402
 import kernel_inventory as ki  # noqa: E402
 import kvcache_append_oracle as kao  # noqa: E402
@@ -104,39 +104,6 @@ def _same_bits(a, b, what):
 
 
 # ------------------------------------------------------------------------------------------------ attention references
-def _attend(q, k, v, scale, causal, cd):
-    """One sequence: q [Lq, H, D], k, v [Lk, H_kv, D] -> (o [Lq, H, D], lse [Lq, H]) computed in dtype cd on the device.
-    Key j is visible to token t iff j <= t + Lk - Lq when causal; a row with no visible key is 0 with lse -inf."""
-    Lq, H, D = q.shape
-    Lk, H_kv = k.shape[0], k.shape[1]
-    qh = q.to(cd).transpose(0, 1)
-    kh = k.to(cd).transpose(0, 1).repeat_interleave(H // H_kv, 0)
-    vh = v.to(cd).transpose(0, 1).repeat_interleave(H // H_kv, 0)
-    s = (qh @ kh.transpose(1, 2)) * scale
-    if causal:
-        keep = torch.arange(Lk, device=q.device).view(1, Lk) <= torch.arange(Lq, device=q.device).view(Lq, 1) + Lk - Lq
-        s = s.masked_fill(~keep, float("-inf"))
-    lse = torch.logsumexp(s.double(), -1)
-    p = torch.softmax(s, -1).nan_to_num(0.0)
-    return (p @ vh).transpose(0, 1), lse.transpose(0, 1)
-
-
-def _packed_refs(q, k, v, cu_q, cu_k, scale, causal):
-    """(o64, lse64, o in q's dtype) over packed sequences: q [total_q, H, D], k / v [total_k, H_kv, D]."""
-    cq, ck = cu_q.tolist(), cu_k.tolist()
-    o64 = torch.zeros(q.shape, dtype=torch.float64, device="cuda")
-    od = torch.zeros_like(q)
-    l64 = torch.full(q.shape[:2], float("-inf"), dtype=torch.float64, device="cuda")
-    for b in range(len(cq) - 1):
-        qs, ks, vs = q[cq[b]:cq[b + 1]], k[ck[b]:ck[b + 1]], v[ck[b]:ck[b + 1]]
-        if qs.shape[0] == 0 or ks.shape[0] == 0:
-            continue
-        o, lse = _attend(qs, ks, vs, scale, causal, torch.float64)
-        o64[cq[b]:cq[b + 1]], l64[cq[b]:cq[b + 1]] = o, lse
-        od[cq[b]:cq[b + 1]] = _attend(qs, ks, vs, scale, causal, q.dtype)[0]
-    return o64, l64, od
-
-
 def _rule(got, ref, o64, what):
     """max|got - o64| <= 2 max|ref - o64| + one ulp of the dtype at max|o64| (ref: the same math in got's dtype)."""
     assert bool(torch.isfinite(got).all()), "%s: non-finite output" % what
@@ -175,13 +142,12 @@ def _dense(toks, dt, D, lse):
     _guards(ob, *([lb] if lse else []))
     if not lse:
         assert torch.isnan(l).all()
-    sc = 1 / math.sqrt(D)
+    o64, l64 = ar.dense(q, k, v, causal=causal)
+    od = ar.dense(q, k, v, causal=causal, dtype=dt)[0]
     for b in range(B):
-        o64, l64 = _attend(q[b].transpose(0, 1), k[b].transpose(0, 1), v[b].transpose(0, 1), sc, causal, torch.float64)
-        od, _ = _attend(q[b].transpose(0, 1), k[b].transpose(0, 1), v[b].transpose(0, 1), sc, causal, dt)
-        _rule(o[b].transpose(0, 1), od, o64, "dense O")
+        _rule(o[b], od[b], o64[b], "dense O")
         if lse:
-            _lse_close(l[b].transpose(0, 1), l64, "dense lse")
+            _lse_close(l[b], l64[b], "dense lse")
     return r.names
 
 
@@ -195,8 +161,8 @@ def _ffpa(D):
         ops.ffpa_fwd(q, k, v, o)
     _guards(ob)
     for h in range(H):
-        args = (q[0, h][:, None], k[0, h][:, None], v[0, h][:, None], 1 / math.sqrt(D), False)
-        _rule(o[0, h][:, None], _attend(*args, torch.float16)[0], _attend(*args, torch.float64)[0], "ffpa O")
+        args = (q[0, h][:, None], k[0, h][:, None], v[0, h][:, None], 1 / math.sqrt(D))
+        _rule(o[0, h][:, None], ar.sequence(*args, dtype=torch.float16)[0], ar.sequence(*args)[0], "ffpa O")
     return r.names
 
 
@@ -213,8 +179,8 @@ def _packed_inputs(dt, D, H, H_kv, seed):
 
 
 def _check_packed(o, l, lse, q, k, v, cu_q, cu_k, causal, what):
-    o64, l64, od = _packed_refs(q, k, v, cu_q, cu_k, 1 / math.sqrt(q.shape[-1]), causal)
-    _rule(o, od, o64, what + " O")
+    o64, l64 = ar.packed(q, k, v, cu_q, cu_k, causal=causal)
+    _rule(o, ar.packed(q, k, v, cu_q, cu_k, causal=causal, dtype=q.dtype)[0], o64, what + " O")
     if lse:
         _lse_close(l, l64, what + " lse")
 
@@ -312,8 +278,9 @@ def _decode(toks, dt, D, lse, fmt):
         _same_bits(o.view(B * Lq, H, D), ov, "unsplit decode vs fa2_fwd_varlen: O")
     if lse and fmt:
         _same_bits(l, l2, "fp8 decode vs 16-bit decode: lse")
-    o64, l64, od = _packed_refs(q.view(B * Lq, H, D), kg, vg, cu_q, cu_k, 1 / math.sqrt(D), causal)
-    _rule(o.view(B * Lq, H, D), od, o64, "decode O")
+    o64, l64 = ar.packed(q.view(B * Lq, H, D), kg, vg, cu_q, cu_k, causal=causal)
+    _rule(o.view(B * Lq, H, D), ar.packed(q.view(B * Lq, H, D), kg, vg, cu_q, cu_k, causal=causal, dtype=dt)[0], o64,
+          "decode O")
     if lse:
         _lse_close(l.view(B * Lq, H), l64, "decode lse")
     return r.names
@@ -385,8 +352,9 @@ def _append(toks, dt, fmt):
     vd = fo.dequantize(vc.cpu(), dt, vs) if fmt else vc.cpu()
     kg, vg, cu_k = (t.cuda() for t in kvcache_oracle.gather(kd, vd, new_lens.cpu(), table.cpu()))
     cu_q = torch.arange(B + 1, dtype=torch.int32, device="cuda") * Lq
-    o64, _, od = _packed_refs(q_rot.view(B * Lq, H, D), kg, vg, cu_q, cu_k, 1 / math.sqrt(D), True)
-    _rule(o.view(B * Lq, H, D), od, o64, "append O")
+    q_rot = q_rot.view(B * Lq, H, D)
+    _rule(o.view(B * Lq, H, D), ar.packed(q_rot, kg, vg, cu_q, cu_k, causal=True, dtype=dt)[0],
+          ar.packed(q_rot, kg, vg, cu_q, cu_k, causal=True)[0], "append O")
     return r.names
 
 
@@ -429,9 +397,9 @@ def _bwd(toks, dt, D):
         with _Record() as r:
             ops.fa2_bwd(q, k, v, o, lse, do, *(t for t, _ in outs), causal=True, seqlens_k=sl)
         _guards(*(b for _, b in outs))
-        g64 = bo.grads(q, k, v, do, None, True, sl)[:3]
+        g64 = ar.dense_grads(q, k, v, do, None, True, sl)[:3]
         qa, ka, va = (t.clone().requires_grad_() for t in (q, k, v))
-        bo.forward(qa, ka, va, None, True, sl)[0].backward(do)
+        ar.dense(qa, ka, va, None, True, sl, dt)[0].backward(do)
         ref = (qa.grad, ka.grad, va.grad)
     else:
         H, H_kv = 4, 2

@@ -1,9 +1,7 @@
 """Paged caches for packed attention (ops.fa2_fwd_varlen with block_table), used by test_attention_varlen_paged_cpu.py and
-test_gpu_attention_varlen_paged.py: packed K/V scattered into the pages of a shuffled block table, the gather back through
-the table, and a per-sequence fp64 reference that reads keys straight from the pages."""
+test_gpu_attention_varlen_paged.py: packed K/V scattered into the pages of a shuffled block table, and the gather back
+through the table that attention_ref.paged attends over."""
 from __future__ import annotations
-
-import math
 
 import torch
 
@@ -47,31 +45,3 @@ def gather(k_cache, v_cache, cu_seqlens_k, block_table):
     """Packed K, V (on the CPU) and int32 cu_seqlens_k of the keys the paged call reads: the clamped lengths."""
     cap = block_table.size(1) * k_cache.size(1)
     return kvcache_oracle.gather(k_cache, v_cache, lengths(cu_seqlens_k, cap), block_table)
-
-
-def attention_pages(q, k_cache, v_cache, cu_seqlens_q, cu_seqlens_k, block_table, scale=None, causal=False):
-    """(O [total_q, H, D] fp64, lse [total_q, H] fp64) on the CPU, one sequence at a time, each key read from its page.
-    Rows that see no key are 0 with lse -inf; tokens outside every sequence are 0 and -inf."""
-    total_q, H, D = q.shape
-    ps, H_kv = k_cache.size(1), k_cache.size(2)
-    scale = 1.0 / math.sqrt(D) if scale is None else scale
-    cq = torch.as_tensor(cu_seqlens_q).cpu().tolist()
-    table = torch.as_tensor(block_table).cpu().long()
-    lens = lengths(cu_seqlens_k, table.size(1) * ps)
-    kc, vc, qd = k_cache.cpu().double(), v_cache.cpu().double(), q.cpu().double()
-    out = torch.zeros(total_q, H, D, dtype=torch.float64)
-    lse = torch.full((total_q, H), float("-inf"), dtype=torch.float64)
-    for b, Lk in enumerate(lens):
-        Lq = cq[b + 1] - cq[b]
-        for h in range(H):
-            hk = h // (H // H_kv)
-            keys = torch.stack([kc[table[b, j // ps], j % ps, hk] for j in range(Lk)]) if Lk else torch.zeros(0, D)
-            vals = torch.stack([vc[table[b, j // ps], j % ps, hk] for j in range(Lk)]) if Lk else torch.zeros(0, D)
-            for r in range(Lq):
-                n = min(Lk, r + Lk - Lq + 1) if causal else Lk
-                if n <= 0:
-                    continue
-                s = (keys[:n] @ qd[cq[b] + r, h]) * scale
-                lse[cq[b] + r, h] = torch.logsumexp(s, 0)
-                out[cq[b] + r, h] = torch.softmax(s, 0) @ vals[:n]
-    return out, lse
